@@ -1,4 +1,4 @@
-"""bayes.js_b200 -- B200-native many-chain AMWG sampler behind the bayes.js API.
+"""bayes.js_b200 -- H100-native many-chain AMWG sampler behind the bayes.js API.
 
     from bayes_js_b200 import mcmc, ld          (see __graft_entry__.load_package for the import shim:
                                                  the directory name `bayes.js_b200` is not a Python identifier)

@@ -3,7 +3,7 @@
 // The ABI hands log_post over as bytecode (include/amwg.h). For the interpreter kernels that bytecode is data; here it is
 // SOURCE: the programs of a model eligible for pre-evaluated plate statistics (amwg_model.stat_prog) are decoded, turned into
 // straight-line CUDA C++ (one function per class of structurally identical component programs, indices that differ between the
-// members of a class read from small tables), joined with the kernel skeleton amwg_jit_kernel.cuh and compiled for sm_100a by
+// members of a class read from small tables), joined with the kernel skeleton amwg_jit_kernel.cuh and compiled for sm_90a by
 // NVRTC (dlopen'ed: the library loads without it; a model that cannot be specialised runs on the interpreter kernels -- there
 // is still no CPU path). The cubin is loaded through the runtime's library API (cudaLibraryLoadData), cached per process by
 // source hash. What the generated step computes differs from the interpreter's in one respect (DESIGN.md section 2): it forms
@@ -529,8 +529,8 @@ static std::string choose_shape(Plan& pl, unsigned off, size_t per_thread, unsig
     double eff; int r_need;
     if (ctas <= cap) { const double per_sm = std::ceil(ctas / sm_count); eff = ((double)n_chains / sm_count) / (per_sm * t); r_need = (int)per_sm; }
     else { eff = ctas / (std::ceil(ctas / cap) * cap) * ((double)n_chains / (ctas * t)); r_need = r_max; }
-    // 128-thread CTAs are the default; another size has to fill the SMs a good deal more evenly to win (config 4 at 2^16 chains:
-    // 224 x 2 CTAs/SM is 14 % better balanced than 128 x 4 and measured 6 % SLOWER -- more, smaller CTAs overlap their phases)
+    // 128-thread CTAs are the default; another size has to fill the SMs a good deal more evenly (15 % in `eff`) to be chosen,
+    // because more, smaller CTAs overlap the CTA-wide phases of a sweep better than a few larger ones balanced more evenly
     if (eff > best_eff + (best_t == 0 ? 0.0 : 0.15)) { best_eff = eff; best_t = t; best_r = r_need; best_ws = ws_smem; }
     if (forced_t) break;
   }
@@ -802,7 +802,7 @@ static std::string build_source(const amwg_model* md, const std::vector<double>&
       << "#define JSTREAM " << (pl.stream_col >= 0 ? 1 : 0) << "\n#define JS_COL " << std::max(pl.stream_col, 0) << "\n#define JS_BEGIN " << s_begin << "\n#define JS_TOTAL " << s_total << "\n"
       << "#define JN_SSTAT " << s_entries.size() << "\n#define JRING_OFF " << pl.ring_off << "u\n#define JRING_STAGES " << pl.ring_stages << "\n#define JRING_TILE " << pl.ring_tile << "\n"
       << "#define JNORM_C0 " << lit(norm_c0) << "\n#define AMWG_REAL 0\n#define AMWG_INT 1\n#define AMWG_BINARY 2\n";
-  // accumulators of the plate loop: four (eight measured 5 % slower on config 4 at 3.5 warps per scheduler, profiles/r02_config4_tuning.txt)
+  // accumulators of the plate loop: four by default (AMWG_JIT_NACC=8 selects eight, for A/B runs)
   int nacc = 4;
   if (const char* e = getenv("AMWG_JIT_NACC")) { int v = atoi(e); if (v == 4 || v == 8) nacc = v; }
   pre << "#define AMWG_NACC " << nacc << "\n";
@@ -1003,7 +1003,9 @@ static std::string main_source(const Source& s) {
          (s.full ? "amwg_jit_full_kernel.cuh" : "amwg_jit_kernel.cuh") + "\"\n";
 }
 
-// Compile to a cubin for sm_100a. Returns "" on success.
+static const char* const kJitArch = "--gpu-architecture=sm_90a";
+
+// Compile to a cubin for sm_90a. Returns "" on success.
 static std::string compile(const Source& s, std::vector<char>& cubin, std::string& log) {
   Nvrtc* nv = nvrtc();
   if (!nv->error.empty()) return nv->error;
@@ -1013,7 +1015,7 @@ static std::string compile(const Source& s, std::vector<char>& cubin, std::strin
   nvrtcProgram_t prog = nullptr;
   nvrtcResult_t rc = nv->CreateProgram(&prog, main_src.c_str(), "amwg_jit_model.cu", 6, headers, names);
   if (rc != 0) return std::string("nvrtcCreateProgram: ") + nv->GetErrorString(rc);
-  const char* opts[] = {"--gpu-architecture=sm_100a", "--std=c++17", "--fmad=false", "-lineinfo", "-DAMWG_JIT=1", "--ptxas-options=-v"};
+  const char* opts[] = {kJitArch, "--std=c++17", "--fmad=false", "-lineinfo", "-DAMWG_JIT=1", "--ptxas-options=-v"};
   rc = nv->CompileProgram(prog, 6, opts);
   size_t ln = 0;
   if (nv->GetProgramLogSize(prog, &ln) == 0 && ln > 1) { log.resize(ln); nv->GetProgramLog(prog, &log[0]); }
@@ -1040,16 +1042,17 @@ struct Loaded { cudaLibrary_t lib = nullptr; cudaKernel_t kernel = nullptr; };
 static std::mutex g_cache_mu;
 static std::map<std::pair<int, unsigned long long>, Loaded> g_cache;      // (device, source hash) -> loaded kernel
 
-// disk cache of cubins (compile once per source): $AMWG_JIT_CACHE or <library dir>/jit_cache
+// disk cache of cubins (compile once per source): $AMWG_JIT_CACHE, else a directory of this user's under $TMPDIR (or /tmp), so
+// that an installation the user cannot write to still caches. A directory that another user owns or may write to is not used:
+// its cubins would run in this process.
 static std::string cache_dir() {
   if (const char* e = getenv("AMWG_JIT_CACHE")) return e;
-  Dl_info info;
-  if (dladdr((void*)&fnv1a, &info) && info.dli_fname) {
-    std::string p(info.dli_fname);
-    size_t k = p.find_last_of('/');
-    return (k == std::string::npos ? std::string(".") : p.substr(0, k)) + "/jit_cache";
-  }
-  return "";
+  const char* t = getenv("TMPDIR");
+  const std::string dir = std::string(t && *t ? t : "/tmp") + "/amwg_jit_cache-" + std::to_string((long long)getuid());
+  mkdir(dir.c_str(), 0700);
+  struct stat st;
+  if (lstat(dir.c_str(), &st) != 0 || !S_ISDIR(st.st_mode) || st.st_uid != getuid() || (st.st_mode & 022)) return "";
+  return dir;
 }
 
 static bool read_file(const std::string& path, std::vector<char>& out) {
@@ -1074,7 +1077,7 @@ static void write_file(const std::string& dir, const std::string& path, const st
 }
 
 static std::string get_cubin(const Source& s, std::vector<char>& cubin, std::string& log, bool* from_cache) {
-  const unsigned long long h = fnv1a(s.generated, fnv1a(s.prelude, fnv1a(kSrcJitKernel, fnv1a(kSrcJitFullKernel, fnv1a(kSrcTma, fnv1a(kSrcMath, fnv1a(kSrcLd)))))));
+  const unsigned long long h = fnv1a(s.generated, fnv1a(s.prelude, fnv1a(kSrcJitKernel, fnv1a(kSrcJitFullKernel, fnv1a(kSrcTma, fnv1a(kSrcMath, fnv1a(kSrcLd, fnv1a(kJitArch))))))));
   char name[64];
   snprintf(name, sizeof name, "/amwg_%016llx.cubin", h);
   const std::string dir = cache_dir(), path = dir + name;

@@ -1,4 +1,4 @@
-// amwg_jit_kernel.cuh -- the sweep kernel that amwg_jit.cuh specialises per model and compiles with NVRTC for sm_100a.
+// amwg_jit_kernel.cuh -- the sweep kernel that amwg_jit.cuh specialises per model and compiles with NVRTC for sm_90a.
 //
 // Reference path (all under /root/reference/): Sampler.sample / burn / step (mcmc.js:985-1039), AmwgStepper.step (:886-892),
 // MultidimComponentMetropolisStepper.step (:685-688), OnedimMetropolisStepper.step (:517-553), rnorm / shuffle_array (:43-54,

@@ -1,4 +1,4 @@
-// amwg_kernels.cu -- libamwg_b200.so: the AMWG hot path of bayes.js as sm_100a CUDA + the C ABI of include/amwg.h.
+// amwg_kernels.cu -- libamwg_b200.so: the AMWG hot path of bayes.js as sm_90a CUDA + the C ABI of include/amwg.h.
 //
 // Reference path replaced (all under /root/reference/):
 //   Sampler.sample / burn / step                     mcmc.js:985-1039
@@ -354,9 +354,8 @@ __device__ __forceinline__ void pois_rows(unsigned xsa, int rows, const double (
 // ---- the same rows on the fp64 tensor core (K = 8, a full warp) ------------------------------------------------------------------
 // eta[row, chain] = sum_k X[row, k] beta[chain, k] is a GEMM: DMMA.8x8x4 (mma.sync m8n8k4 f64) forms it for 8 rows x 8 chains per
 // instruction, so a warp's 32 chains take 8 DMMAs per 8 rows instead of 64 DFMAs per thread -- and, what matters more, ONE
-// conflict-free LDS.128 per 8 rows instead of 32 broadcast LDS.128 (measured on this part, scripts/microbench/fp64_pipes.cu: a
-// broadcast LDS.128 costs 2.5 cycles of the SM's shared-memory pipe and overlaps poorly with the fp64 pipe; the per-thread form
-// spends as long on its loads as on its arithmetic. DMMA runs on the same fp64 pipe as DFMA at the same flop rate, 16 cycles each).
+// conflict-free LDS.128 per 8 rows instead of 32 broadcast LDS.128 (broadcast loads occupy the SM's shared-memory pipe and
+// compete with the fp64 instructions for issue; scripts/microbench/fp64_pipes.cu measures DFMA, DMMA and LDS.128 rates).
 // Fragment layout (PTX ISA, m8n8k4 .f64): lane = 4 * g + j. A: row g, one k per step; B: column (chain) g of the tile, one k per
 // step; C: row g, chains 2j and 2j + 1 of the tile. Lane j takes k = 2j (step 0) and k = 2j + 1 (step 1), adjacent in the row.
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
@@ -1877,9 +1876,10 @@ extern "C" int amwg_jit_status(const amwg_sampler* s, char* note, int64_t cap) {
   return s->jit_kernel ? 1 : 0;
 }
 
-// Generate and compile the specialised sweep of `model` without a GPU (NVRTC targets sm_100a from any host): 0 = compiled,
+// Generate and compile the specialised sweep of `model` without a GPU (NVRTC targets sm_90a from any host): 0 = compiled,
 // 1 = the model is not eligible (reason in `log`), -1 = generation or compilation failed (message in `log`). `src`, when given,
-// receives the generated source. Constants that the device would fold at create are left as they are in the model.
+// receives the generated source. Constants that the device would fold at create are left as they are in the model; the launch
+// shape is planned for the 132 SMs of an H100 SXM.
 extern "C" int amwg_jit_compile_check(const amwg_model* md, uint64_t n_chains, char* log, int64_t log_cap, char* src_out, int64_t src_cap) {
   auto put = [](char* dst, int64_t cap, const std::string& s) { if (dst && cap > 0) snprintf(dst, (size_t)cap, "%s", s.c_str()); };
   if (validate_model(md)) { put(log, log_cap, g_last_error); return -1; }
@@ -1887,8 +1887,8 @@ extern "C" int amwg_jit_compile_check(const amwg_model* md, uint64_t n_chains, c
   if (consts.empty()) consts.push_back(0.0);
   jit::Source src;
   const bool stat_model = md->comp_prog && md->n_terms > 0 && md->stat_prog >= 0;
-  std::string why = stat_model ? jit::build_source(md, consts, n_chains ? n_chains : 1, 148, -0.9189385332046727, src)
-                               : jit::build_source_full(md, consts, n_chains ? n_chains : 1, 148, -0.9189385332046727, src);
+  std::string why = stat_model ? jit::build_source(md, consts, n_chains ? n_chains : 1, 132, -0.9189385332046727, src)
+                               : jit::build_source_full(md, consts, n_chains ? n_chains : 1, 132, -0.9189385332046727, src);
   if (!why.empty()) { put(log, log_cap, why); return 1; }
   put(src_out, src_cap, src.prelude + src.generated);
   std::vector<char> cubin;

@@ -2,7 +2,7 @@
 //
 // MEASURED_PEAKS.json (driver-written) holds HBM and bf16 tensor peaks only; the AMWG hot path is bound by the fp64 pipe
 // (DADD + DFMA per data point, DESIGN.md section 4), so bench.py measures that roof itself, in the same process and at the
-// same clocks as the timed region: a grid of 148 x 8 CTAs x 256 threads, every thread running 8 independent DFMA chains
+// same clocks as the timed region: a grid of (SM count) x 8 CTAs x 256 threads, every thread running 8 independent DFMA chains
 // (enough ILP and resident warps to keep the pipe issuing back to back), timed with CUDA events on the launching stream.
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once

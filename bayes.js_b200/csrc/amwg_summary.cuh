@@ -16,6 +16,9 @@
 namespace summary {
 
 constexpr int kMaxPrefixes = 32;      // distinct prefixes per entry and pass (order statistics being selected at once)
+// CTAs per entry of the chain-wise kernels (fewer when there are fewer 256-chain groups): a fixed number, not the device's SM
+// count, because it sets the merge order of the moments and so their last bits; ~9 CTAs per SM of an H100.
+constexpr long long kChainCtas = 1184;
 
 __device__ __forceinline__ unsigned long long ordered_key(double x) {
   unsigned long long u = (unsigned long long)__double_as_longlong(x);
@@ -152,7 +155,7 @@ extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64
   if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_moments: empty sample block");
   if (!dev_samples || !host_stats) return fail("amwg_summary_moments: null pointer");
   CUDA_TRY(cudaSetDevice(device));
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, 148 * 8);     // depends on `chains` only: a fixed merge order
+  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);     // depends on `chains` only: a fixed merge order
   // scratch that lives as long as the process (per device, grown on demand): no cudaMalloc / cudaFree on the path of a call
   struct Scratch { void* p = nullptr; size_t bytes = 0; };
   static Scratch scratch[64];
@@ -191,7 +194,7 @@ extern "C" int amwg_summary_digit_hist(int device, const double* dev_samples, in
   if (!dev_samples || !dev_prefix || !dev_counts) return fail("amwg_summary_digit_hist: null pointer");
   CUDA_TRY(cudaSetDevice(device));
   // a CTA's shared bins are 32-bit: bound the values one CTA sees by 2^32 (rows < 2^32 and the grid below keeps chains per CTA small)
-  int64_t bx = std::min<int64_t>((chains + 255) / 256, 148 * 8);
+  int64_t bx = std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
   while (bx < (chains + 255) / 256 && ((chains + bx - 1) / bx) * rows >= ((int64_t)1 << 32)) bx *= 2;
   summary::amwg_digit_hist_kernel<<<dim3((unsigned)bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, pass,
                                                                                   reinterpret_cast<const unsigned long long*>(dev_prefix), n_prefix,

@@ -4,7 +4,7 @@
     sampler.burn(1000); samples = sampler.sample(5000)              # mcmc.js:1035-1039, 1005-1030
 
 Same names, argument meaning and error strings as the reference; the stepping itself happens in
-libamwg_b200.so (CUDA, sm_100a) for ``options["chains"]`` independent chains at once.  The host
+libamwg_b200.so (CUDA, sm_90a) for ``options["chains"]`` independent chains at once.  The host
 language is Python because no JavaScript engine exists in this image; INTEGRATION.md shows the N-API
 binding a Node host would put under the same `mcmc` / `ld` module names.
 
@@ -316,7 +316,7 @@ class Sampler:
 
 
 class AmwgSampler(Sampler):
-    """mcmc.js:1090-1099 -- the AMWG sampler, `options["chains"]` chains at once on one B200."""
+    """mcmc.js:1090-1099 -- the AMWG sampler, `options["chains"]` chains at once on one H100."""
 
     # -- construction ---------------------------------------------------------------------------
     def _resolve_options(self, params, options):

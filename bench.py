@@ -29,8 +29,9 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 import __graft_entry__ as graft  # noqa: E402
 
-METRIC = "posterior draws/sec (chains x iters) Normal(mu,sigma) N=1024 at 1/2/4/8 B200"
-FP64_NOMINAL_TFLOPS = 37.0       # B200 non-tensor fp64 (HGX B200 datasheet: 296 TF / 8 GPUs); only used when the measurement fails
+METRIC = "posterior draws/sec (chains x iters) Normal(mu,sigma) N=1024 at 1/2/4/8 H100"
+FP64_NOMINAL_TFLOPS = 34.0       # H100 SXM non-tensor fp64 (NVIDIA data sheet, 700 W); only used when the measurement fails
+DUMP_BYTES = 32 << 20            # --dump-outputs: at most this many bytes of draws
 PARAMS = {"mu": {"type": "real"}, "sigma": {"type": "real", "lower": 0}}
 N_DATA = 1024
 CHAINS_PER_GPU = 1 << 20
@@ -201,31 +202,39 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "nominal (H100 SXM data sheet, 700 W)"
 
 
 def ncu_traffic(cfg_k: int, chains: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, as scripts/ncu_traffic.py wrote it into
-    profiles/ from an `ncu --set full` capture of THIS bench command (the build it was taken on is recorded beside it)."""
+    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel, as scripts/ncu_traffic.py recorded it in
+    profiles/ncu_traffic.json from an `ncu --set full` capture of this bench command (the build it was taken on is recorded beside
+    it). None when no record exists for this config and chain count."""
     p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if not os.path.exists(p):
         return None, None
-    try:
-        with open(p) as f:
-            d = json.load(f)
-        e = d.get(f"config{cfg_k}")
-        if e and int(e.get("chains", -1)) == int(chains):
-            return e, "profiles/ncu_traffic.json (%s)" % e.get("source", "?")
-    except Exception:
-        try:                                         # cgroup v1
-            q = float(open("/sys/fs/cgroup/cpu/cpu.cfs_quota_us").read())
-            per = float(open("/sys/fs/cgroup/cpu/cpu.cfs_period_us").read())
-            if q > 0:
-                quota = q / per
-                cores = max(1, min(visible, int(quota + 0.999)))
-        except Exception:
-            pass
+    with open(p) as f:
+        e = json.load(f).get(f"config{cfg_k}")
+    if e and int(e.get("chains", -1)) == int(chains):
+        return e, "profiles/ncu_traffic.json (%s)" % e.get("source", "?")
     return None, None
+
+
+def dump_chains(local: int, bytes_per_chain: int, max_bytes: int = DUMP_BYTES) -> np.ndarray:
+    """The chains --dump-outputs writes: all of them, or above `max_bytes` a fixed, seeded sample (sorted chain indices)."""
+    k = min(local, max(1, max_bytes // bytes_per_chain))
+    return np.arange(local) if k == local else np.sort(np.random.default_rng(20240501).choice(local, k, replace=False))
+
+
+def dump_outputs(out_dir: str, sampler, cfg: Config, dev_out, max_bytes: int = DUMP_BYTES) -> None:
+    """The draws of the last timed step, as sample() would shape them ([iters, chains, *dim]), one float64 .npy per parameter,
+    for the chains dump_chains() picks: the same chains for the same arguments."""
+    import torch
+    iters, entries, local = dev_out.shape
+    pick = dump_chains(local, iters * entries * 8, max_bytes)
+    block = dev_out.index_select(2, torch.from_numpy(pick).to(dev_out.device)).cpu().numpy()
+    os.makedirs(out_dir, exist_ok=True)
+    for name in cfg.params:
+        np.save(os.path.join(out_dir, name + ".npy"), sampler._shape_out(name, block[:, sampler._entries(name), :]).astype(np.float64))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -410,6 +419,8 @@ def run_ours(args):
     dt = time.perf_counter() - t0
     launches = sampler.kernel_launches() - launches0
     clk = clocks.stop() if clocks else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sampler, cfg, dev_out)
     del dev_out
 
     # ---- the measured fp64 roof, same process, same clocks ------------------------------------------------------------
@@ -490,7 +501,7 @@ def run_ours(args):
                        "burn_in_setup": burn, "adapting": True, "gpus_quoted_in_BASELINE": cfg.gpus_quoted,
                        "parallelism": f"chains sharded x{world}, no data-path collective",
                        "l2": "every step writes its samples (iters*entries*chains*8 B = %.2f GB per GPU) and re-reads per-chain state; "
-                             "inputs + outputs exceed the 126 MB L2" % (iters * E * local * 8 / 1e9),
+                             "inputs + outputs exceed the 50 MB L2" % (iters * E * local * 8 / 1e9),
                        "lowering": info[-1] if info else None, "create_seconds": round(t_create, 2)},
             "roofline": {"bound": "hbm", "achieved": ach_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": ach_gbs / hbm_peak,
                          "traffic": (traffic or {}).get("dram_bytes_per_launch"), "traffic_source": traffic_src,
@@ -532,7 +543,7 @@ def run_ours(args):
                 line["cpu_baseline"] = {"value": v, "unit": "draws/s", "cores": 1, "kind": "port", "sample": sample,
                                         "published_reference": "README.md:252: ~4e4 draws/s at N=1000 (author's machine, 2015)"}
             # The probe steps `faithful` handles (the reference's arithmetic, term by term) on the FULL-SIZE data. On config 5 that is
-            # 8 x 1e6 interpreted point-terms per sweep for a single warp (minutes): asked for with --probe, recorded in profiles/.
+            # 8 x 1e6 interpreted point-terms per sweep for a single warp (minutes): asked for with --probe.
             # At N > 1 the other ranks would idle behind rank 0: the probe belongs to the single-GPU run of the same config.
             want_probe = args.probe or (not args.no_probe and world == 1 and cfg.k != 5)
             if want_probe:
@@ -556,7 +567,12 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg and the parity probe")
     ap.add_argument("--no-probe", action="store_true", help="skip the in-run parity probe")
     ap.add_argument("--probe", action="store_true", help="force the in-run parity probe (default: single-GPU runs of configs 2-4)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the draws of the last one to DIR/<parameter>.npy (float64; a fixed sample of "
+                         "the chains when they exceed %d MB)" % (DUMP_BYTES >> 20))
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * amwg.h -- C ABI of the B200-native many-chain AMWG sampler (libamwg_b200.so).
+ * amwg.h -- C ABI of the H100-native many-chain AMWG sampler (libamwg_b200.so).
  *
  * The reference (rasmusab/bayes.js) has no FFI: its boundary is the JavaScript object API
  *     new mcmc.AmwgSampler(params, log_post, data, options)   mcmc.js:1090-1092, 940-966
@@ -279,7 +279,7 @@ AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int6
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it
- * for sm_100a with NVRTC and steps with that kernel instead of the bytecode interpreter (csrc/amwg_jit.cuh; AMWG_JIT=0 in the
+ * for sm_90a with NVRTC and steps with that kernel instead of the bytecode interpreter (csrc/amwg_jit.cuh; AMWG_JIT=0 in the
  * environment keeps the interpreter, AMWG_JIT=1 specialises whatever the number of chains). amwg_jit_status: 1 when the handle
  * runs a specialised kernel, with a one-line description (or the reason it does not) in `note`. amwg_jit_compile_check: generate
  * and compile without a GPU (0 compiled, 1 model not eligible, -1 error; message in `log`, generated source in `src`). */

@@ -1,6 +1,6 @@
 // amwg_rewrite.js -- turn the SOURCE of a log_post closure into a function that can be run on symbolic values.
 //
-// The reference calls an opaque JS closure per step (mcmc.js:958-960, 524-526). The B200 sampler needs that closure as a
+// The reference calls an opaque JS closure per step (mcmc.js:958-960, 524-526). The H100 sampler needs that closure as a
 // program (include/amwg.h), and JavaScript has no operator overloading: `log_post += ld.norm(data[i], state.mu, state.sigma)`
 // cannot be intercepted at run time. So the closure is recorded FROM ITS SOURCE: `log_post.toString()` is parsed (ES5), every
 // operator, property read, method call and truth test is rewritten into a call on a runtime object `__r`, and the rewritten

@@ -1,4 +1,4 @@
-// distributions.js -- the `ld` log-density surface of rasmusab/bayes.js (distributions.js:63-284) for the B200 sampler.
+// distributions.js -- the `ld` log-density surface of rasmusab/bayes.js (distributions.js:63-284) for the H100 sampler.
 //
 // Inside log_post the calls are recorded from source (amwg_rewrite.js / amwg_trace.js) and become device opcodes whose
 // implementation (csrc/amwg_ld.cuh) follows the reference operation by operation; this module is what `ld.norm(183, 180, 5)`

@@ -1,10 +1,10 @@
-// mcmc.js -- the JavaScript host side of the B200-native AMWG sampler: a drop-in for rasmusab/bayes.js' `mcmc` module on the one
+// mcmc.js -- the JavaScript host side of the H100-native AMWG sampler: a drop-in for rasmusab/bayes.js' `mcmc` module on the one
 // path this package accelerates,
 //
 //     var sampler = new mcmc.AmwgSampler(params, log_post, data, options);      // reference: mcmc.js:1090-1092, 940-966
 //     sampler.burn(1000); var samples = sampler.sample(5000);                    //            mcmc.js:1035-1039, 1005-1030
 //
-// Same names, argument meaning and thrown strings as the reference; the stepping happens in libamwg_b200.so (CUDA, sm_100a)
+// Same names, argument meaning and thrown strings as the reference; the stepping happens in libamwg_b200.so (CUDA, sm_90a)
 // for `options.chains` independent chains at once, reached through the N-API addon js/amwg_napi.cc (`require("./amwg_native")`,
 // a thin wrapper over include/amwg.h). log_post is recorded from its source (amwg_rewrite.js) and lowered to the device program
 // (amwg_trace.js). Nothing here computes a log density or draws a proposal: there is no CPU path.

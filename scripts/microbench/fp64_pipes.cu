@@ -1,5 +1,5 @@
 // Micro-benchmark behind DESIGN.md's Poisson-plate notes: how fast are DFMA, DMMA (mma.sync m8n8k4 f64) and broadcast LDS.128 on
-// this GPU, alone and together?  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_pipes fp64_pipes.cu && ./fp64_pipes
+// this GPU, alone and together?  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_pipes fp64_pipes.cu && ./fp64_pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an `ncu --set full` capture of the sweep kernel into a small markdown file under profiles/.
+"""Summarise an `ncu --set full` capture of the sweep kernel into a small markdown file.
 
-    python scripts/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r01_xxx.md [--so path/to/libamwg_b200.so] [--warp-steps N]
+    python scripts/ncu_summary.py prof.ncu-rep summary.md [--so path/to/libamwg_b200.so] [--warp-steps N]
 
 Reads the report here (no GPU needed): raw metrics page + SASS source page. With --so the SASS page is split per device
 function (the noinline functions are sub-symbols of the kernel) using `cuobjdump -elf`.

@@ -3,9 +3,9 @@
 
     python scripts/ncu_traffic.py <report.ncu-rep> --config 2 --chains 1048576 --sweeps-per-launch 50 [--note "..."]
 
-Reads one `ncu --set full` capture (taken under gpurun from the SAME bench command, e.g.
-`ncu --set full --clock-control none -k regex:amwg_jit_sweep -s 6 -c 1 -o gpurun_out/prof_c2 python bench.py --steps 1 --warmup 1 --no-cpu`)
-here, without a GPU, and writes dram__bytes_read.sum + dram__bytes_write.sum of that launch into profiles/ncu_traffic.json,
+Reads one `ncu --set full` capture of the SAME bench command, e.g.
+`ncu --set full --clock-control none -k regex:amwg_jit_sweep -s 6 -c 1 -o prof_c2 python bench.py --steps 1 --warmup 1 --no-cpu`
+(reading the report needs no GPU), and writes dram__bytes_read.sum + dram__bytes_write.sum of that launch into profiles/ncu_traffic.json,
 keyed by config, together with the commit it was taken on. bench.py reads the file; nothing is hard-coded there."""
 import argparse
 import csv
@@ -42,6 +42,7 @@ def main():
              "dram_bytes_per_launch": rd + wr, "duration_ns_under_ncu": m.get("gpu__time_duration.sum", ("", "?"))[1],
              "source": os.path.basename(a.report) + " @ " + head + (" -- " + a.note if a.note else "")}
     path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     data = {}
     if os.path.exists(path):
         with open(path) as f:

@@ -14,7 +14,7 @@ graft.load_package()          # registers `bayes_js_b200` (the directory name ba
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 @pytest.fixture(scope="session")

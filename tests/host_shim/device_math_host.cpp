@@ -1,5 +1,5 @@
 // Test infrastructure: the product's device arithmetic (csrc/amwg_math.cuh, csrc/amwg_ld.cuh -- the same files nvcc and NVRTC compile
-// for sm_100a) compiled for the host behind a C ABI. Built by tests/test_device_math_on_host.py with -ffp-contract=off (the GPU build
+// for sm_90a) compiled for the host behind a C ABI. Built by tests/test_device_math_on_host.py with -ffp-contract=off (the GPU build
 // uses --fmad=false): every operation is one IEEE-754 fp64 operation on both sides.
 #include "amwg_math.cuh"
 #include "amwg_ld.cuh"

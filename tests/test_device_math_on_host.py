@@ -1,7 +1,7 @@
 """The product's device arithmetic, compiled for the HOST, against the oracle -- without a GPU.
 
 csrc/amwg_math.cuh (Math.log / Math.exp as fdlibm, Math.round, the Philox "Math.random()" stream, rnorm of mcmc.js:43-54) and
-csrc/amwg_ld.cuh (every scalar ld.* of distributions.js:63-284) are the files nvcc and NVRTC compile for sm_100a. Here g++ compiles the
+csrc/amwg_ld.cuh (every scalar ld.* of distributions.js:63-284) are the files nvcc and NVRTC compile for sm_90a. Here g++ compiles the
 same text (tests/host_shim supplies the five CUDA intrinsics they use; -ffp-contract=off matches --fmad=false) and the results are
 held against the C oracle bit for bit on the inputs tests/test_gpu_parity.py uses on the GPU. What this adds to the GPU tests: an edit
 to either header is caught by the CPU suite; what it cannot show: that the GPU's own sqrt / division / pow round like the host's

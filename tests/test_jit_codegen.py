@@ -1,4 +1,4 @@
-"""Run-time specialisation (csrc/amwg_jit.cuh), CPU side: the generated CUDA source of eligible models compiles for sm_100a
+"""Run-time specialisation (csrc/amwg_jit.cuh), CPU side: the generated CUDA source of eligible models compiles for sm_90a
 with NVRTC (no GPU needed), ineligible models say why, and malformed programs are refused by amwg_create's validation."""
 import ctypes as C
 
@@ -37,7 +37,7 @@ def test_hierarchical_model_classes_loops_and_streaming(pkg):
     # the 64 group means are ONE class (indices from tables), sigma's 64 plate terms are a loop, y (512 KB) streams through the ring
     assert "const int m = JMEM[c];" in src and "for (int j = 0; j < 63; ++j)" in src
     assert "#define JSTREAM 1" in src and "#define JN_SSTAT 64" in src and "#define JS_TOTAL 65536" in src
-    # 2^16 chains: 512 CTAs of 128 threads, four per SM (measured faster than the better balanced 224 x 2)
+    # 2^16 chains: 512 CTAs of 128 threads, four per SM (the default CTA size; no other size balances the SMs markedly better)
     assert "#define JTHREADS 128" in src and "#define JMINB 4" in src
 
 
@@ -139,7 +139,7 @@ def test_parameter_array_indexed_out_of_bounds_is_refused(pkg):
 
 def test_every_golden_model_is_specialised_or_says_why(pkg):
     """Code generation over the reference's own fixtures (the 32 sampler scenarios of tests/golden/reference_js.json, `faithful`
-    lowering as the golden tests run them): each model either compiles for sm_100a or is turned down for a stated reason -- the
+    lowering as the golden tests run them): each model either compiles for sm_90a or is turned down for a stated reason -- the
     generator never fails on a valid program. (With AMWG_JIT=1 the GPU golden tests run these kernels against the vectors.)"""
     import copy
     import golden_util as gu

@@ -1,6 +1,6 @@
 """What the code generator prints, executed -- without a GPU.
 
-tests/test_jit_codegen.py checks that the specialised full-program sweep of a model COMPILES for sm_100a; the GPU tests check that it
+tests/test_jit_codegen.py checks that the specialised full-program sweep of a model COMPILES for sm_90a; the GPU tests check that it
 draws what the interpreter kernels draw. This file closes the gap on the CPU tier: the generated `jit_logpost()` / `jit_derived()`
 (csrc/amwg_jit.cuh) is compiled for the host together with the product's own arithmetic headers and the plate helpers of the kernel
 skeleton (csrc/amwg_jit_full_kernel.cuh, taken from the file's text) and evaluated at random states, moved components and proposal
