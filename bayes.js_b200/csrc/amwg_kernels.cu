@@ -81,6 +81,20 @@ struct ModelDev {
   int variant_derived[1 << AMWG_MAX_VARIANT_COMPS];
 };
 
+// Where a plate reads its O(N) column. The kernels (stage_model, plate_sum_sq, pois_plate_k) and the host's report of it
+// (amwg_plate_sources) decide with these two functions, so the report says what runs.
+enum PlateSource : int { kSrcShared = 0, kSrcRing = 1, kSrcL2 = 2 };
+// the TMA tile ring is usable when the model reserved it and the whole CTA walks the plates together (uniform steps, one program)
+__host__ __device__ __forceinline__ bool ring_active(int ring_smem_off, int phase_sync, int n_variant_comps) {
+  return ring_smem_off >= 0 && phase_sync && n_variant_comps == 0;
+}
+// resident columns are read from shared memory; otherwise a plate with a streamed form (NORM_IID, POIS_LOGLIN) whose data starts on
+// a 16-byte boundary (the ring's bulk copies) goes through the ring when there is one, and everything else reads global/L2
+__host__ __device__ __forceinline__ int plate_source(bool resident, bool ring, bool streamable, const void* start) {
+  if (resident) return kSrcShared;
+  return (ring && streamable && (reinterpret_cast<unsigned long long>(start) & 15ull) == 0) ? kSrcRing : kSrcL2;
+}
+
 struct Ctx {                       // lives in shared memory
   const int* code;
   const double* consts;
@@ -142,7 +156,7 @@ __device__ __forceinline__ void stage_model(const ModelDev& m, unsigned char* sm
     mbar_init(bar, 1);
     for (int k = 0; k < kRingStages; ++k) { mbar_init(&ctx.ring_bar[k], 1); ctx.ring_uses[k] = 0; }
     // the ring needs every thread of the CTA to walk the same plates in the same order: uniform steps and a single program
-    ctx.ring_saddr = (m.ring_smem_off >= 0 && m.phase_sync && m.n_variant_comps == 0) ? smem_u32(smem + m.ring_smem_off) : 0u;
+    ctx.ring_saddr = ring_active(m.ring_smem_off, m.phase_sync, m.n_variant_comps) ? smem_u32(smem + m.ring_smem_off) : 0u;
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -225,7 +239,7 @@ __device__ __forceinline__ double plate_sum_sq(const Ctx& ctx, int q, double mea
   int c = pl.col[0], off = pl.iparam[2];
   unsigned sa = ctx.col_saddr[c] ? ctx.col_saddr[c] + 8u * (unsigned)off : 0u;
   const double* gx = ctx.col[c] + off;
-  if (sa == 0u && ctx.ring_saddr && (reinterpret_cast<unsigned long long>(gx) & 15ull) == 0)
+  if (plate_source(sa != 0u, ctx.ring_saddr != 0u, true, gx) == kSrcRing)
     return sum_sq_stream(const_cast<Ctx&>(ctx), gx, pl.n, mean);       // column lives in HBM/L2: TMA tile ring
   return sum_sq_dev(gx, sa, pl.n, mean);
 }
@@ -450,9 +464,10 @@ __device__ __forceinline__ double pois_plate_k(Ctx& ctx, const amwg_plate& pl, c
   const unsigned tab_sa = smem_u32(ctx.exp_tab);
   double s0 = 0.0, s1 = 0.0;
   const unsigned xres = ctx.col_saddr[pl.col[1]];
-  if (xres) {
+  const int src = plate_source(xres != 0u, ctx.ring_saddr != 0u, true, X);
+  if (src == kSrcShared) {
     pois_rows<K>(xres, n, beta, tab_sa, s0, s1);
-  } else if (!ctx.ring_saddr || (reinterpret_cast<unsigned long long>(X) & 15ull)) {
+  } else if (src == kSrcL2) {
     pois_rows_global<K>(X, n, beta, tab_sa, s0, s1);
   } else {
     const int R = (int)((kRingStageBytes / (unsigned)(K * 8)) & ~1u);          // rows per stage (even: every tile is a multiple of 16 B)
@@ -1258,6 +1273,7 @@ struct amwg_sampler {
   double last_sweep_ms = 0.0;
   // run-time specialised sweep (amwg_jit.cuh): active when jit_kernel != nullptr
   cudaKernel_t jit_kernel = nullptr;
+  std::string plate_note;          // amwg_plate_sources
   unsigned jit_smem = 0;
   int jit_threads = 0;
   std::string jit_note = "not attempted";
@@ -1437,6 +1453,27 @@ static int device_norm_c0(int device, double* out) {
   if (amwg_primitive_eval(0, &two_pi, 1, 0, 0, &lg, device)) return -1;
   *out = -0.5 * lg;
   return 0;
+}
+
+// Where the interpreter kernels (init, sweeps, log_post re-evaluation) read each plate's O(N) column, with the kernels' own
+// predicates: "shared", "ring", "L2", or "loop" for a bytecode plate, which reads point by point. NORM_GROUPED and BERN_IID have
+// no streamed form.
+static std::string plate_sources(const ModelDev& m, const amwg_model* md) {
+  static const char* kName[] = {"shared", "ring", "L2"};
+  const bool ring = ring_active(m.ring_smem_off, m.phase_sync, m.n_variant_comps);
+  std::string out;
+  for (int q = 0; q < md->n_plates; ++q) {
+    const amwg_plate& pl = md->plates[q];
+    const char* where = "loop";
+    if (pl.kind != AMWG_PLATE_GENERIC) {
+      const bool pois = pl.kind == AMWG_PLATE_POIS_LOGLIN;
+      const int c = pois ? pl.col[1] : pl.col[0];
+      const double* start = m.col_global[c] + (pois ? 0 : pl.iparam[2]);
+      where = kName[plate_source(m.col_smem_off[c] >= 0, ring, pois || pl.kind == AMWG_PLATE_NORM_IID, start)];
+    }
+    out += (q ? "," : "") + std::string(where);
+  }
+  return out;
 }
 
 // Try to replace the interpreter sweep of this handle by a kernel specialised for its model (amwg_jit.cuh). Never fatal: on any
@@ -1657,6 +1694,7 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
   if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
   if (e != cudaSuccess) return bail(fail(std::string("amwg_init_kernel: ") + cudaGetErrorString(e)));
   try_jit(s, md);
+  s->plate_note = plate_sources(m, md);
   *out = s;
   return 0;
 }
@@ -1874,6 +1912,13 @@ extern "C" int amwg_jit_status(const amwg_sampler* s, char* note, int64_t cap) {
   if (!s) return 0;
   if (note && cap > 0) { snprintf(note, (size_t)cap, "%s", s->jit_note.c_str()); }
   return s->jit_kernel ? 1 : 0;
+}
+
+// where the interpreter kernels read each plate's column, comma-separated in plate order (plate_sources); returns the plate count
+extern "C" int amwg_plate_sources(const amwg_sampler* s, char* out, int64_t cap) {
+  if (!s) return -1;
+  if (out && cap > 0) { snprintf(out, (size_t)cap, "%s", s->plate_note.c_str()); }
+  return s->plate_note.empty() ? 0 : 1 + (int)std::count(s->plate_note.begin(), s->plate_note.end(), ',');
 }
 
 // Generate and compile the specialised sweep of `model` without a GPU (NVRTC targets sm_90a from any host): 0 = compiled,

@@ -657,6 +657,13 @@ class AmwgSampler(Sampler):
         on = _ffi.lib().amwg_jit_status(self._handle, buf, len(buf))
         return bool(on), buf.value.decode("utf-8", "replace")
 
+    def plate_sources(self) -> List[str]:
+        """Where the interpreter kernels (init, sweeps, the log_post() re-evaluation) read each plate's column, in plate order:
+        "shared", "ring", "L2", or "loop" for a bytecode plate."""
+        buf = C.create_string_buffer(4096)
+        n = _ffi.lib().amwg_plate_sources(self._handle, buf, len(buf))
+        return buf.value.decode().split(",") if n > 0 else []
+
     def jit_compile_check(self, n_chains=None):
         """Generate and compile the specialised sweep of this model without running it (works without a GPU).
         -> (rc, message, source): rc 0 compiled, 1 model not eligible, -1 error."""

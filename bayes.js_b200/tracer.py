@@ -725,10 +725,12 @@ class Lowering:
             p.summary.append(f"plate BERN_IID n={n}")
         elif body.op == "LD_POIS" and data_i(body.args[0]) and body.args[1].op == "EXP":
             lin = self._loglinear(body.args[1].args[0])
-            if lin is not None:
+            y = body.args[0]
+            ycol = self.t.columns[y.val[0]][y.val[1]: y.val[1] + n]
+            # ld.pois of a negative count is -Infinity (distributions.js:282-284), whatever the rate; the factorised sum has no place
+            # for it (its lfactorial constant would be NaN), so such data keeps the term-by-term loop
+            if lin is not None and not np.any(ycol < 0):
                 xcol, K, base = lin
-                y = body.args[0]
-                ycol = self.t.columns[y.val[0]][y.val[1]: y.val[1] + n]
                 # sum_i [y_i eta_i - exp(eta_i) - lfactorial(y_i)]: the first part is beta . (X^T y), the last a constant; both are
                 # precomputed here (constant in the parameters), the device sums exp(eta_i) over the rows
                 X = self.t.columns[xcol][: n * K].reshape(n, K)

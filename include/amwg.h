@@ -285,6 +285,10 @@ AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int6
  * and compile without a GPU (0 compiled, 1 model not eligible, -1 error; message in `log`, generated source in `src`). */
 AMWG_API int amwg_jit_status(const amwg_sampler* s, char* note, int64_t cap);
 AMWG_API int amwg_jit_compile_check(const amwg_model* model, uint64_t n_chains, char* log, int64_t log_cap, char* src, int64_t src_cap);
+/* amwg_plate_sources: where the interpreter kernels (init, sweeps, the log_post re-evaluation) read each plate's column, in plate
+ * order, comma-separated: "shared" (resident), "ring" (the TMA tile ring), "L2" (global loads) or "loop" (a bytecode plate).
+ * Returns the number of plates. */
+AMWG_API int amwg_plate_sources(const amwg_sampler* s, char* out, int64_t cap);
 
 /* ---- measurement ---------------------------------------------------------------------------------------------------------
  * The binding roof of this path is the non-tensor fp64 pipe (DADD + DFMA per data point), which MEASURED_PEAKS.json does not

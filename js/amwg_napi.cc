@@ -372,6 +372,13 @@ BINDING(jit_status)
   const int on = amwg_jit_status(handle_of(env, a.at(0))->s, note, sizeof note);
   return js_string(env, std::string(on ? "specialised: " : "interpreter: ") + note);
 END_BINDING
+// plate_sources(handle) -> "shared,ring,..." (where each plate's column is read) amwg_plate_sources
+BINDING(plate_sources)
+  char out[1024];
+  out[0] = 0;
+  amwg_plate_sources(handle_of(env, a.at(0))->s, out, sizeof out);
+  return js_string(env, out);
+END_BINDING
 // jit_compile_check(descriptor, n_chains) -> {rc, log}                           amwg_jit_compile_check
 BINDING(jit_compile_check)
   Model M;
@@ -393,7 +400,7 @@ NAPI_MODULE_INIT() {
       {"get_log_post", get_log_post}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
-      {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"peak_fp64", peak_fp64}, {"jit_status", jit_status},
+      {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
     napi_value fn;

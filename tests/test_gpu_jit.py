@@ -84,19 +84,27 @@ def test_config2_size_data_thin_monitor_and_stop_adaptation(gpu_pkg, monkeypatch
 def _hier_data(J, per, seed=5):
     g = np.repeat(np.arange(J), per)
     mu_true = np.random.default_rng(seed).normal(100, 20, J)
-    y = mu_true[g] + np.random.default_rng(seed + 1).normal(0, 5, J * per)
+    y = mu_true[g] + np.random.default_rng(seed + 1).normal(0, 5, g.size)
     return {"y": y, "g": g.astype(float)}, mu_true
 
 
-@pytest.mark.parametrize("J,per,chains", [(6, 40, 4096), (12, 1024, 2200)])
+# unequal groups of >= 8 points on a streamed column (tiles of 1024 points): boundaries mid-tile, a 2500-point group spanning more
+# than two tiles, a 9-point group inside one, an odd total (9563)
+RAGGED = (9, 2500, 37, 1111, 3001, 14, 777, 1500, 614)
+
+
+@pytest.mark.parametrize("J,per,chains", [(6, 40, 4096), (12, 1024, 2200), (len(RAGGED), RAGGED, 2200)])
 def test_hierarchical_model_resident_and_streamed(gpu_pkg, monkeypatch, J, per, chains):
     """(6 x 40): every column resident in shared memory; (12 x 1024 = 96 KB): the column streams through the TMA tile ring, with a
-    chain count that is not a multiple of the CTA size (shadow threads take part in the ring)."""
+    chain count that is not a multiple of the CTA size (shadow threads take part in the ring); unequal groups: the sweep splits a
+    streamed tile between plates wherever a group ends inside it."""
     pkg = gpu_pkg
-    data, mu_true = _hier_data(J, per)
+    sizes = np.broadcast_to(per, (J,))
+    data, mu_true = _hier_data(J, sizes)
+    g = data["g"].astype(np.int64)
     P = {"mu": {"type": "real", "dim": [J], "init": 100.0}, "sigma": {"type": "real", "lower": 0, "init": 5.0}}
     a, b = _pair(pkg, monkeypatch, P, models.hier_norm_post(pkg.ld), data, chains, seed=21)
-    assert ("streamed column" in b.jit_status()[1]) == (J * per * 8 > 64 * 1024)
+    assert ("streamed column" in b.jit_status()[1]) == (g.size * 8 > 64 * 1024)
     for s in (a, b):
         s.burn(55)
     da, db = a.sample(6), b.sample(6)
@@ -105,9 +113,9 @@ def test_hierarchical_model_resident_and_streamed(gpu_pkg, monkeypatch, J, per, 
     assert _agreement(da["sigma"][:, :, None], db["sigma"][:, :, None]) > 0.98
     b.burn(2500)
     d = b.sample(20)
-    ybar = data["y"].reshape(J, per).mean(axis=1)
-    assert np.allclose(d["mu"].mean(axis=(0, 1)), ybar, atol=6 * 5 / np.sqrt(per) / np.sqrt(chains * 20 / 50) + 0.05)
-    assert abs(d["sigma"].mean() - np.sqrt(((data["y"].reshape(J, per) - ybar[:, None]) ** 2).sum() / (J * per - J))) < 0.05 + 2.0 / np.sqrt(J * per)
+    ybar = np.bincount(g, weights=data["y"]) / sizes
+    assert np.allclose(d["mu"].mean(axis=(0, 1)), ybar, atol=6 * 5 / np.sqrt(sizes) / np.sqrt(chains * 20 / 50) + 0.05)
+    assert abs(d["sigma"].mean() - np.sqrt(((data["y"] - ybar[g]) ** 2).sum() / (g.size - J))) < 0.05 + 2.0 / np.sqrt(g.size)
 
 
 def test_expression_means_int_parameter_and_bounds(gpu_pkg, monkeypatch):

@@ -556,14 +556,21 @@ def test_the_statistics_sweep_on_the_host_headline_model(pkg, orc, tmp_path):
     assert np.isfinite(out).all() and np.unique(out[-1, 0]).size > 50
 
 
-@pytest.mark.parametrize("J,per,stream", [(8, 32, False), (6, 1500, True), (8, 1100, True)])
+# unequal groups (all >= 8 points, so each is a plate of its own) on a streamed column: boundaries fall mid-tile (tiles of 1024
+# points), the 2500-point group spans more than two tiles, the 9-point group lies inside one, and the total (9563) is odd
+RAGGED = (9, 2500, 37, 1111, 3001, 14, 777, 1500, 614)
+
+
+@pytest.mark.parametrize("J,per,stream", [(8, 32, False), (6, 1500, True), (8, 1100, True), (len(RAGGED), RAGGED, True)])
 def test_the_statistics_sweep_on_the_host_hierarchical_model(pkg, orc, tmp_path, J, per, stream):
     """BASELINE config 4's shape: a vector of group means (one class, indices from tables, stepped as an index-ordered block between
     the steps the chain visits before and after it) and a shared sd whose plate terms are a loop; with 9000 points the column streams
-    through the tile ring (memcpy here)."""
+    through the tile ring (memcpy here). `per` may list unequal group sizes: then a streamed tile is split between plates wherever
+    a group ends inside it."""
+    sizes = np.broadcast_to(per, (J,))
     rng = np.random.default_rng(4)
-    g = np.repeat(np.arange(J), per)
-    y = rng.normal(100, 5, J * per) + np.repeat(rng.normal(0, 3, J), per)
+    g = np.repeat(np.arange(J), sizes)
+    y = rng.normal(100, 5, g.size) + np.repeat(rng.normal(0, 3, J), sizes)
     P = {"mu": {"type": "real", "dim": [J], "init": 100.0}, "sigma": {"type": "real", "lower": 0, "init": 5.0}}
     data = {"y": y, "g": g.astype(float)}
     hk = HostStatKernel(pkg, orc, tmp_path, P, models.hier_norm_post(pkg.ld), data)

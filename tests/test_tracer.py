@@ -180,6 +180,33 @@ def test_hierarchical_and_regression_plates(pkg, orc):
     assert abs(prog_eval.logpost(prog, consts, st, orc.lib()) - ref) <= 1e-11 * abs(ref)
 
 
+def test_poisson_plate_with_a_negative_count_is_minus_infinity(pkg, orc):
+    """ld.pois of a negative count is -Infinity (distributions.js:282-284). The factorised plate would carry lfactorial(-1) = NaN in
+    its constant, so such data keeps the term-by-term loop: log_post is -Infinity, as the oracle's, at every state."""
+    ld, mcmc = pkg.ld, pkg.mcmc
+    rng = np.random.default_rng(6)
+    K, n_pts = 2, 30
+    X = np.column_stack([np.ones(n_pts), rng.normal(0, 0.5, n_pts)])
+    yy = rng.poisson(1.5, n_pts).astype(float)
+    yy[11] = -1.0
+
+    def poisreg(state, d):
+        lp = 0
+        for k in range(K):
+            lp += ld.norm(state.beta[k], 0, 10)
+        for i in mcmc.points(len(d.y)):
+            lp += ld.pois(d.y[i], mcmc.Math.exp(d.X[i][0] * state.beta[0] + d.X[i][1] * state.beta[1]))
+        return lp
+    params = {"beta": {"type": "real", "dim": [K]}}
+    prog, _, _ = _trace(pkg, poisreg, params, {"y": yy.tolist(), "X": X.tolist()})
+    assert prog.summary[-1] == f"plate GENERIC n={n_pts} body=LD_POIS"
+    consts = prog_eval.fold_constants(prog, orc.lib())
+    for _ in range(5):
+        st = list(rng.normal(0, 0.3, K))
+        ref, _ = _oracle_logpost(orc, "pois_reg", {"y": yy, "X": X}, params, st)
+        assert ref == -np.inf and prog_eval.logpost(prog, consts, st, orc.lib()) == -np.inf
+
+
 def test_pre_evaluated_statistics_programs(pkg, orc, monkeypatch):
     """amwg.h stat_prog: NORM_IID plates whose mean reads one component are split into S (one data pass per sweep, at every
     component's proposal) and f(S, sd); the per-component programs then hold no O(N) work and still give the full program's value."""
