@@ -10,6 +10,9 @@
 //   K_q   amwg_digit_hist_kernel    : one pass of an exact MSD radix select over the order-preserving 64-bit key of the draws:
 //                                     counts of the next 8-bit digit among the values whose higher digits equal a given prefix
 //                                     (integer counts: exact, order independent, summed across GPUs by the caller)
+//   K_a1  amwg_autocov_kernel       : one thread per chain: split-chain (two halves) moment records and lag sums of the draws and
+//                                     of two tail indicators, for 16 lags per pass (effective sample size, split R-hat)
+//   K_a2  amwg_merge_sums_kernel    : one CTA per (entry, series, lag) sums the per-CTA lag sums in a FIXED order
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
 
@@ -149,6 +152,154 @@ __global__ void __launch_bounds__(256) amwg_digit_hist_kernel(const double* __re
     if (hist[i]) atomicAdd(&counts[(size_t)e * n_prefix * 256 + i], (unsigned long long)hist[i]);
 }
 
+// ---- split-chain autocovariances (effective sample size, split R-hat) ------------------------------------------------------
+// Every chain of `rows` kept draws is split into a first half (rows [0, h)) and a second half (rows [rows-h, rows)), h = rows/2.
+// Per half-chain m and series y (the draws, or an indicator 1[x <= q] of them), centred by the half-chain's own mean:
+//   record  {1, mean_m, 0, sum_n d_n^2}                 merged like Moments (Chan, fixed order)
+//   lag sum sum_n d_n d_{n+t} = h * acov_m(t)           summed in a fixed order, for t in the lag window
+constexpr int kLagSlots = 16;         // lags per kernel pass: the ring of centred lead values a thread keeps in registers
+
+template <int THREADS>
+__device__ __forceinline__ double cta_sum(double* sh, double mine) {            // fixed tree, like cta_merge
+  const int t = threadIdx.x;
+  sh[t] = mine;
+  __syncthreads();
+  for (int w = THREADS >> 1; w > 0; w >>= 1) {
+    if (t < w) sh[t] += sh[t + w];
+    __syncthreads();
+  }
+  const double r = sh[0];
+  __syncthreads();                                                               // sh is reused by the next call
+  return r;
+}
+
+// K_a1: one thread per chain (grid-stride), both halves. Pass 1 reads the half for its means; pass 2 reads it again and keeps
+// the kLagSlots centred values at positions n+lag0 .. n+lag0+15 in a register ring, so every loaded value serves all lags of the
+// window. NS = 1: the draws only; NS = 3: also 1[x <= thr[e][0]] and 1[x <= thr[e][1]], formed from the same loads (the ring holds
+// their bits). Positions at or past h count as 0, so a product exists exactly when both ends lie in the half.
+// pmom[(e*NS + s)][block] (skipped when null), psum[((e*NS + s)*n_total + k_base + k)][block] for k < n_lags.
+template <int NS>
+__global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                           const double* __restrict__ thr, long long lag0, int n_lags, int k_base, int n_total,
+                                                           Moments* __restrict__ pmom, double* __restrict__ psum) {
+  __shared__ Moments sh[256];
+  const int e = blockIdx.y;
+  const long long h = rows / 2;
+  const size_t stride = (size_t)entries * C;
+  double q0 = 0.0, q1 = 0.0;
+  if constexpr (NS == 3) { q0 = thr[2 * e]; q1 = thr[2 * e + 1]; }
+  double acc[NS][kLagSlots];
+#pragma unroll
+  for (int s = 0; s < NS; ++s)
+#pragma unroll
+    for (int k = 0; k < kLagSlots; ++k) acc[s][k] = 0.0;
+  Moments mom[NS];
+#pragma unroll
+  for (int s = 0; s < NS; ++s) mom[s] = Moments{0.0, 0.0, 0.0, 0.0};
+
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    for (int half = 0; half < 2; ++half) {
+      const double* p = x + (size_t)e * C + c + (size_t)(half ? rows - h : 0) * stride;
+      double s0 = 0.0;
+      long long n0 = 0, n1 = 0;
+      long long r = 0;
+      for (; r + 8 <= h; r += 8) {                           // eight loads in flight per thread, the sum stays sequential
+        double v[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) { s0 += v[u]; if constexpr (NS == 3) { n0 += v[u] <= q0; n1 += v[u] <= q1; } }
+      }
+      for (; r < h; ++r) { const double v = p[r * stride]; s0 += v; if constexpr (NS == 3) { n0 += v <= q0; n1 += v <= q1; } }
+      double m[NS];
+      m[0] = s0 / (double)h;
+      if constexpr (NS == 3) { m[1] = (double)n0 / (double)h; m[2] = (double)n1 / (double)h; }
+
+      double ring[kLagSlots];
+      unsigned valid = 0u, b0 = 0u, b1 = 0u;                  // bit k: slot k lies in the half / its draw is <= q0 / <= q1
+#pragma unroll
+      for (int k = 0; k < kLagSlots; ++k) {
+        const long long pp = lag0 + k;
+        ring[k] = 0.0;
+        if (pp < h) {
+          const double v = p[pp * stride];
+          ring[k] = v - m[0];
+          valid |= 1u << k;
+          if constexpr (NS == 3) { b0 |= (unsigned)(v <= q0) << k; b1 |= (unsigned)(v <= q1) << k; }
+        }
+      }
+      double sw[NS];
+#pragma unroll
+      for (int s = 0; s < NS; ++s) sw[s] = 0.0;
+      for (long long j = 0; j < h; j += kLagSlots) {
+#pragma unroll
+        for (int u = 0; u < kLagSlots; ++u) {                 // unrolled: the ring's slot indices are compile-time constants
+          const long long n = j + u;
+          if (n < h) {
+            const double v = p[n * stride];
+            double cur[NS];
+            cur[0] = v - m[0];
+            if constexpr (NS == 3) { cur[1] = v <= q0 ? 1.0 - m[1] : -m[1]; cur[2] = v <= q1 ? 1.0 - m[2] : -m[2]; }
+#pragma unroll
+            for (int s = 0; s < NS; ++s) sw[s] = fma(cur[s], cur[s], sw[s]);
+#pragma unroll
+            for (int k = 0; k < kLagSlots; ++k) {
+              const int slot = (u + k) % kLagSlots;         // holds position n + lag0 + k
+              acc[0][k] = fma(cur[0], ring[slot], acc[0][k]);
+              if constexpr (NS == 3) {
+                const bool in = (valid >> slot) & 1u;
+                const double a0 = in ? (((b0 >> slot) & 1u) ? 1.0 - m[1] : -m[1]) : 0.0;
+                const double a1 = in ? (((b1 >> slot) & 1u) ? 1.0 - m[2] : -m[2]) : 0.0;
+                acc[1][k] = fma(cur[1], a0, acc[1][k]);
+                acc[2][k] = fma(cur[2], a1, acc[2][k]);
+              }
+            }
+            const long long pp = n + lag0 + kLagSlots;        // slot u moves on to position n + lag0 + kLagSlots
+            const unsigned bit = 1u << u;
+            ring[u] = 0.0;
+            valid &= ~bit; b0 &= ~bit; b1 &= ~bit;
+            if (pp < h) {
+              const double w = p[pp * stride];
+              ring[u] = w - m[0];
+              valid |= bit;
+              if constexpr (NS == 3) { if (w <= q0) b0 |= bit; if (w <= q1) b1 |= bit; }
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int s = 0; s < NS; ++s) mom[s] = merge(mom[s], Moments{1.0, m[s], 0.0, sw[s]});
+    }
+  }
+  if (pmom) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s) {
+      const Moments tot = cta_merge<256>(sh, mom[s]);
+      if (threadIdx.x == 0) pmom[((size_t)e * NS + s) * gridDim.x + blockIdx.x] = tot;
+      __syncthreads();
+    }
+  }
+  double* shd = reinterpret_cast<double*>(sh);
+#pragma unroll
+  for (int s = 0; s < NS; ++s)
+#pragma unroll
+    for (int k = 0; k < kLagSlots; ++k)
+      if (k < n_lags) {
+        const double tot = cta_sum<256>(shd, acc[s][k]);
+        if (threadIdx.x == 0) psum[(((size_t)e * NS + s) * n_total + k_base + k) * gridDim.x + blockIdx.x] = tot;
+      }
+}
+
+// K_a2: one CTA per (entry, series, lag) sums the per-CTA lag sums in a fixed order.
+__global__ void __launch_bounds__(256) amwg_merge_sums_kernel(const double* __restrict__ psum, int n_partial, double* __restrict__ out) {
+  __shared__ double sh[256];
+  const size_t row = blockIdx.x;
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n_partial; i += 256) acc += psum[row * n_partial + i];
+  const double tot = cta_sum<256>(sh, acc);
+  if (threadIdx.x == 0) out[row] = tot;
+}
+
 }  // namespace summary
 
 extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats) {
@@ -201,5 +352,64 @@ extern "C" int amwg_summary_digit_hist(int device, const double* dev_samples, in
                                                                                   reinterpret_cast<unsigned long long*>(dev_counts));
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+extern "C" int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                    const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out) {
+  if (rows < 2) return fail("amwg_summary_autocov: rows must be at least 2 (two half-chains of one draw)");
+  if (entries <= 0 || chains <= 0) return fail("amwg_summary_autocov: empty sample block");
+  if (n_lags < 1 || n_lags > 2 * summary::kLagSlots) return fail("amwg_summary_autocov: n_lags must be 1.." + std::to_string(2 * summary::kLagSlots));
+  if (lag0 < 0 || lag0 + n_lags > rows / 2)
+    return fail("amwg_summary_autocov: the lag window [lag0, lag0 + n_lags) must lie in [0, rows/2) (rows/2 = " + std::to_string(rows / 2) + ")");
+  if (!dev_samples || !host_out) return fail("amwg_summary_autocov: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_autocov: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const int ns = host_thresholds ? 3 : 1;
+  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);     // depends on `chains` only: a fixed merge order
+  const size_t rec = (size_t)entries * ns, sums = rec * n_lags;
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t b_pmom = up(rec * bx * sizeof(summary::Moments)), b_psum = up(sums * bx * sizeof(double));
+  const size_t b_mom = up(rec * 4 * sizeof(double)), b_sum = up(sums * sizeof(double)), b_thr = up((size_t)entries * 2 * sizeof(double));
+  const size_t need = b_pmom + b_psum + b_mom + b_sum + b_thr;
+  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
+  struct Scratch { void* p = nullptr; size_t bytes = 0; };
+  static Scratch scratch[64];
+  static std::mutex scratch_mu;
+  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
+  Scratch& sc = scratch[device];
+  if (sc.bytes < need) {
+    if (sc.p) cudaFree(sc.p);
+    sc.p = nullptr; sc.bytes = 0;
+    CUDA_TRY(cudaMalloc(&sc.p, need));
+    sc.bytes = need;
+  }
+  char* base = reinterpret_cast<char*>(sc.p);
+  auto* pmom = reinterpret_cast<summary::Moments*>(base);
+  auto* psum = reinterpret_cast<double*>(base + b_pmom);
+  auto* d_mom = reinterpret_cast<double*>(base + b_pmom + b_psum);
+  auto* d_sum = reinterpret_cast<double*>(base + b_pmom + b_psum + b_mom);
+  auto* d_thr = reinterpret_cast<double*>(base + b_pmom + b_psum + b_mom + b_sum);
+  if (host_thresholds) CUDA_TRY(cudaMemcpy(d_thr, host_thresholds, (size_t)entries * 2 * sizeof(double), cudaMemcpyHostToDevice));
+  for (int k0 = 0; k0 < n_lags; k0 += summary::kLagSlots) {                 // one pass over the block per kLagSlots lags
+    const int nk = std::min(summary::kLagSlots, n_lags - k0);
+    summary::Moments* pm = k0 == 0 ? pmom : nullptr;                         // the records do not depend on the lags
+    if (ns == 3)
+      summary::amwg_autocov_kernel<3><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, d_thr, lag0 + k0, nk, k0, n_lags, pm, psum);
+    else
+      summary::amwg_autocov_kernel<1><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, nullptr, lag0 + k0, nk, k0, n_lags, pm, psum);
+  }
+  summary::amwg_merge_moments_kernel<<<(unsigned)rec, 1024>>>(pmom, (int)bx, d_mom);
+  summary::amwg_merge_sums_kernel<<<(unsigned)sums, 256>>>(psum, (int)bx, d_sum);
+  std::vector<double> mom(rec * 4), sm(sums);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(mom.data(), d_mom, mom.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(sm.data(), d_sum, sm.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return fail(std::string("amwg_summary_autocov: ") + cudaGetErrorString(e));
+  const size_t w = 4 + (size_t)n_lags;                                        // host_out[entry][series][4 + n_lags]
+  for (size_t r = 0; r < rec; ++r) {
+    for (int i = 0; i < 4; ++i) host_out[r * w + i] = mom[r * 4 + i];
+    for (int k = 0; k < n_lags; ++k) host_out[r * w + 4 + k] = sm[r * n_lags + k];
+  }
   return 0;
 }

@@ -543,13 +543,18 @@ class AmwgSampler(Sampler):
             raise JsThrow(L.amwg_last_error().decode())
         return buf
 
-    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975)):
+    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
         statistics with numpy.quantile's linear rule; a long grid such as numpy.linspace(0, 1, 41) gives an equal-mass histogram and
         runs as several radix selects of 16 probabilities each). With options.distributed every rank returns the all-GPU summary
-        (two small collectives, summary.py). Advances the chains exactly as sample(n) does."""
+        (two small collectives, summary.py). Advances the chains exactly as sample(n) does.
+        diagnostics=True adds, per parameter and shaped like "mean": "ess_mean" and "ess_tail" (split-chain effective sample
+        sizes of the draws and of the 5 % / 95 % tail indicators, Vehtari et al. 2021), "mcse_mean" (sd / sqrt(ess_mean)) and
+        "rhat_split" (split-chain R-hat, not rank-normalised); the other keys keep their values bit for bit. Fewer than 10 kept
+        rows give NaN; see summary.split_chain_diagnostics for the estimator and its edge cases. All chains start from the same
+        init, so "rhat" and "rhat_split" only mean something after burn-in."""
         import torch
         from .summary import CudaBlockReducer, summarise_block
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
@@ -580,7 +585,8 @@ class AmwgSampler(Sampler):
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
         t2 = time.perf_counter()
-        mean, sd, rhat, q = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed)
+        res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
+        mean, sd, rhat, q = res[:4]
         del block
         if timing:
             print("sample_summary: alloc %.2f ms, sweeps %.2f ms, reductions %.2f ms" %
@@ -595,6 +601,9 @@ class AmwgSampler(Sampler):
             out[name] = {"mean": shape(mean[s0:s0 + ln]), "sd": shape(sd[s0:s0 + ln]), "rhat": shape(rhat[s0:s0 + ln]),
                          "quantiles": q[:, s0] if dim == [1] else q[:, s0:s0 + ln].reshape(len(q), *dim),
                          "n_draws": rows * self.n_chains}
+            if diagnostics:
+                for key, val in res[4][0].items():
+                    out[name][key] = shape(val[s0:s0 + ln])
         return out
 
     def start_adaptation(self):

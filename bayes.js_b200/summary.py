@@ -8,7 +8,8 @@ small collectives -- an all-gather of the per-rank moment records (merged exactl
 radix-select digit counts (integers) -- so every rank returns the same numbers as a single GPU holding all chains.
 
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
-amwg_summary_digit_hist). There is no CPU fallback: without the library or a GPU the reducer raises.
+amwg_summary_digit_hist, and amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True). There is no
+CPU fallback: without the library or a GPU the reducer raises.
 """
 from __future__ import annotations
 
@@ -133,7 +134,7 @@ class RadixSelect:
 
 # ---------------------------------------------------------------------------------------------------------------------
 class CudaBlockReducer:
-    """The two device reductions over a torch CUDA tensor block[rows, entries, chains] (fp64, contiguous)."""
+    """The device reductions over a torch CUDA tensor block[rows, entries, chains] (fp64, contiguous)."""
 
     def __init__(self, device: int):
         from . import _ffi
@@ -160,12 +161,180 @@ class CudaBlockReducer:
                                                        pre.data_ptr(), n_prefix, counts.data_ptr()))
         return counts
 
+    def autocov(self, block, thresholds, lag0: int, n_lags: int) -> np.ndarray:
+        """-> [entries, series, 4 + n_lags] split-chain records and lag sums of this shard (series: 1, or 3 with thresholds
+        [entries, 2]); see amwg_summary_autocov in include/amwg.h."""
+        rows, entries, chains = block.shape
+        ns = 1 if thresholds is None else 3
+        out = np.empty((entries, ns, 4 + n_lags), dtype=np.float64)
+        thr = None if thresholds is None else np.ascontiguousarray(thresholds, dtype=np.float64).reshape(entries, 2)
+        import torch
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_autocov(self.device, block.data_ptr(), rows, entries, chains,
+                                                    None if thr is None else thr.ctypes.data, lag0, n_lags, out.ctypes.data))
+        return out
 
-def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], distributed: bool):
+
+# ---------------------------------------------------------------------------------------------------------------------
+# split-chain effective sample size (Vehtari et al. 2021, §3; Stan's `ess` on split chains, ArviZ's method="mean"/"tail")
+MAX_LAGS = 32                          # include/amwg.h: n_lags <= 32 per amwg_summary_autocov call
+MIN_ROWS = 10                          # h = rows // 2 >= 5: Geyer's sequence can take at least one pair step
+
+
+def merge_autocov_records(records: Sequence[np.ndarray]) -> np.ndarray:
+    """Per-shard [entries, series, 4 + n] records in rank order -> one: moment part by merge_moment_records, lag sums added in
+    the order given."""
+    first = np.asarray(records[0], dtype=np.float64)
+    E, S, W = first.shape
+    mom = merge_moment_records([np.asarray(r, dtype=np.float64)[:, :, :4].reshape(E * S, 4) for r in records]).reshape(E, S, 4)
+    sums = np.array(first[:, :, 4:], copy=True)
+    for r in records[1:]:
+        sums = sums + np.asarray(r, dtype=np.float64)[:, :, 4:]
+    return np.concatenate([mom, sums], axis=2)
+
+
+class GeyerESS:
+    """ESS of one series from its merged split-chain record, one lag window at a time. Geyer's initial positive sequence and
+    then the initial monotone sequence, exactly as written in the docstring of `split_chain_diagnostics`. `need()` is the first
+    lag it has not got yet (None once done); `add(sums)` appends the lag sums of the next window."""
+
+    def __init__(self, record: np.ndarray, h: int):
+        M, _mean, m2, sum_w = np.asarray(record[:4], dtype=np.float64)        # numpy scalars: 0/0 is NaN, not an exception
+        self.h, self.M = h, M
+        with np.errstate(invalid="ignore", divide="ignore"):
+            self.W = sum_w / (M * (h - 1))                        # h/(h-1) * mean_m acov_m(0)
+            B = m2 / (M - 1)                                      # variance (ddof 1) of the half-chain means
+            self.varplus = (h - 1) / h * self.W + B
+        self.rho: List[float] = []
+        self.r = [1.0, 0.0]
+        self.ev, self.od, self.t = 1.0, None, 1
+        self.ess = None
+
+    def _rho(self, sums: np.ndarray) -> np.ndarray:
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return 1.0 - (self.W - np.asarray(sums, dtype=np.float64) / (self.M * self.h)) / self.varplus
+
+    def need(self):
+        return None if self.ess is not None else len(self.rho)
+
+    def add(self, sums: np.ndarray) -> None:
+        self.rho.extend(float(v) for v in self._rho(sums))
+        self._run()
+
+    def _run(self) -> None:
+        h, rho, r = self.h, self.rho, self.r
+        if self.od is None:
+            if len(rho) < 2:
+                return
+            self.od = rho[1]
+            r[1] = self.od
+        while self.t < h - 3 and self.ev + self.od > 0:
+            if self.t + 2 >= len(rho):
+                return                                            # the next pair is in the next lag window
+            ev, od = rho[self.t + 1], rho[self.t + 2]
+            self.ev, self.od = ev, od
+            r.extend([0.0] * (self.t + 3 - len(r)))
+            if ev + od >= 0:
+                r[self.t + 1], r[self.t + 2] = ev, od
+            self.t += 2
+        max_t = self.t - 2
+        r.extend([0.0] * (max_t + 2 - len(r)))
+        if self.ev > 0:
+            r[max_t + 1] = self.ev
+        t = 1
+        while t <= max_t - 2:
+            if r[t + 1] + r[t + 2] > r[t - 1] + r[t]:
+                r[t + 1] = r[t + 2] = (r[t - 1] + r[t]) / 2
+            t += 2
+        Mh = self.M * h
+        tau = -1.0 + 2.0 * sum(r[:max_t + 1]) + r[max_t + 1]
+        tau = max(tau, 1.0 / np.log10(Mh))
+        self.ess = Mh / tau
+
+
+def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.ndarray, hi: np.ndarray, vmin: np.ndarray,
+                            vmax: np.ndarray, distributed: bool, max_lags: int = MAX_LAGS):
+    """-> ({"ess_mean", "ess_tail", "mcse_mean", "rhat_split"} per entry, number of lag windows used).
+
+    Every chain is split into rows [0, h) and [rows-h, rows), h = rows // 2 (for odd rows the middle row is in neither half):
+    M = 2 * chains half-chains of h draws. For a series y, with acov_m(t) = (1/h) sum_{n<h-t} (y_mn - ybar_m)(y_m,n+t - ybar_m):
+    W = h/(h-1) mean_m acov_m(0), B = variance (ddof 1) of the ybar_m, var+ = (h-1)/h W + B, rho(t) = 1 - (W - mean_m acov_m(t)) / var+.
+    Geyer's initial positive sequence, then the initial monotone sequence, give tau; tau = max(tau, 1/log10(M h)); ESS = M h / tau.
+      ess_mean   ESS of the draws
+      ess_tail   min of the ESS of 1[x <= q05] and of 1[x <= q95] (lo, hi: the pooled exact quantiles; ties count as <=)
+      mcse_mean  sd / sqrt(ess_mean), sd the pooled sd
+      rhat_split sqrt(var+ / W) of the draws (not rank-normalised)
+    Edge cases: fewer than 10 rows (h < 5): all NaN. A constant entry (vmin == vmax) has ESS = M h and MCSE 0, and an indicator
+    that is constant (all 1 when the quantile equals the maximum) has ESS = M h. A non-finite minimum or maximum (an infinite or
+    NaN draw) makes all four values NaN.
+    Lag windows of at most `max_lags` lags are asked for only while some series' Geyer loop still needs a lag it has not got,
+    the way RadixSelect asks for its next pass. Distributed: each window's per-rank records are all-gathered and merged in rank
+    order, so every rank returns the same numbers."""
+    entries = block.shape[1]
+    h = rows // 2
+    nan = np.full(entries, np.nan)
+    out = {"ess_mean": nan.copy(), "ess_tail": nan.copy(), "mcse_mean": nan.copy(), "rhat_split": nan.copy()}
+    if rows < MIN_ROWS:
+        return out, 0
+    thr = np.stack([np.asarray(lo, dtype=np.float64), np.asarray(hi, dtype=np.float64)], axis=1)
+    est: List[List[GeyerESS]] = []
+    windows = 0
+    lag0 = 0
+    while True:
+        n_lags = min(max_lags, h - lag0)
+        rec = _gather_autocov(reducer.autocov(block, thr, lag0, n_lags), block, distributed)
+        windows += 1
+        if not est:
+            est = [[GeyerESS(rec[e, s], h) for s in range(3)] for e in range(entries)]
+        for e in range(entries):
+            for s in range(3):
+                if est[e][s].need() is not None:
+                    est[e][s].add(rec[e, s, 4:])
+        lag0 += n_lags
+        if all(g.need() is None for row in est for g in row) or lag0 >= h:
+            break
+    Mh = est[0][0].M * h
+    finite = np.isfinite(np.asarray(vmin, dtype=np.float64)) & np.isfinite(np.asarray(vmax, dtype=np.float64))
+    for e in range(entries):
+        if not finite[e]:
+            continue
+        const = (vmin[e] == vmax[e], thr[e, 0] >= vmax[e] or thr[e, 0] < vmin[e], thr[e, 1] >= vmax[e] or thr[e, 1] < vmin[e])
+        ess = [Mh if c else g.ess for g, c in zip(est[e], const)]
+        out["ess_mean"][e] = ess[0]
+        out["ess_tail"][e] = min(ess[1], ess[2])
+        with np.errstate(invalid="ignore", divide="ignore"):
+            out["mcse_mean"][e] = 0.0 if vmin[e] == vmax[e] else sd[e] / np.sqrt(ess[0])
+            out["rhat_split"][e] = np.sqrt(est[e][0].varplus / est[e][0].W)
+    return out, windows
+
+
+def _gather_autocov(rec: np.ndarray, block, distributed: bool) -> np.ndarray:
+    if not distributed:
+        return rec
+    import torch
+    import torch.distributed as dist
+    ws = dist.get_world_size()
+    mine = torch.from_numpy(np.ascontiguousarray(rec))
+    if block.is_cuda:
+        mine = mine.to(block.device)
+    gathered = torch.empty((ws * rec.shape[0],) + rec.shape[1:], dtype=mine.dtype, device=mine.device)
+    dist.all_gather_into_tensor(gathered, mine)
+    return merge_autocov_records(list(gathered.cpu().numpy().reshape((ws,) + rec.shape)))
+
+
+DIAGNOSTIC_PROBS = (0.0, 0.05, 0.95, 1.0)
+
+
+def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], distributed: bool, diagnostics: bool = False):
     """-> (mean, sd, rhat, quantiles[len(probs)]) per entry, over all shards. `reducer` does the per-shard device work;
-    the collectives run on the tensors it returns (NCCL for CUDA tensors, gloo for the CPU stand-in used in the tests)."""
+    the collectives run on the tensors it returns (NCCL for CUDA tensors, gloo for the CPU stand-in used in the tests).
+    diagnostics=True appends (split_chain_diagnostics' dict, lag windows used): the select also forms the minimum, q05, q95 and
+    the maximum (each quantile is its own order statistics, so the requested ones are unchanged)."""
     import torch
     entries = block.shape[1]
+    user_probs = [float(p) for p in probs]
+    if diagnostics:
+        probs = user_probs + list(DIAGNOSTIC_PROBS)
     rec = reducer.moments(block)
     if distributed:
         import torch.distributed as dist
@@ -195,4 +364,8 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
         vals = sel.values()                                   # [entries, T]
         for i, (lo, hi, g) in enumerate(plan):
             q[first + i] = _lerp(vals[:, lo], vals[:, hi], g)
-    return mean, sd, rhat, q
+    if not diagnostics:
+        return mean, sd, rhat, q
+    vmin, q05, q95, vmax = q[len(user_probs):]
+    diag = split_chain_diagnostics(reducer, block, rows, sd, q05, q95, vmin, vmax, distributed)
+    return mean, sd, rhat, q[:len(user_probs)], diag

@@ -272,10 +272,22 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   64-bit key of the draws: dev_counts[entry][prefix][256] += number of values of `entry` whose key's top 8*pass bits equal
  *   dev_prefix[entry][prefix] and whose next byte is the bin (pass 0 ignores the prefixes). Integer counts: exact and
  *   order-independent; the caller sums them over GPUs, picks the byte holding each wanted order statistic and extends the
- *   prefixes. n_prefix <= 32. */
+ *   prefixes. n_prefix <= 32.
+ *
+ * amwg_summary_autocov: split-chain autocovariances for the effective sample size and split R-hat (Vehtari et al. 2021, §3).
+ *   Every chain is split into rows [0, h) and rows [rows-h, rows), h = rows/2 (for odd rows the middle row is in neither half):
+ *   M = 2*chains half-chains of h draws. Series: the draws, plus, when host_thresholds[entry][2] is not null, the indicators
+ *   1[x <= thresholds[entry][0]] and 1[x <= thresholds[entry][1]] (all formed from one pass over the block). Each half-chain
+ *   is centred by its own mean. host_out[entry][series][4 + n_lags] = { M, mean of the half-chain means, M2 of the half-chain
+ *   means, sum over half-chains of sum_n d_n^2, then for t = lag0 .. lag0+n_lags-1 the sum over half-chains of
+ *   sum_{n<h-t} d_n d_{n+t} (= h * acov(t)) }. The first four merge like amwg_summary_moments' records, the lag sums add;
+ *   both are formed in a fixed order (deterministic). Errors: rows < 2, n_lags outside 1..32, lag0 + n_lags > h, null
+ *   dev_samples / host_out. */
 AMWG_API int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats);
 AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t pass,
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
+AMWG_API int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                  const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out);
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it

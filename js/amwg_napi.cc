@@ -12,6 +12,7 @@
 // `new mcmc.AmwgSampler(params, log_post, data, options)` (mcmc.js:1090-1092) while the stepping moves to the GPU.
 #include <node_api.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 #include <cstring>
@@ -355,6 +356,23 @@ BINDING(summary_digit_hist)
     fail_from_library();
   return js_undefined(env);
 END_BINDING
+// summary_autocov(device, samples ptr, rows, entries, chains, thresholds [entries][2] or null, lag0, n_lags)
+//   -> Float64Array [entries][series][4 + n_lags]                                                         amwg_summary_autocov
+BINDING(summary_autocov)
+  const int32_t entries = (int32_t)to_double(env, a.at(3));
+  const int32_t n_lags = (int32_t)to_double(env, a.at(7));
+  napi_valuetype t;
+  check(env, napi_typeof(env, a.at(5), &t), "typeof");
+  std::vector<double> thr;
+  if (t != napi_null && t != napi_undefined) thr = doubles(env, a.at(5));
+  if (!thr.empty() && thr.size() != (size_t)std::max(entries, 0) * 2) throw Throw{"summary_autocov: thresholds must hold [entries][2] numbers"};
+  const size_t series = thr.empty() ? 1 : 3;
+  std::vector<double> out((size_t)std::max(entries, 0) * series * (4 + (size_t)std::max(n_lags, 0)));
+  if (amwg_summary_autocov((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)), entries,
+                           (int64_t)to_double(env, a.at(4)), thr.empty() ? nullptr : thr.data(), (int64_t)to_double(env, a.at(6)), n_lags, out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
 // peak_fp64(device, reps) -> {tflops, ms}                                        amwg_peak_fp64
 BINDING(peak_fp64)
   double tf = 0.0, ms = 0.0;
@@ -400,7 +418,8 @@ NAPI_MODULE_INIT() {
       {"get_log_post", get_log_post}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
-      {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources},
+      {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
+      {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
     napi_value fn;
