@@ -13,6 +13,10 @@
 //   K_a1  amwg_autocov_kernel       : one thread per chain: split-chain (two halves) moment records and lag sums of the draws and
 //                                     of two tail indicators, for 16 lags per pass (effective sample size, split R-hat)
 //   K_a2  amwg_merge_sums_kernel    : one CTA per (entry, series, lag) sums the per-CTA lag sums in a FIXED order
+//   K_r0..K_r3  amwg_rank_hist / sort_count / sort_scan / sort_scatter : LSD radix sort of one entry's half-chain keys (8-bit
+//                                     digits, stable; digit positions equal in all keys skipped) for the rank-normalised diagnostics
+//   K_r4  amwg_rank_count_kernel    : merge-path rank counts of a sorted key array against another (integer, exact)
+//   K_r5  amwg_rank_z_kernel        : normal scores of the average ranks, scattered into a [2h][1][chains] z-block
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
 
@@ -300,6 +304,252 @@ __global__ void __launch_bounds__(256) amwg_merge_sums_kernel(const double* __re
   if (threadIdx.x == 0) out[row] = tot;
 }
 
+// ---- ranks over the pooled half-chain draws (rank-normalised R-hat, bulk effective sample size) -------------------------------
+// One entry at a time. Its n = 2h * chains half-chain draws are numbered i = r * chains + c, r < 2h: rows [0, h) are r = 0..h-1
+// and rows [rows-h, rows) are r = h..2h-1 (the middle row of odd rows is not ranked). A (key, i) pair per draw is sorted by an LSD
+// radix sort of 8-bit digits with a stable scatter; ties keep the order of i, so the result is fully determined.
+constexpr int kSortThreads = 256;
+constexpr int kSortItems = 8;
+constexpr int kSortTile = kSortThreads * kSortItems;           // keys per CTA in the count and scatter kernels
+constexpr int kMergeItems = 8;
+constexpr int kMergeTile = 256 * kMergeItems;                  // merged elements per CTA of the rank-count kernel
+
+// canonical rank key: ordered_key of x (bulk) or of |x - centre| (folded), with -0 made +0 so that the two zeros tie
+__device__ __forceinline__ unsigned long long rank_key(double x, bool folded, double centre) {
+  const double v = folded ? fabs(x - centre) : x;
+  return ordered_key(v == 0.0 ? 0.0 : v);
+}
+
+// Where a pass reads its (key, index) pairs: the first executed pass forms them from the block (index = i), later passes read
+// the previous pass's output.
+struct RankSource {
+  const double* x; long long rows, C; size_t stride; int e; bool folded; double centre;
+  const unsigned long long* keys; const unsigned* index;
+  template <bool FROM_BLOCK>
+  __device__ __forceinline__ void load(long long i, unsigned long long& k, unsigned& idx) const {
+    if constexpr (FROM_BLOCK) {
+      const long long h = rows / 2, r = i / C, c = i - r * C;
+      k = rank_key(x[(size_t)(r < h ? r : rows - 2 * h + r) * stride + (size_t)e * C + c], folded, centre);
+      idx = (unsigned)i;
+    } else {
+      k = keys[i];
+      idx = index[i];
+    }
+  }
+};
+
+// K_r0: the eight digit histograms of one entry's keys, from one read of the block (hist[digit position][256], position 0 the
+// least significant byte). Per thread, a run of equal bins is counted in a register (the high bytes of one parameter's draws
+// rarely change) and added to the shared histogram once per run.
+__global__ void __launch_bounds__(256) amwg_rank_hist_kernel(RankSource src, long long n, unsigned long long* __restrict__ hist) {
+  __shared__ unsigned sh[8 * 256];
+  for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) sh[i] = 0u;
+  __syncthreads();
+  int last[8];
+  unsigned run[8];
+#pragma unroll
+  for (int d = 0; d < 8; ++d) { last[d] = -1; run[d] = 0u; }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    unsigned long long k;
+    unsigned idx;
+    src.load<true>(i, k, idx);
+#pragma unroll
+    for (int d = 0; d < 8; ++d) {
+      const int b = d * 256 + (int)((k >> (8 * d)) & 255ull);
+      if (b == last[d]) { ++run[d]; continue; }
+      if (last[d] >= 0) atomicAdd(&sh[last[d]], run[d]);
+      last[d] = b; run[d] = 1u;
+    }
+  }
+#pragma unroll
+  for (int d = 0; d < 8; ++d)
+    if (last[d] >= 0) atomicAdd(&sh[last[d]], run[d]);
+  __syncthreads();
+  for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x)
+    if (sh[i]) atomicAdd(&hist[i], (unsigned long long)sh[i]);
+}
+
+// every pass skipped (all keys equal): the keys in input order
+__global__ void __launch_bounds__(256) amwg_rank_fill_kernel(RankSource src, long long n, unsigned long long* __restrict__ keys,
+                                                             unsigned* __restrict__ index) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    src.load<true>(i, keys[i], index[i]);
+}
+
+__device__ __forceinline__ int sort_digit(unsigned long long k, int shift) { return (int)((k >> shift) & 255ull); }
+
+// K_r1 (upsweep): counts[digit][tile] of one pass's digit among the keys of each tile of kSortTile keys
+template <bool FROM_BLOCK>
+__global__ void __launch_bounds__(kSortThreads) amwg_sort_count_kernel(RankSource src, long long n, int shift, unsigned* __restrict__ counts) {
+  __shared__ unsigned sh[256];
+  const long long tiles = gridDim.x, tile = blockIdx.x, base = tile * kSortTile;
+  sh[threadIdx.x] = 0u;
+  __syncthreads();
+  const unsigned lane = threadIdx.x & 31u;
+#pragma unroll
+  for (int j = 0; j < kSortItems; ++j) {
+    const long long i = base + j * kSortThreads + threadIdx.x;
+    int d = 256;                                               // 256: past the end, counted nowhere
+    if (i < n) { unsigned long long k; unsigned idx; src.load<FROM_BLOCK>(i, k, idx); d = sort_digit(k, shift); }
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    if (d < 256 && lane == (unsigned)(__ffs(peers) - 1)) atomicAdd(&sh[d], (unsigned)__popc(peers));
+  }
+  __syncthreads();
+  counts[(size_t)threadIdx.x * tiles + tile] = sh[threadIdx.x];
+}
+
+// K_r2 (scan): one CTA per digit turns counts[digit][tile] into the global position of the tile's first key of that digit:
+// (keys of smaller digits, from the pass's histogram) + (keys of this digit in earlier tiles)
+__global__ void __launch_bounds__(1024) amwg_sort_scan_kernel(const unsigned* __restrict__ counts, long long tiles,
+                                                              const unsigned long long* __restrict__ hist, unsigned* __restrict__ offsets) {
+  __shared__ unsigned long long sh[1024];
+  const int d = blockIdx.x, t = threadIdx.x;
+  unsigned long long below = 0;
+  for (int b = t; b < d; b += 1024) below += hist[b];
+  const long long per = (tiles + 1023) / 1024, lo = t * per, hi = lo + per < tiles ? lo + per : tiles;
+  unsigned long long mine = 0;
+  for (long long i = lo; i < hi; ++i) mine += counts[(size_t)d * tiles + i];
+  sh[t] = below;
+  __syncthreads();
+  for (int w = 512; w > 0; w >>= 1) { if (t < w) sh[t] += sh[t + w]; __syncthreads(); }
+  const unsigned long long start = sh[0];
+  __syncthreads();
+  sh[t] = mine;                                                // inclusive Hillis-Steele scan of the per-thread sums
+  __syncthreads();
+  for (int w = 1; w < 1024; w <<= 1) {
+    const unsigned long long v = t >= w ? sh[t - w] : 0ull;
+    __syncthreads();
+    sh[t] += v;
+    __syncthreads();
+  }
+  unsigned long long run = start + sh[t] - mine;
+  for (long long i = lo; i < hi; ++i) {
+    const unsigned c = counts[(size_t)d * tiles + i];
+    offsets[(size_t)d * tiles + i] = (unsigned)run;
+    run += c;
+  }
+}
+
+// K_r3 (downsweep): every tile ranks its keys stably by digit (rounds of 256 keys in input order; within a round, warp-level
+// matching gives each key its place among equal digits), reorders them in shared memory and writes each digit's keys as one
+// contiguous run at the tile's offset for that digit.
+template <bool FROM_BLOCK>
+__global__ void __launch_bounds__(kSortThreads) amwg_sort_scatter_kernel(RankSource src, long long n, int shift,
+                                                                         const unsigned* __restrict__ counts, const unsigned* __restrict__ offsets,
+                                                                         unsigned long long* __restrict__ keys_out, unsigned* __restrict__ index_out) {
+  __shared__ unsigned long long sk[kSortTile];
+  __shared__ unsigned si[kSortTile];
+  __shared__ unsigned warp_cnt[kSortThreads / 32][256];
+  __shared__ unsigned warp_off[kSortThreads / 32][256];
+  __shared__ unsigned start[256];                              // first local position of each digit in the tile
+  __shared__ unsigned seen[256];                               // keys of each digit placed by earlier rounds
+  __shared__ long long dest[256];                              // global position of local position start[d]
+  const long long tiles = gridDim.x, tile = blockIdx.x, base = tile * kSortTile;
+  const int t = threadIdx.x, w = t >> 5;
+  const unsigned lane = t & 31u, lt = (1u << lane) - 1u;
+  {
+    const unsigned c = counts[(size_t)t * tiles + tile];
+    start[t] = c;
+    __syncthreads();
+    for (int s = 1; s < 256; s <<= 1) {                        // inclusive scan of the tile's digit counts
+      const unsigned v = t >= s ? start[t - s] : 0u;
+      __syncthreads();
+      start[t] += v;
+      __syncthreads();
+    }
+    const unsigned st = start[t] - c;
+    __syncthreads();
+    start[t] = st;
+    seen[t] = 0u;
+    dest[t] = (long long)offsets[(size_t)t * tiles + tile] - (long long)st;
+    for (int v = 0; v < kSortThreads / 32; ++v) warp_cnt[v][t] = 0u;
+  }
+  __syncthreads();
+#pragma unroll 1
+  for (int j = 0; j < kSortItems; ++j) {
+    const long long i = base + j * kSortThreads + t;
+    unsigned long long k = 0;
+    unsigned idx = 0;
+    int d = 256;
+    if (i < n) { src.load<FROM_BLOCK>(i, k, idx); d = sort_digit(k, shift); }
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    const unsigned rank = __popc(peers & lt);
+    if (d < 256 && rank == 0) warp_cnt[w][d] = __popc(peers);
+    __syncthreads();
+    unsigned run = seen[t];                                    // thread t owns digit t: exclusive prefix over the warps
+#pragma unroll
+    for (int v = 0; v < kSortThreads / 32; ++v) { const unsigned c = warp_cnt[v][t]; warp_off[v][t] = run; run += c; warp_cnt[v][t] = 0u; }
+    seen[t] = run;
+    __syncthreads();
+    if (d < 256) {
+      const unsigned pos = start[d] + warp_off[w][d] + rank;
+      sk[pos] = k;
+      si[pos] = idx;
+    }
+  }
+  __syncthreads();
+  const long long m = n - base < kSortTile ? n - base : kSortTile;
+  for (int p = t; p < m; p += kSortThreads) {
+    const unsigned long long k = sk[p];
+    const long long g = dest[sort_digit(k, shift)] + p;
+    keys_out[g] = k;
+    index_out[g] = si[p];
+  }
+}
+
+// K_r4: rank counts by merge path. acc[i] += #(R < Q[i]) (UPPER = false: Q first on ties) or #(R <= Q[i]) (UPPER = true: R
+// first). Every CTA takes kMergeTile consecutive elements of the merged sequence; its share of Q and R is found by a binary
+// search on the two cross diagonals, staged in shared memory, and merged there kMergeItems elements per thread.
+template <bool UPPER>
+__device__ __forceinline__ bool q_first(unsigned long long q, unsigned long long r) { return UPPER ? q < r : q <= r; }
+
+template <bool UPPER>
+__device__ __forceinline__ long long merge_path(const unsigned long long* Q, long long nq, const unsigned long long* R, long long nr, long long diag) {
+  long long lo = diag > nr ? diag - nr : 0, hi = diag < nq ? diag : nq;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (q_first<UPPER>(Q[mid], R[diag - 1 - mid])) lo = mid + 1; else hi = mid;
+  }
+  return lo;                                                   // elements of Q among the first `diag` of the merge
+}
+
+template <bool UPPER>
+__global__ void __launch_bounds__(256) amwg_rank_count_kernel(const unsigned long long* __restrict__ Q, long long nq,
+                                                              const unsigned long long* __restrict__ R, long long nr, long long* __restrict__ acc) {
+  __shared__ unsigned long long s[kMergeTile];                 // Q's share at [0, na), R's at [na, na + nb)
+  __shared__ long long cnt[kMergeTile];
+  __shared__ long long bounds[2];
+  const long long d0 = (long long)blockIdx.x * kMergeTile, total = nq + nr;
+  const long long d1 = d0 + kMergeTile < total ? d0 + kMergeTile : total;
+  if (threadIdx.x < 2) bounds[threadIdx.x] = merge_path<UPPER>(Q, nq, R, nr, threadIdx.x ? d1 : d0);
+  __syncthreads();
+  const long long a0 = bounds[0], a1 = bounds[1], b0 = d0 - a0, b1 = d1 - a1;
+  const int na = (int)(a1 - a0), nb = (int)(b1 - b0);
+  for (int i = threadIdx.x; i < na + nb; i += blockDim.x) s[i] = i < na ? Q[a0 + i] : R[b0 + i - na];
+  __syncthreads();
+  const int diag = threadIdx.x * kMergeItems;
+  if (diag < na + nb) {
+    const unsigned long long* sq = s;
+    const unsigned long long* sr = s + na;
+    int i = (int)merge_path<UPPER>(sq, na, sr, nb, diag), j = diag - i;
+    for (int step = 0; step < kMergeItems && i + j < na + nb; ++step) {
+      if (i < na && (j >= nb || q_first<UPPER>(sq[i], sr[j]))) { cnt[i] = b0 + j; ++i; }
+      else ++j;
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < na; i += blockDim.x) acc[a0 + i] += cnt[i];
+}
+
+// K_r5: z = Phi^-1((r - 3/8) / (S + 1/4)) with the average rank r = (acc + 1) / 2, written at the draw's place in the z-block
+__global__ void __launch_bounds__(256) amwg_rank_z_kernel(const long long* __restrict__ acc, const unsigned* __restrict__ index, long long n,
+                                                          double total, double* __restrict__ z) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const double r = (double)(acc[i] + 1) * 0.5;
+    z[index[i]] = normcdfinv((r - 0.375) / (total + 0.25));
+  }
+}
+
 }  // namespace summary
 
 extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats) {
@@ -411,5 +661,105 @@ extern "C" int amwg_summary_autocov(int device, const double* dev_samples, int64
     for (int i = 0; i < 4; ++i) host_out[r * w + i] = mom[r * 4 + i];
     for (int k = 0; k < n_lags; ++k) host_out[r * w + 4 + k] = sm[r * n_lags + k];
   }
+  return 0;
+}
+
+extern "C" int amwg_summary_rank_sort(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t entry,
+                                      double centre, uint64_t* dev_keys, uint32_t* dev_index, int32_t* host_passes) {
+  if (rows < 2) return fail("amwg_summary_rank_sort: rows must be at least 2 (two half-chains of one draw)");
+  if (entries <= 0 || chains <= 0) return fail("amwg_summary_rank_sort: empty sample block");
+  if (entry < 0 || entry >= entries) return fail("amwg_summary_rank_sort: entry outside [0, entries)");
+  const int64_t n = 2 * (rows / 2) * chains;
+  if (n >= ((int64_t)1 << 32) || chains >= ((int64_t)1 << 32))
+    return fail("amwg_summary_rank_sort: 2 * (rows / 2) * chains = " + std::to_string(n) + " draws, the indices hold fewer than 2^32");
+  if (!dev_samples || !dev_keys || !dev_index) return fail("amwg_summary_rank_sort: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_rank_sort: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const long long tiles = (n + summary::kSortTile - 1) / summary::kSortTile;
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t b_hist = up(8 * 256 * sizeof(unsigned long long)), b_tab = up((size_t)256 * tiles * sizeof(unsigned));
+  const size_t need = b_hist + 2 * b_tab;
+  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
+  struct Scratch { void* p = nullptr; size_t bytes = 0; };
+  static Scratch scratch[64];
+  static std::mutex scratch_mu;
+  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the last pass
+  Scratch& sc = scratch[device];
+  if (sc.bytes < need) {
+    if (sc.p) cudaFree(sc.p);
+    sc.p = nullptr; sc.bytes = 0;
+    CUDA_TRY(cudaMalloc(&sc.p, need));
+    sc.bytes = need;
+  }
+  char* base = reinterpret_cast<char*>(sc.p);
+  auto* hist = reinterpret_cast<unsigned long long*>(base);
+  auto* counts = reinterpret_cast<unsigned*>(base + b_hist);
+  auto* offsets = reinterpret_cast<unsigned*>(base + b_hist + b_tab);
+  auto* keys = reinterpret_cast<unsigned long long*>(dev_keys);
+  summary::RankSource src{dev_samples, rows, chains, (size_t)entries * chains, entry, !std::isnan(centre), centre, nullptr, nullptr};
+  CUDA_TRY(cudaMemset(hist, 0, 8 * 256 * sizeof(unsigned long long)));
+  // one read of the block forms all eight digit histograms. A digit position where one bin holds every key has the same digit
+  // in all keys: its pass would move nothing and is skipped. The first executed pass forms the keys from the block again, into
+  // the half that makes the last pass end in the first half.
+  const unsigned gx = (unsigned)std::min<long long>((n + 255) / 256, summary::kChainCtas);
+  summary::amwg_rank_hist_kernel<<<gx, 256>>>(src, n, hist);
+  CUDA_TRY(cudaGetLastError());
+  std::vector<unsigned long long> h(8 * 256);
+  CUDA_TRY(cudaMemcpy(h.data(), hist, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  std::vector<int> run;
+  for (int d = 0; d < 8; ++d)
+    if (*std::max_element(h.begin() + d * 256, h.begin() + (d + 1) * 256) != (unsigned long long)n) run.push_back(d);
+  if (run.empty()) summary::amwg_rank_fill_kernel<<<gx, 256>>>(src, n, keys, dev_index);
+  int dst = run.size() % 2 ? 0 : 1;
+  for (size_t p = 0; p < run.size(); ++p) {
+    const int d = run[p];
+    const unsigned tg = (unsigned)tiles;
+    if (p == 0) {
+      summary::amwg_sort_count_kernel<true><<<tg, summary::kSortThreads>>>(src, n, 8 * d, counts);
+      summary::amwg_sort_scan_kernel<<<256, 1024>>>(counts, tiles, hist + d * 256, offsets);
+      summary::amwg_sort_scatter_kernel<true><<<tg, summary::kSortThreads>>>(src, n, 8 * d, counts, offsets, keys + dst * n, dev_index + dst * n);
+    } else {
+      summary::RankSource prev = src;
+      prev.keys = keys + (1 - dst) * n;
+      prev.index = dev_index + (1 - dst) * n;
+      summary::amwg_sort_count_kernel<false><<<tg, summary::kSortThreads>>>(prev, n, 8 * d, counts);
+      summary::amwg_sort_scan_kernel<<<256, 1024>>>(counts, tiles, hist + d * 256, offsets);
+      summary::amwg_sort_scatter_kernel<false><<<tg, summary::kSortThreads>>>(prev, n, 8 * d, counts, offsets, keys + dst * n, dev_index + dst * n);
+    }
+    dst = 1 - dst;
+  }
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  if (host_passes) *host_passes = (int32_t)run.size();
+  return 0;
+}
+
+extern "C" int amwg_summary_rank_count(int device, const uint64_t* dev_q, int64_t nq, const uint64_t* dev_r, int64_t nr, int64_t* dev_acc) {
+  if (nq < 1 || nr < 1) return fail("amwg_summary_rank_count: empty key array");
+  if (nq >= ((int64_t)1 << 32) || nr >= ((int64_t)1 << 32)) return fail("amwg_summary_rank_count: more than 2^32 - 1 keys");
+  if (!dev_q || !dev_r || !dev_acc) return fail("amwg_summary_rank_count: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_rank_count: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const unsigned grid = (unsigned)((nq + nr + summary::kMergeTile - 1) / summary::kMergeTile);
+  auto* q = reinterpret_cast<const unsigned long long*>(dev_q);
+  auto* r = reinterpret_cast<const unsigned long long*>(dev_r);
+  auto* acc = reinterpret_cast<long long*>(dev_acc);
+  summary::amwg_rank_count_kernel<false><<<grid, 256>>>(q, nq, r, nr, acc);
+  summary::amwg_rank_count_kernel<true><<<grid, 256>>>(q, nq, r, nr, acc);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+extern "C" int amwg_summary_rank_z(int device, const int64_t* dev_acc, const uint32_t* dev_index, int64_t n, int64_t total, double* dev_z) {
+  if (n < 1 || n >= ((int64_t)1 << 32)) return fail("amwg_summary_rank_z: n must be 1..2^32-1");
+  if (total < n || total >= ((int64_t)1 << 52)) return fail("amwg_summary_rank_z: total must be at least n and below 2^52");
+  if (!dev_acc || !dev_index || !dev_z) return fail("amwg_summary_rank_z: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_rank_z: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, summary::kChainCtas);
+  summary::amwg_rank_z_kernel<<<grid, 256>>>(reinterpret_cast<const long long*>(dev_acc), dev_index, n, (double)total, dev_z);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
   return 0;
 }

@@ -554,9 +554,15 @@ class AmwgSampler(Sampler):
         sizes of the draws and of the 5 % / 95 % tail indicators, Vehtari et al. 2021), "mcse_mean" (sd / sqrt(ess_mean)) and
         "rhat_split" (split-chain R-hat, not rank-normalised); the other keys keep their values bit for bit. Fewer than 10 kept
         rows give NaN; see summary.split_chain_diagnostics for the estimator and its edge cases. All chains start from the same
-        init, so "rhat" and "rhat_split" only mean something after burn-in."""
+        init, so "rhat" and "rhat_split" only mean something after burn-in.
+        diagnostics="rank" returns everything diagnostics=True does, bit for bit, plus "ess_bulk" (ESS of the rank-normalised
+        split chains) and "rhat_rank" (the larger split R-hat of the rank-normalised draws and of the rank-normalised folded draws
+        |x - median|), ranked over the pooled draws of all chains on all GPUs (Vehtari et al. 2021, §4; the numbers Stan and
+        ArviZ print). They stay finite with +-inf draws and catch chains that differ in scale only; see summary.rank_diagnostics.
+        Ranking needs 56 bytes of device scratch per ranked draw for one parameter entry at a time. Any other value raises."""
         import torch
-        from .summary import CudaBlockReducer, summarise_block
+        from .summary import CudaBlockReducer, check_diagnostics, summarise_block
+        check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
         spans = {}
@@ -575,6 +581,15 @@ class AmwgSampler(Sampler):
         free, _total = torch.cuda.mem_get_info(dev)
         if need + 2 * len(entries) * self.local_chains * 8 > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
+        if diagnostics == "rank" and rows >= 10:
+            # rank_diagnostics, per entry: keys 2 x 8 B, indices 2 x 4 B, rank sums 8 B, a ring buffer 8 B and two z-blocks 2 x 8 B per
+            # ranked draw (the ring buffers hold the largest shard, at most one chain more than this one), and the sort's tile
+            # tables (2 x 256 x 4 B per 2048 keys)
+            ranked = 2 * (rows // 2) * (self.local_chains + (1 if self.distributed else 0))
+            scratch = 56 * ranked + 2 * 256 * 4 * (-(-ranked // 2048))
+            if need + 2 * len(entries) * self.local_chains * 8 + scratch > 0.9 * free:
+                raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
+                              "device memory; raise thin() or lower n" % (need / 1e9, scratch / 1e9))
         timing = os.environ.get("AMWG_SUMMARY_TIMING") == "1"
         t0 = time.perf_counter()
         block = torch.empty((rows, len(entries), self.local_chains), dtype=torch.float64, device=dev)

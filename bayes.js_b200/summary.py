@@ -8,7 +8,8 @@ small collectives -- an all-gather of the per-rank moment records (merged exactl
 radix-select digit counts (integers) -- so every rank returns the same numbers as a single GPU holding all chains.
 
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
-amwg_summary_digit_hist, and amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True). There is no
+amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True, and
+amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank"). There is no
 CPU fallback: without the library or a GPU the reducer raises.
 """
 from __future__ import annotations
@@ -174,6 +175,30 @@ class CudaBlockReducer:
                                                     None if thr is None else thr.ctypes.data, lag0, n_lags, out.ctypes.data))
         return out
 
+    def rank_sort(self, block, entry: int, centre: float, keys, index) -> int:
+        """Sorts the half-chain keys of `entry` (centre NaN: the draws; else |x - centre|) into keys[:n] (int64 tensor holding the
+        uint64 keys, 2n long) with their positions in index[:n] (int32 tensor, 2n long); -> radix passes run. See
+        amwg_summary_rank_sort in include/amwg.h."""
+        import torch
+        rows, entries, chains = block.shape
+        passes = C.c_int32(0)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_rank_sort(self.device, block.data_ptr(), rows, entries, chains, entry, centre,
+                                                      keys.data_ptr(), index.data_ptr(), C.byref(passes)))
+        return passes.value
+
+    def rank_count(self, q, nq: int, r, nr: int, acc) -> None:
+        """acc[:nq] += #(r[:nr] < q[i]) + #(r[:nr] <= q[i]) for sorted key tensors q and r."""
+        import torch
+        torch.cuda.current_stream(acc.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_rank_count(self.device, q.data_ptr(), nq, r.data_ptr(), nr, acc.data_ptr()))
+
+    def rank_z(self, acc, index, n: int, total: int, z) -> None:
+        """z.view(-1)[index[i]] = Phi^-1(((acc[i] + 1) / 2 - 3/8) / (total + 1/4)) for i < n."""
+        import torch
+        torch.cuda.current_stream(acc.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_rank_z(self.device, acc.data_ptr(), index.data_ptr(), n, total, z.data_ptr()))
+
 
 # ---------------------------------------------------------------------------------------------------------------------
 # split-chain effective sample size (Vehtari et al. 2021, §3; Stan's `ess` on split chains, ArviZ's method="mean"/"tail")
@@ -322,19 +347,144 @@ def _gather_autocov(rec: np.ndarray, block, distributed: bool) -> np.ndarray:
     return merge_autocov_records(list(gathered.cpu().numpy().reshape((ws,) + rec.shape)))
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# rank-normalised split R-hat and bulk ESS (Vehtari et al. 2021, §4; what Stan, ArviZ and posterior print by default)
+def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarray, vmax: np.ndarray, distributed: bool,
+                     max_lags: int = MAX_LAGS) -> dict:
+    """-> {"ess_bulk", "rhat_rank"} per entry; vmin / vmax are the exact smallest and largest kept draws (a NaN draw makes one
+    of them NaN: its key lies below -inf's or above +inf's).
+
+    The halves are those of `split_chain_diagnostics`: h = rows // 2, rows [0, h) and [rows-h, rows) of every chain (for odd
+    rows the middle row is in neither half and is not ranked). S = 2 h * (chains over all GPUs) draws per entry are ranked
+    together. r(x) is the average rank of x among them (1-based, ties averaged, as scipy.stats.rankdata(method="average")),
+    with -0.0 and +0.0 equal, and z = Phi^-1((r - 3/8) / (S + 1/4)). The folded draws f = |x - med|, med the pooled exact 0.5
+    quantile over all kept rows (numpy.quantile's rule), are ranked and z-scaled the same way into z_f.
+      ess_bulk   the ESS of z, by the estimator of `split_chain_diagnostics` (Geyer's initial positive, then initial monotone
+                 sequence over the split-chain autocorrelations of z)
+      rhat_rank  max(sqrt(var+ / W) of z, sqrt(var+ / W) of z_f), var+ and W as in `split_chain_diagnostics`
+    Edge cases: fewer than 10 rows: NaN. A NaN draw anywhere in the kept rows (vmin or vmax NaN): both NaN. +-inf draws are
+    ranked like any other value, so both stay finite. A constant entry (all ranked draws equal): ess_bulk = M h (M = 2 * chains),
+    rhat_rank NaN. A constant folded series (for example draws +-1 with median 0): rhat_rank is the R-hat of z alone. med not
+    finite (+-inf, or NaN when numpy.quantile's rule interpolates towards an infinite draw): rhat_rank NaN.
+    Device work per entry and series (CudaBlockReducer): a radix sort of the shard's keys, rank counts against every shard's
+    sorted keys, and z written into a [2h][1][chains] block that amwg_summary_autocov splits into exactly the ranked halves.
+    Distributed: the sorted key arrays travel around a ring of torch.distributed send / recv (W - 1 steps, two buffers); the
+    counts are integers, so the ranks and z do not depend on the number of GPUs. The autocovariance records of z merge across
+    ranks as in `split_chain_diagnostics`, so every rank returns the same numbers."""
+    import torch
+    entries, chains = block.shape[1], block.shape[2]
+    h = rows // 2
+    out = {"ess_bulk": np.full(entries, np.nan), "rhat_rank": np.full(entries, np.nan)}
+    if rows < MIN_ROWS:
+        return out
+    dev = block.device
+    n = 2 * h * chains
+    sizes = _gather_ints([n], block, distributed)[:, 0]
+    total = int(sizes.sum())
+    M = total // h
+    keys = torch.empty(n + int(sizes.max()), dtype=torch.int64, device=dev)     # sorted keys + the sort's scratch / a ring buffer
+    index = torch.empty(2 * n, dtype=torch.int32, device=dev)
+    acc = torch.empty(n, dtype=torch.int64, device=dev)
+    ring = torch.empty(int(sizes.max()), dtype=torch.int64, device=dev)
+    z = torch.empty((2, 2 * h, 1, chains), dtype=torch.float64, device=dev)
+
+    def ranked(e: int, centre: float, zb) -> bool:
+        """z-scaled ranks of one series into zb; -> whether all its keys are equal over all shards."""
+        reducer.rank_sort(block, e, centre, keys, index)
+        ends = keys[[0, n - 1]].cpu().numpy().view(np.uint64)
+        ends = _gather_ints(ends.view(np.int64), block, distributed).view(np.uint64)
+        acc.zero_()
+        _ring_counts(reducer, keys, n, sizes, acc, ring, distributed)
+        reducer.rank_z(acc, index, n, total, zb)
+        return bool(ends[:, 0].min() == ends[:, 1].max())
+
+    def records(zb, lag0: int, n_lags: int) -> np.ndarray:
+        return _gather_autocov(reducer.autocov(zb, None, lag0, n_lags), zb, distributed)[0, 0]
+
+    for e in range(entries):
+        if np.isnan(vmin[e]) or np.isnan(vmax[e]):
+            continue
+        if vmin[e] == vmax[e] or ranked(e, float("nan"), z[0]):
+            out["ess_bulk"][e] = M * h
+            continue
+        rec = records(z[0], 0, min(max_lags, h))
+        g = GeyerESS(rec, h)
+        g.add(rec[4:])
+        lag0 = len(g.rho)
+        while g.need() is not None and lag0 < h:
+            n_lags = min(max_lags, h - lag0)
+            g.add(records(z[0], lag0, n_lags)[4:])
+            lag0 += n_lags
+        out["ess_bulk"][e] = g.ess
+        with np.errstate(invalid="ignore", divide="ignore"):
+            rhat = np.sqrt(g.varplus / g.W)
+            if not np.isfinite(med[e]):
+                continue
+            if ranked(e, float(med[e]), z[1]):
+                out["rhat_rank"][e] = rhat
+                continue
+            gf = GeyerESS(records(z[1], 0, 1), h)
+            out["rhat_rank"][e] = max(rhat, np.sqrt(gf.varplus / gf.W))
+    return out
+
+
+def _gather_ints(vals, block, distributed: bool) -> np.ndarray:
+    """int64 values of this rank -> [world, len(vals)] in rank order ([1, len] when not distributed)."""
+    mine = np.asarray(vals, dtype=np.int64).reshape(1, -1)
+    if not distributed:
+        return mine
+    import torch
+    import torch.distributed as dist
+    ws = dist.get_world_size()
+    t = torch.from_numpy(np.ascontiguousarray(mine[0]))
+    if block.is_cuda:
+        t = t.to(block.device)
+    gathered = torch.empty(ws * t.numel(), dtype=torch.int64, device=t.device)
+    dist.all_gather_into_tensor(gathered, t)
+    return gathered.cpu().numpy().reshape(ws, -1)
+
+
+def _ring_counts(reducer, keys, n: int, sizes: np.ndarray, acc, ring, distributed: bool) -> None:
+    """acc += the rank counts of this shard's sorted keys[:n] against every shard's sorted keys: its own first, then the others
+    as they come round the ring (step s brings the keys of rank - s, sent on by the ranks in between)."""
+    reducer.rank_count(keys, n, keys, n, acc)
+    if not distributed:
+        return
+    import torch.distributed as dist
+    ws, rank = dist.get_world_size(), dist.get_rank()
+    bufs = (keys[n:], ring)
+    cur = keys[:n]
+    for step in range(1, ws):
+        src = (rank - step) % ws
+        recv = bufs[(step - 1) % 2][:int(sizes[src])]
+        ops = [dist.P2POp(dist.isend, cur, (rank + 1) % ws), dist.P2POp(dist.irecv, recv, (rank - 1) % ws)]
+        for req in dist.batch_isend_irecv(ops):
+            req.wait()
+        reducer.rank_count(keys, n, recv, int(sizes[src]), acc)
+        cur = recv
+
+
 DIAGNOSTIC_PROBS = (0.0, 0.05, 0.95, 1.0)
+RANK_PROBS = (0.5,)                   # the median that centres the folded draws of diagnostics="rank"
 
 
-def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], distributed: bool, diagnostics: bool = False):
+def check_diagnostics(diagnostics) -> None:
+    if not (isinstance(diagnostics, bool) or (isinstance(diagnostics, str) and diagnostics == "rank")):
+        raise ValueError("diagnostics must be False, True or \"rank\", not %r" % (diagnostics,))
+
+
+def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], distributed: bool, diagnostics=False):
     """-> (mean, sd, rhat, quantiles[len(probs)]) per entry, over all shards. `reducer` does the per-shard device work;
     the collectives run on the tensors it returns (NCCL for CUDA tensors, gloo for the CPU stand-in used in the tests).
     diagnostics=True appends (split_chain_diagnostics' dict, lag windows used): the select also forms the minimum, q05, q95 and
-    the maximum (each quantile is its own order statistics, so the requested ones are unchanged)."""
+    the maximum (each quantile is its own order statistics, so the requested ones are unchanged). diagnostics="rank" also forms
+    the median and adds rank_diagnostics' "ess_bulk" and "rhat_rank" to that dict; every other value is the same bits."""
     import torch
+    check_diagnostics(diagnostics)
     entries = block.shape[1]
     user_probs = [float(p) for p in probs]
     if diagnostics:
-        probs = user_probs + list(DIAGNOSTIC_PROBS)
+        probs = user_probs + list(DIAGNOSTIC_PROBS) + (list(RANK_PROBS) if diagnostics == "rank" else [])
     rec = reducer.moments(block)
     if distributed:
         import torch.distributed as dist
@@ -349,6 +499,7 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
 
     probs = [float(p) for p in probs]
     q = np.empty((len(probs), entries))
+    low = np.empty((len(probs), entries))                     # the lower order statistic of each probability, not interpolated
     per_select = MAX_PREFIXES // 2                            # every probability needs at most two order statistics
     for first in range(0, len(probs), per_select):            # long probability grids (equal-mass histograms): several selects
         chunk = probs[first:first + per_select]
@@ -364,8 +515,13 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
         vals = sel.values()                                   # [entries, T]
         for i, (lo, hi, g) in enumerate(plan):
             q[first + i] = _lerp(vals[:, lo], vals[:, hi], g)
+            low[first + i] = vals[:, lo]
     if not diagnostics:
         return mean, sd, rhat, q
-    vmin, q05, q95, vmax = q[len(user_probs):]
+    vmin, q05, q95, vmax = q[len(user_probs):len(user_probs) + len(DIAGNOSTIC_PROBS)]
     diag = split_chain_diagnostics(reducer, block, rows, sd, q05, q95, vmin, vmax, distributed)
+    if diagnostics == "rank":
+        # the exact minimum and maximum: interpolating an infinite extreme with itself gives NaN, and these must tell +-inf from NaN
+        lo_min, lo_max = low[len(user_probs)], low[len(user_probs) + 3]
+        diag[0].update(rank_diagnostics(reducer, block, rows, q[-1], lo_min, lo_max, distributed))
     return mean, sd, rhat, q[:len(user_probs)], diag

@@ -282,12 +282,33 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   means, sum over half-chains of sum_n d_n^2, then for t = lag0 .. lag0+n_lags-1 the sum over half-chains of
  *   sum_{n<h-t} d_n d_{n+t} (= h * acov(t)) }. The first four merge like amwg_summary_moments' records, the lag sums add;
  *   both are formed in a fixed order (deterministic). Errors: rows < 2, n_lags outside 1..32, lag0 + n_lags > h, null
- *   dev_samples / host_out. */
+ *   dev_samples / host_out.
+ *
+ * Ranks over the pooled half-chain draws (rank-normalised R-hat and bulk ESS, Vehtari et al. 2021, §4). One entry per call; the
+ * caller owns every device buffer (keys, indices, rank sums, z-block), so the three calls keep no state between them.
+ * amwg_summary_rank_sort: sorts the n = 2*(rows/2)*chains half-chain draws of `entry` (numbered i = r*chains + c, r < 2h: rows
+ *   [0, h) then rows [rows-h, rows); the middle row of odd rows is not ranked). Key: the order-preserving 64-bit key of x
+ *   (centre NaN: the bulk series) or of |x - centre| (the folded series), with -0 made +0. dev_keys and dev_index hold 2n
+ *   values each; on return dev_keys[0, n) is ascending and dev_index[0, n) holds each key's i (ties in ascending i: a stable
+ *   LSD radix sort of 8-bit digits, so two calls give the same bits); [n, 2n) is scratch. Digit positions that are the same
+ *   for all keys are skipped; *host_passes (when not null) receives the number of passes run (0..8). Errors: rows < 2, entry
+ *   outside [0, entries), n >= 2^32, null dev_samples / dev_keys / dev_index.
+ * amwg_summary_rank_count: for sorted key arrays Q[nq] (this shard's) and R[nr] (any shard's, or Q itself),
+ *   dev_acc[i] += #(R < Q[i]) + #(R <= Q[i]) (merge path). Summed over all shards R, acc + 1 = twice the average rank
+ *   (1-based, ties averaged) of Q[i] among all shards' keys. Integers: exact, independent of the order of the shards.
+ *   Errors: nq or nr < 1 or >= 2^32, null pointers.
+ * amwg_summary_rank_z: dev_z[dev_index[i]] = Phi^-1((r - 3/8) / (total + 1/4)), r = (dev_acc[i] + 1) / 2, for i < n; total is the
+ *   number of ranked draws over all shards. Sized [2h][chains], dev_z is a [2h][1][chains] block whose two halves
+ *   amwg_summary_autocov splits exactly as they were ranked. Errors: n outside 1..2^32-1, total < n or >= 2^52, null pointers. */
 AMWG_API int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats);
 AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t pass,
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
 AMWG_API int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
                                   const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out);
+AMWG_API int amwg_summary_rank_sort(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t entry,
+                                    double centre, uint64_t* dev_keys, uint32_t* dev_index, int32_t* host_passes);
+AMWG_API int amwg_summary_rank_count(int device, const uint64_t* dev_q, int64_t nq, const uint64_t* dev_r, int64_t nr, int64_t* dev_acc);
+AMWG_API int amwg_summary_rank_z(int device, const int64_t* dev_acc, const uint32_t* dev_index, int64_t n, int64_t total, double* dev_z);
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it

@@ -373,6 +373,30 @@ BINDING(summary_autocov)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// summary_rank_sort(device, samples ptr, rows, entries, chains, entry, centre (NaN: bulk), keys ptr [2n], index ptr [2n])
+//   -> number of radix passes run                                                                          amwg_summary_rank_sort
+BINDING(summary_rank_sort)
+  int32_t passes = 0;
+  if (amwg_summary_rank_sort((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                             (int32_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), (int32_t)to_double(env, a.at(5)), to_double(env, a.at(6)),
+                             (uint64_t*)(uintptr_t)to_u64(env, a.at(7)), (uint32_t*)(uintptr_t)to_u64(env, a.at(8)), &passes) != 0)
+    fail_from_library();
+  return js_number(env, (double)passes);
+END_BINDING
+// summary_rank_count(device, Q ptr, nq, R ptr, nr, acc ptr)                                               amwg_summary_rank_count
+BINDING(summary_rank_count)
+  if (amwg_summary_rank_count((int)to_double(env, a.at(0)), (const uint64_t*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                              (const uint64_t*)(uintptr_t)to_u64(env, a.at(3)), (int64_t)to_double(env, a.at(4)), (int64_t*)(uintptr_t)to_u64(env, a.at(5))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// summary_rank_z(device, acc ptr, index ptr, n, total, z ptr)                                             amwg_summary_rank_z
+BINDING(summary_rank_z)
+  if (amwg_summary_rank_z((int)to_double(env, a.at(0)), (const int64_t*)(uintptr_t)to_u64(env, a.at(1)), (const uint32_t*)(uintptr_t)to_u64(env, a.at(2)),
+                          (int64_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), (double*)(uintptr_t)to_u64(env, a.at(5))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
 // peak_fp64(device, reps) -> {tflops, ms}                                        amwg_peak_fp64
 BINDING(peak_fp64)
   double tf = 0.0, ms = 0.0;
@@ -419,6 +443,7 @@ NAPI_MODULE_INIT() {
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
+      {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
