@@ -31,6 +31,7 @@
 #include "amwg_math.cuh"
 #include "amwg_ld.cuh"
 #include "amwg_tma.cuh"
+#include "amwg_init.cuh"
 
 namespace amwg {
 
@@ -772,9 +773,11 @@ __global__ void __launch_bounds__(kThreads) amwg_init_kernel(ModelDev m, ChainAr
   if (valid) a.curr_lp[chain] = lp0;
 }
 
-// log_post at the chains' CURRENT state, evaluated afresh with the full program (nothing is stored): what sampler.log_post()
-// returns for handles whose sweep kernel does not carry the value along (the run-time specialised sweep works on differences).
-__global__ void __launch_bounds__(kThreads) amwg_relp_kernel(ModelDev m, ChainArrays a) {
+// log_post at the chains' CURRENT state, evaluated afresh with the full program: what sampler.log_post() returns for handles
+// whose sweep kernel does not carry the value along (the run-time specialised sweep works on differences). With store_terms the
+// term cache (statistic slots included) is rewritten too, exactly as amwg_init_kernel fills it: after amwg_set_state /
+// amwg_disperse_state every quantity a sweep kernel reads at launch start then belongs to the new state.
+__global__ void __launch_bounds__(kThreads) amwg_relp_kernel(ModelDev m, ChainArrays a, int store_terms) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -784,8 +787,51 @@ __global__ void __launch_bounds__(kThreads) amwg_relp_kernel(ModelDev m, ChainAr
   if (!valid && !ctx.ring_saddr) return;
   const unsigned long long chain = valid ? tid : a.C - 1;              // shadow threads keep a streamed plate CTA-uniform
   EvalState es{a.state + chain, a.C, -1, 0.0};
+  if (store_terms && m.n_terms > 0 && valid) { es.tval = a.tval + chain; es.tcand = a.tcand + chain; es.tstride = a.C; es.direct = true; }
   const double lp = eval_logpost(ctx, es, logpost_pc(m, es));
   if (valid) a.curr_lp[chain] = lp;
+}
+
+// One attempt of amwg_disperse_state (DESIGN.md §2 "Dispersed starting points"): every chain that has no starting point yet draws
+// one into its column of `scratch` ([D][C]) and keeps it when every component is valid and log_post there is finite. The evaluation
+// stores nothing. It stays CTA-uniform: chains that are done evaluate their kept point, shadow threads chain C-1's, and neither
+// writes. `remaining` receives the number of chains still without a point (one atomic per CTA).
+__global__ void __launch_bounds__(kThreads) amwg_disperse_kernel(ModelDev m, ChainArrays a, const double* __restrict__ init, double radius,
+                                                                int attempt, double* __restrict__ scratch, unsigned char* __restrict__ done,
+                                                                unsigned long long* __restrict__ remaining) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ Ctx ctx;
+  __shared__ __align__(8) unsigned long long bar;
+  stage_model(m, smem, ctx, &bar);
+  const unsigned long long tid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = tid < a.C;
+  const unsigned long long chain = valid ? tid : a.C - 1;
+  const bool todo = valid && !done[chain];
+  bool ok = true;
+  if (todo) {
+    for (int p = 0; p < m.n_params; ++p) {
+      const amwg_param& pa = ctx.params[p];
+      for (int k = 0; k < pa.n_comp; ++k) {
+        const int c = pa.comp_offset + k;
+        const double U = disperse_uniform(a.seed, a.first_chain + chain, attempt, m.D, c);
+        double x;
+        ok = disperse_component(pa.type, pa.lower, pa.upper, init[c], radius, U, &x) && ok;
+        scratch[(unsigned long long)c * a.C + chain] = x;
+      }
+    }
+  }
+  __syncthreads();                                                     // chain C-1's column is written before its shadows read it
+  bool pending = false;
+  if (valid || ctx.ring_saddr) {
+    EvalState es{scratch + chain, a.C, -1, 0.0};
+    const double lp = eval_logpost(ctx, es, logpost_pc(m, es));
+    if (todo) {
+      if (ok && lp - lp == 0.0) done[chain] = 1;                     // lp - lp == 0: finite (NaN and +-inf fail)
+      else pending = true;
+    }
+  }
+  const int n_pending = __syncthreads_count(pending);
+  if (threadIdx.x == 0 && n_pending) atomicAdd(remaining, (unsigned long long)n_pending);
 }
 
 // ---- K1: n_sweeps Sampler.step()s per chain, samples recorded before each kept sweep --------------------------------
@@ -1267,6 +1313,7 @@ struct amwg_sampler {
   std::vector<double> iter_since, batch_count;   // chain-invariant counters (mcmc.js:510-511)
   std::vector<void*> dev_allocs;
   unsigned char* d_adapting = nullptr;
+  double* d_init = nullptr;                   // amwg_model.init on the device: the centre of amwg_disperse_state
   double* d_out = nullptr; size_t d_out_bytes = 0;
   int* d_monitor = nullptr; int d_monitor_cap = 0;
   long long launches = 0;
@@ -1312,6 +1359,17 @@ struct JitArgsHost {
   const unsigned char* adapting;
 };
 
+// Binary components hold 0 or 1 (the values BinaryStepper flips between, mcmc.js:753-767): the init at amwg_create and every
+// chain's value at amwg_set_state. x is [n_comp][per_comp].
+static int check_binary_values(const amwg_param* params, int n_params, const double* x, size_t per_comp, const char* who) {
+  for (int p = 0; p < n_params; ++p) {
+    if (params[p].type != AMWG_BINARY) continue;
+    for (size_t k = (size_t)params[p].comp_offset * per_comp; k < (size_t)(params[p].comp_offset + params[p].n_comp) * per_comp; ++k)
+      if (x[k] != 0.0 && x[k] != 1.0) return fail(std::string(who) + ": binary parameters must start at 0 or 1");
+  }
+  return 0;
+}
+
 static int validate_model(const amwg_model* md) {
   if (!md) return fail("amwg_create: model is NULL");
   if (md->abi_version != AMWG_ABI_VERSION) return fail("amwg_create: ABI version mismatch");
@@ -1326,12 +1384,10 @@ static int validate_model(const amwg_model* md) {
     if (pa.n_comp < 1 || pa.dim0 < 1 || pa.n_comp % pa.dim0) return fail("amwg_create: bad parameter dimensions");
     if (pa.dim0 > kMaxDim0) return fail("amwg_create: dim[0] > 65535 is not supported");
     if (pa.comp_offset != D) return fail("amwg_create: comp_offset must be the running component count");
-    if (pa.type == AMWG_BINARY)
-      for (int c = 0; c < pa.n_comp; ++c)
-        if (md->init[D + c] != 0.0 && md->init[D + c] != 1.0) return fail("amwg_create: binary parameters must start at 0 or 1");
     D += pa.n_comp;
   }
   if (D != md->n_comp) return fail("amwg_create: n_comp does not match the parameter list");
+  if (check_binary_values(md->params, md->n_params, md->init, 1, "amwg_create")) return -1;
   if (md->logpost_prog < 0 || md->logpost_prog >= md->n_code) return fail("amwg_create: logpost_prog out of range");
   if (md->n_variant_comps < 0 || md->n_variant_comps > AMWG_MAX_VARIANT_COMPS) return fail("amwg_create: at most 4 program-selecting binary components are supported");
   for (int k = 0; k < md->n_variant_comps; ++k)
@@ -1646,6 +1702,7 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
       cudaFuncSetAttribute(amwg_stat_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_relp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
+      cudaFuncSetAttribute(amwg_disperse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_derived_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess)
     return bail(fail("cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed"));
@@ -1681,6 +1738,7 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
   std::vector<double> pls0(s->D);
   for (int c = 0; c < s->D; ++c) pls0[c] = s->opts[c].prop_log_scale;
   if (dev_upload(s, md->init, (size_t)s->D, &d_init) || dev_upload(s, pls0.data(), (size_t)s->D, &d_pls0)) return bail(-1);
+  s->d_init = d_init;
 
   if (md->n_fold > 0) {
     int *d_fp = nullptr, *d_fd = nullptr;
@@ -1875,13 +1933,69 @@ extern "C" int amwg_get_log_post(amwg_sampler* s, double* host_out) {
   if (!s || !host_out) return fail("amwg_get_log_post: NULL argument");
   CUDA_TRY(cudaSetDevice(s->device));
   if (s->jit_kernel) {          // the specialised sweep steps on differences: evaluate log_post at the current state now
-    amwg_relp_kernel<<<grid_for(s->a.C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a);
+    amwg_relp_kernel<<<grid_for(s->a.C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, 0);
     CUDA_TRY(cudaGetLastError());
     s->launches++;
   }
   CUDA_TRY(cudaMemcpyAsync(host_out, s->a.curr_lp, sizeof(double) * (size_t)s->a.C, cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   return 0;
+}
+
+// Place every chain at src ([D][C], host or device memory), then recompute what the sweep kernels carry across launches from it:
+// curr_lp and the term cache. Proposal scales, acceptance counts, permutations, stream positions and adaptation counters stay.
+static int commit_state(amwg_sampler* s, const double* src, cudaMemcpyKind kind) {
+  CUDA_TRY(cudaMemcpyAsync(s->a.state, src, sizeof(double) * (size_t)s->D * (size_t)s->a.C, kind, s->stream));
+  amwg_relp_kernel<<<grid_for(s->a.C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, 1);
+  CUDA_TRY(cudaGetLastError());
+  s->launches++;
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+extern "C" int amwg_set_state(amwg_sampler* s, const double* host_in) {
+  if (!s || !host_in) return fail("amwg_set_state: NULL argument");
+  if (check_binary_values(s->params.data(), s->P, host_in, (size_t)s->a.C, "amwg_set_state")) return -1;
+  CUDA_TRY(cudaSetDevice(s->device));
+  return commit_state(s, host_in, cudaMemcpyHostToDevice);
+}
+
+extern "C" int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_failed) {
+  if (n_failed) *n_failed = 0;
+  if (!s) return fail("amwg_disperse_state: NULL handle");
+  if (!(radius > 0.0) || radius == INFINITY) return fail("amwg_disperse_state: radius must be finite and > 0");
+  CUDA_TRY(cudaSetDevice(s->device));
+  const unsigned long long C = s->a.C;
+  double* d_x = nullptr;
+  unsigned char* d_done = nullptr;
+  unsigned long long* d_left = nullptr;
+  unsigned long long left = C;
+  auto run = [&]() -> cudaError_t {
+    cudaError_t e = cudaMalloc(&d_x, sizeof(double) * (size_t)s->D * (size_t)C);
+    if (e == cudaSuccess) e = cudaMalloc(&d_done, (size_t)C);
+    if (e == cudaSuccess) e = cudaMalloc(&d_left, sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_done, 0, (size_t)C, s->stream);
+    for (int attempt = 0; e == cudaSuccess && left > 0 && attempt < kDisperseAttempts; ++attempt) {
+      e = cudaMemsetAsync(d_left, 0, sizeof(unsigned long long), s->stream);
+      if (e != cudaSuccess) break;
+      amwg_disperse_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, s->d_init, radius, attempt, d_x, d_done, d_left);
+      s->launches++;
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaMemcpyAsync(&left, d_left, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+    }
+    return e;
+  };
+  const cudaError_t e = run();
+  int rc = 0;
+  if (e != cudaSuccess) rc = fail(std::string("amwg_disperse_state: ") + cudaGetErrorString(e));
+  else if (left > 0) {
+    if (n_failed) *n_failed = (int64_t)left;
+    rc = fail("amwg_disperse_state: " + std::to_string(left) + " of " + std::to_string(C) + " chains found no starting point with a finite log_post in " +
+              std::to_string(kDisperseAttempts) + " attempts");
+  } else rc = commit_state(s, d_x, cudaMemcpyDeviceToDevice);
+  cudaFree(d_x); cudaFree(d_done); cudaFree(d_left);
+  return rc;
 }
 
 extern "C" int amwg_set_adapting(amwg_sampler* s, int32_t flag) {

@@ -10,7 +10,9 @@ binding a Node host would put under the same `mcmc` / `ld` module names.
 
 New, non-reference options (the many-chain setting needs them): ``chains`` (default 1: output is
 shaped exactly like the reference's), ``seed``, ``device``, ``distributed``, ``first_chain`` (global id of
-the first chain, default 0), ``faithful`` (no factorised likelihood plates: bit-faithful, slower).
+the first chain, default 0), ``faithful`` (no factorised likelihood plates: bit-faithful, slower),
+``init_radius`` (over-dispersed starting points drawn on the device, DESIGN.md §2; default: every chain
+starts at the params' init). ``sampler.set_state(values)`` places the chains anywhere.
 """
 from __future__ import annotations
 
@@ -246,6 +248,21 @@ def rnorm(mean, sd):
     return (v / u) * sd + mean
 
 
+DISPERSE_ATTEMPTS = 100         # csrc/amwg_init.cuh kDisperseAttempts
+
+
+def dispersal_failure_message(n_failed: int, n_chains: int, distributed: bool = False, device: int = 0) -> Optional[str]:
+    """What options.init_radius raises when chains found no starting point (None: every chain found one). `n_failed` counts this
+    handle's chains; with `distributed` it is summed over all ranks first, so that every rank takes the same decision."""
+    if distributed:
+        from .parallel import total_over_ranks
+        n_failed = total_over_ranks(n_failed, device)
+    if n_failed <= 0:
+        return None
+    return "options.init_radius: %d of %d chains found no starting point with a finite log_post in %d attempts" % (
+        n_failed, n_chains, DISPERSE_ATTEMPTS)
+
+
 def _default_device() -> int:
     return int(os.environ.get("LOCAL_RANK", "0")) if os.environ.get("AMWG_DEVICE") is None else int(os.environ["AMWG_DEVICE"])
 
@@ -336,6 +353,10 @@ class AmwgSampler(Sampler):
         if self.gather not in ("all", "root", "none"):
             raise JsThrow("options.gather must be \"all\", \"root\" or \"none\"")
         self.faithful = bool(get_option("faithful", options, False))      # no factorised plates: bit-faithful sums, slower
+        radius = get_option("init_radius", options, None)                  # over-dispersed starting points (DESIGN.md §2)
+        if radius is not None and not (is_number(radius) and math.isfinite(radius) and radius > 0):
+            raise JsThrow("options.init_radius must be a finite number > 0")
+        self.init_radius = None if radius is None else float(radius)
 
         # flat component layout: Object.keys(params) order, row-major inside a parameter
         self._offsets: Dict[str, int] = {}
@@ -442,6 +463,20 @@ class AmwgSampler(Sampler):
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
         self._handle = h
+        if self.init_radius is not None:
+            self._disperse(self.init_radius)
+
+    def _disperse(self, radius: float):
+        """options.init_radius: every chain to its first valid point of the device's dispersal (amwg_disperse_state). With
+        options.distributed the failed chains are counted over all ranks, so that every rank raises the same message or none."""
+        L = _ffi.lib()
+        failed = C.c_int64(0)
+        rc = L.amwg_disperse_state(self._handle, float(radius), C.byref(failed))
+        err = L.amwg_last_error().decode() if rc != 0 else ""
+        msg = dispersal_failure_message(failed.value, self.n_chains, self.distributed, self.device)
+        if rc != 0 or msg:
+            self.close()
+            raise JsThrow(msg or err)
 
     def __del__(self):
         try:
@@ -491,6 +526,50 @@ class AmwgSampler(Sampler):
         for name in self._state_keys():
             e = self._entries(name)
             out[name] = self._shape_out(name, buf[e][None, :, :])[0]
+        return out
+
+    def set_state(self, values: Dict[str, Any]):
+        """Not in the reference: place the chains, e.g. where a previous run, prior draws or an optimiser left them. `values` is keyed
+        by parameter name; each value is shaped like `state[name]` ([chains, *dim], [chains] for a scalar parameter; the reference's
+        shape for one chain), or like one chain's value (`dim`, a number for a scalar parameter), which every chain receives.
+        Parameters not named keep their values. log_post and its cached terms are evaluated afresh; proposal scales, adaptation and
+        the random streams carry on untouched, so each chain continues as the reference chain would from that point. With
+        options.distributed the arrays cover all `chains` global chains and every rank takes its own."""
+        if not isinstance(values, dict):
+            raise JsThrow("set_state expects an object keyed by parameter name")
+        L = _ffi.lib()
+        cur = np.empty((self.n_comp + len(self._derived_names), self.local_chains))
+        _ffi.check(L.amwg_get_state(self._handle, cur.ctypes.data))
+        block = np.ascontiguousarray(self._set_state_block(values, cur[:self.n_comp]))
+        if L.amwg_set_state(self._handle, block.ctypes.data) != 0:
+            raise JsThrow(L.amwg_last_error().decode())
+
+    def _set_state_block(self, values: Dict[str, Any], current: np.ndarray) -> np.ndarray:
+        """set_state's argument over `current` ([n_comp, local_chains]: the state now) -> the [n_comp, local_chains] block of
+        amwg_set_state. Host-side shaping only: checked without a device."""
+        from .parallel import local_chain_rows
+        out = np.array(current, dtype=np.float64, copy=True)
+        first = self.first_chain if self.distributed else 0
+        for name, v in values.items():
+            if name in self._derived_names:
+                raise JsThrow("set_state: " + name + " is a derived quantity, not a parameter")
+            if name not in self._offsets:
+                raise JsThrow("set_state: " + name + " is not a parameter of this sampler")
+            dim = list(self.params[name]["dim"])
+            n, off = int(np.prod(dim)), self._offsets[name]
+            try:
+                a = np.asarray(v, dtype=np.float64)
+            except (TypeError, ValueError):
+                raise JsThrow("set_state: the value of " + name + " is not numeric") from None
+            one = [] if dim == [1] else dim                       # one chain's value: a number for a scalar parameter
+            per_chain = [self.n_chains] + one
+            if list(a.shape) in (one, dim):
+                out[off:off + n, :] = a.reshape(n, 1)
+            elif list(a.shape) == per_chain:
+                out[off:off + n, :] = local_chain_rows(a.reshape(self.n_chains, n), first, self.local_chains).T
+            else:
+                raise JsThrow("set_state: " + name + " is of dimension [" + _js_join(list(a.shape)) + "] but should be [" + _js_join(dim) +
+                              "] or [" + _js_join(per_chain) + "]")
         return out
 
     def log_post(self):
@@ -553,8 +632,10 @@ class AmwgSampler(Sampler):
         diagnostics=True adds, per parameter and shaped like "mean": "ess_mean" and "ess_tail" (split-chain effective sample
         sizes of the draws and of the 5 % / 95 % tail indicators, Vehtari et al. 2021), "mcse_mean" (sd / sqrt(ess_mean)) and
         "rhat_split" (split-chain R-hat, not rank-normalised); the other keys keep their values bit for bit. Fewer than 10 kept
-        rows give NaN; see summary.split_chain_diagnostics for the estimator and its edge cases. All chains start from the same
-        init, so "rhat" and "rhat_split" only mean something after burn-in.
+        rows give NaN; see summary.split_chain_diagnostics for the estimator and its edge cases. The R-hats compare chains, so they
+        can only flag what the chains' starting points let them see: by default every chain starts at the same init, and chains
+        that all stay in one mode report R-hat near 1. options.init_radius draws over-dispersed starting points (DESIGN.md §2);
+        set_state places the chains anywhere.
         diagnostics="rank" returns everything diagnostics=True does, bit for bit, plus "ess_bulk" (ESS of the rank-normalised
         split chains) and "rhat_rank" (the larger split R-hat of the rank-normalised draws and of the rank-normalised folded draws
         |x - median|), ranked over the pooled draws of all chains on all GPUs (Vehtari et al. 2021, §4; the numbers Stan and

@@ -37,6 +37,24 @@ def shard_chains(n_chains: int) -> Tuple[int, int]:
     return shard_bounds(n_chains, rank, ws)
 
 
+def local_chain_rows(values: np.ndarray, first_chain: int, count: int) -> np.ndarray:
+    """This rank's chains [first_chain, first_chain + count) of a per-chain array over all global chains (chain axis first)."""
+    if values.shape[0] < first_chain + count:
+        raise ValueError("the array covers %d chains, the shard ends at chain %d" % (values.shape[0], first_chain + count))
+    return values[first_chain:first_chain + count]
+
+
+def total_over_ranks(n: int, device: int = 0) -> int:
+    """The sum of an integer over all ranks: one tiny all-reduce (on the GPU under NCCL, on the CPU under gloo), so that every rank
+    takes the same decision from it."""
+    import torch
+    import torch.distributed as dist
+    dev = torch.device("cuda", device) if dist.get_backend() == "nccl" else torch.device("cpu")
+    t = torch.tensor([int(n)], dtype=torch.int64, device=dev)
+    dist.all_reduce(t)
+    return int(t.item())
+
+
 def _rank_major_to_chain_axis(stacked, ws: int, rows: int, entries: int, cmax: int, counts):
     """`stacked[ws][rows][entries][cmax]` (what one collective delivers) -> `[rows, entries, sum(counts)]`, chains in global order:
     one strided device copy (the kernel's layout keeps the chain axis fastest, so the rank axis has to move inside)."""

@@ -234,6 +234,21 @@ AMWG_API int amwg_get_state(amwg_sampler* s, double* host_out);
 /* sampler.log_post() -- the closure the Sampler ctor stores (mcmc.js:958-960): log_post at the chain's current state, out[chain] */
 AMWG_API int amwg_get_log_post(amwg_sampler* s, double* host_out);
 
+/* Per-chain starting points (not in the reference, which runs one chain from params[*].init).
+ * amwg_set_state: host_in is [n_comp][chain] fp64 -- the first n_comp rows of what amwg_get_state returns. Every chain is placed
+ *   there and log_post and its cached terms are evaluated afresh from it; derived quantities follow from the state. Proposal scales,
+ *   acceptance counts, visiting orders, stream positions and adaptation counters are untouched and no random number is drawn: chain
+ *   g then continues exactly like the reference chain g continued from host_in at the same point of its run. Binary components
+ *   must be 0 or 1 (as at amwg_create); otherwise an error is returned and the handle is unchanged.
+ * amwg_disperse_state: over-dispersed starting points drawn on the device, for convergence diagnostics that need chains to start
+ *   apart (DESIGN.md §2 "Dispersed starting points"). Per chain, attempts a = 0..99 draw every component uniformly within +-radius
+ *   of its init on the unconstrained scale (uniform #(2^63 + a*n_comp + c) of the chain's Philox stream, so the draws do not
+ *   depend on sharding and never meet Math.random()'s); a chain keeps its first attempt whose components are valid and whose
+ *   log_post is finite. The points are then committed as by amwg_set_state. radius must be finite and > 0. If some chains find no
+ *   point in 100 attempts, *n_failed (when not null) receives their number, an error is returned and the handle is unchanged. */
+AMWG_API int amwg_set_state(amwg_sampler* s, const double* host_in);
+AMWG_API int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_failed);
+
 /* sampler.start_adaptation() / stop_adaptation() -- mcmc.js:1060-1073 */
 AMWG_API int amwg_set_adapting(amwg_sampler* s, int32_t flag);
 

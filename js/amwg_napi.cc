@@ -279,6 +279,20 @@ BINDING(get_log_post)
   if (amwg_get_log_post(h->s, out.data()) != 0) fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// set_state(handle, values [n_comp][chains])                                    amwg_set_state
+BINDING(set_state)
+  Handle* h = handle_of(env, a.at(0));
+  std::vector<double> x = doubles(env, a.at(1));
+  if (x.size() != (size_t)h->n_comp * (size_t)h->n_chains) throw Throw{"amwg_native: set_state expects n_comp x chains numbers"};
+  if (amwg_set_state(h->s, x.data()) != 0) fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// disperse_state(handle, radius) -> chains without a starting point (0: all placed)   amwg_disperse_state
+BINDING(disperse_state)
+  int64_t failed = 0;
+  if (amwg_disperse_state(handle_of(env, a.at(0))->s, to_double(env, a.at(1)), &failed) != 0 && failed == 0) fail_from_library();
+  return js_number(env, (double)failed);
+END_BINDING
 // set_adapting(handle, flag)                                                    amwg_set_adapting (mcmc.js:1060-1073)
 BINDING(set_adapting)
   if (amwg_set_adapting(handle_of(env, a.at(0))->s, to_double(env, a.at(1)) != 0 ? 1 : 0) != 0) fail_from_library();
@@ -439,7 +453,7 @@ END_BINDING
 NAPI_MODULE_INIT() {
   const struct { const char* name; napi_callback fn; } table[] = {
       {"create", create}, {"destroy", destroy}, {"burn", burn}, {"sample", sample}, {"sample_device", sample_device}, {"get_state", get_state},
-      {"get_log_post", get_log_post}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
+      {"get_log_post", get_log_post}, {"set_state", set_state}, {"disperse_state", disperse_state}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},

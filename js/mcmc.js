@@ -11,7 +11,8 @@
 //
 // New, non-reference options: `chains` (default 1: output shaped exactly like the reference's), `seed`, `device`, `first_chain`,
 // `faithful` (no factorised likelihood plates: bit-faithful sums, slower), `scope` ({name: value} for identifiers log_post uses
-// from an enclosing scope that a recording from source cannot see).
+// from an enclosing scope that a recording from source cannot see), `init_radius` (over-dispersed starting points drawn on the
+// device, DESIGN.md §2). New method: `sampler.set_state(values)` places the chains anywhere.
 (function (root, factory) {
   if (typeof define === "function" && define.amd) { define(["./amwg_trace", "./amwg_native"], factory); }
   else if (typeof module === "object" && module.exports) { module.exports = factory(require("./amwg_trace"), require("./amwg_native")); }
@@ -176,7 +177,7 @@
 
   // ---------------------------------------------------------------------------------------------- the device model
   function DeviceModel(params, names, log_post, data, options, resolved) {
-    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed;
+    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed, radius, failed;
     this.params = params; this.names = names; this.offsets = {};
     for (i = 0; i < names.length; i++) { this.offsets[names[i]] = n_comp; n_comp += product(params[names[i]].dim); }
     this.n_comp = n_comp;
@@ -186,7 +187,9 @@
     this.seed = seed === null ? Math.floor(Math.random() * 9007199254740992) : seed;
     this.device = get_option("device", options, 0);
     this.first_chain = get_option("first_chain", options, 0);
-    prog = tracer.trace(log_post, names, params, this.offsets, n_comp, data, {faithful: !!get_option("faithful", options, false), scope: get_option("scope", options, null),
+    radius = get_option("init_radius", options, null);            // over-dispersed starting points (DESIGN.md §2)
+    if (radius !== null && !(typeof radius === "number" && isFinite(radius) && radius > 0)) { throw "options.init_radius must be a finite number > 0"; }
+    prog =tracer.trace(log_post, names, params, this.offsets, n_comp, data, {faithful: !!get_option("faithful", options, false), scope: get_option("scope", options, null),
                                                                                 base_state: get_option("base_state", options, null)});
     this.program = prog;
     this.derived_names = prog.derived_names;
@@ -213,6 +216,14 @@
       }
     }
     this.handle = native.create(desc, this.n_chains, this.first_chain, this.seed, this.device);
+    if (radius !== null) {
+      failed = native.disperse_state(this.handle, radius);
+      if (failed > 0) {
+        native.destroy(this.handle);
+        this.handle = null;
+        throw "options.init_radius: " + failed + " of " + this.n_chains + " chains found no starting point with a finite log_post in 100 attempts";
+      }
+    }
   }
   DeviceModel.prototype.state_keys = function () { return this.names.concat(this.derived_names); };
   DeviceModel.prototype.entries = function (name) {
@@ -243,6 +254,32 @@
     var keys = this.state_keys(), n_entries = this.n_comp + this.derived_names.length, raw = native.get_state(this.handle), out = {}, i, e;
     for (i = 0; i < keys.length; i++) { e = this.entries(keys[i]); out[keys[i]] = this.shape_out(keys[i], raw, 1, n_entries, e[0], e.length)[0]; }
     return out;
+  };
+  // values: {name: value shaped like state()[name], or like one chain's value (given to every chain)} -> amwg_set_state
+  DeviceModel.prototype.set_state = function (values) {
+    var C = this.n_chains, D = this.n_comp, raw = native.get_state(this.handle), block = [], keys, i, k, c, name, dim, n, off, v, got, one, per, flat, scalar;
+    if (values === null || typeof values !== "object" || is_array(values)) { throw "set_state expects an object keyed by parameter name"; }
+    for (i = 0; i < D * C; i++) { block.push(raw[i]); }
+    keys = own_keys(values);
+    for (i = 0; i < keys.length; i++) {
+      name = keys[i];
+      if (this.derived_names.indexOf(name) >= 0) { throw "set_state: " + name + " is a derived quantity, not a parameter"; }
+      if (!this.offsets.hasOwnProperty(name)) { throw "set_state: " + name + " is not a parameter of this sampler"; }
+      dim = this.params[name].dim; n = product(dim); off = this.offsets[name]; v = values[name];
+      scalar = array_equal(dim, [1]);
+      one = scalar ? [] : dim;
+      per = [C].concat(one);
+      got = is_array(v) ? array_dim(v) : [];
+      flat = flatten(v);
+      if ((array_equal(got, one) || array_equal(got, dim)) && flat.length === n) {
+        for (k = 0; k < n; k++) { for (c = 0; c < C; c++) { block[(off + k) * C + c] = flat[k]; } }
+      } else if (array_equal(got, per) && flat.length === C * n) {
+        for (k = 0; k < n; k++) { for (c = 0; c < C; c++) { block[(off + k) * C + c] = flat[c * n + k]; } }
+      } else {
+        throw "set_state: " + name + " is of dimension [" + got + "] but should be [" + dim + "] or [" + per + "]";
+      }
+    }
+    native.set_state(this.handle, block);
   };
   DeviceModel.prototype.sample = function (n, thin, monitored) {
     var entries = [], spans = {}, i, e, rows, raw, out = {}, j, col;
@@ -325,6 +362,9 @@
   };
   AmwgSampler.prototype.step = function () { this.burn(1); return this.model.state(); };
   AmwgSampler.prototype.state = function () { return this.model.state(); };
+  // Not in the reference: place the chains (from a previous run, prior draws, an optimiser). Shapes as state() returns them, or one
+  // chain's value for all chains; parameters not named keep their values; adaptation and the random streams carry on untouched.
+  AmwgSampler.prototype.set_state = function (values) { this.model.set_state(values); };
   AmwgSampler.prototype.log_post = function () { var lp = native.get_log_post(this.model.handle); return this.n_chains === 1 ? lp[0] : lp; };
   AmwgSampler.prototype.start_adaptation = function () { native.set_adapting(this.model.handle, 1); };
   AmwgSampler.prototype.stop_adaptation = function () { native.set_adapting(this.model.handle, 0); };
