@@ -63,7 +63,8 @@ class AmwgModel(C.Structure):
 
 
 EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_sample_device", "amwg_get_state", "amwg_get_log_post",
-           "amwg_set_state", "amwg_disperse_state", "amwg_set_adapting", "amwg_info", "amwg_kernel_launches", "amwg_last_sweep_kernel_ms", "amwg_n_chains",
+           "amwg_set_state", "amwg_disperse_state", "amwg_model_fingerprint", "amwg_checkpoint_size", "amwg_checkpoint_save",
+           "amwg_checkpoint_load", "amwg_set_adapting", "amwg_info", "amwg_kernel_launches", "amwg_last_sweep_kernel_ms", "amwg_n_chains",
            "amwg_last_error", "amwg_abi_version", "amwg_ld_eval", "amwg_primitive_eval",
            "amwg_summary_moments", "amwg_summary_digit_hist", "amwg_summary_autocov", "amwg_summary_rank_sort",
            "amwg_summary_rank_count", "amwg_summary_rank_z", "amwg_peak_fp64", "amwg_jit_status", "amwg_jit_compile_check",
@@ -97,6 +98,10 @@ def lib():
     L.amwg_get_log_post.argtypes = [vp, vp]; L.amwg_get_log_post.restype = C.c_int
     L.amwg_set_state.argtypes = [vp, vp]; L.amwg_set_state.restype = C.c_int
     L.amwg_disperse_state.argtypes = [vp, dbl, C.POINTER(i64)]; L.amwg_disperse_state.restype = C.c_int
+    L.amwg_model_fingerprint.argtypes = [C.POINTER(AmwgModel), C.POINTER(u64)]; L.amwg_model_fingerprint.restype = C.c_int
+    L.amwg_checkpoint_size.argtypes = [vp, C.POINTER(i64)]; L.amwg_checkpoint_size.restype = C.c_int
+    L.amwg_checkpoint_save.argtypes = [vp, vp, i64]; L.amwg_checkpoint_save.restype = C.c_int
+    L.amwg_checkpoint_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]; L.amwg_checkpoint_load.restype = C.c_int
     L.amwg_set_adapting.argtypes = [vp, i32]; L.amwg_set_adapting.restype = C.c_int
     L.amwg_info.argtypes = [vp, vp, vp, vp]; L.amwg_info.restype = C.c_int
     L.amwg_kernel_launches.argtypes = [vp]; L.amwg_kernel_launches.restype = i64

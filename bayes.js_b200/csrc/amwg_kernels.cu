@@ -32,6 +32,7 @@
 #include "amwg_ld.cuh"
 #include "amwg_tma.cuh"
 #include "amwg_init.cuh"
+#include "amwg_checkpoint.h"
 
 namespace amwg {
 
@@ -1230,6 +1231,13 @@ __global__ void __launch_bounds__(256) amwg_adapt_kernel(ChainArrays a, AdaptArg
   }
 }
 
+// ---- amwg_checkpoint_load: the proposal sd of every component of every chain from its restored prop_log_scale -------------------
+// The same js_exp the init and adaptation kernels store, so psd has the bits an uninterrupted run carries.
+__global__ void __launch_bounds__(256) amwg_psd_kernel(ChainArrays a, unsigned long long n) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) a.psd[i] = js_exp(a.pls[i]);
+}
+
 // ---- derived quantities for amwg_get_state ------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) amwg_derived_kernel(ModelDev m, ChainArrays a, double* out /*[n_derived][C]*/) {
   extern __shared__ __align__(16) unsigned char smem[];
@@ -1314,6 +1322,7 @@ struct amwg_sampler {
   std::vector<void*> dev_allocs;
   unsigned char* d_adapting = nullptr;
   double* d_init = nullptr;                   // amwg_model.init on the device: the centre of amwg_disperse_state
+  uint64_t fingerprint = 0;                   // amwg_model_fingerprint of the model: checkpoint images must carry the same
   double* d_out = nullptr; size_t d_out_bytes = 0;
   int* d_monitor = nullptr; int d_monitor_cap = 0;
   long long launches = 0;
@@ -1359,14 +1368,10 @@ struct JitArgsHost {
   const unsigned char* adapting;
 };
 
-// Binary components hold 0 or 1 (the values BinaryStepper flips between, mcmc.js:753-767): the init at amwg_create and every
-// chain's value at amwg_set_state. x is [n_comp][per_comp].
+// Binary components hold 0 or 1 (amwg_checkpoint.h binary_values_ok): the init at amwg_create and every chain's value at
+// amwg_set_state. x is [n_comp][per_comp].
 static int check_binary_values(const amwg_param* params, int n_params, const double* x, size_t per_comp, const char* who) {
-  for (int p = 0; p < n_params; ++p) {
-    if (params[p].type != AMWG_BINARY) continue;
-    for (size_t k = (size_t)params[p].comp_offset * per_comp; k < (size_t)(params[p].comp_offset + params[p].n_comp) * per_comp; ++k)
-      if (x[k] != 0.0 && x[k] != 1.0) return fail(std::string(who) + ": binary parameters must start at 0 or 1");
-  }
+  if (!ckpt::binary_values_ok(params, n_params, x, per_comp)) return fail(std::string(who) + ": binary parameters must start at 0 or 1");
   return 0;
 }
 
@@ -1608,6 +1613,7 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
   if (cudaStreamCreateWithFlags(&s->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
 
   s->D = md->n_comp; s->P = md->n_params; s->n_derived = md->n_derived;
+  s->fingerprint = ckpt::model_fingerprint(md);
   s->params.assign(md->params, md->params + md->n_params);
   s->opts.assign(md->comp_options, md->comp_options + md->n_comp);
   s->comp_type.resize(s->D);
@@ -1996,6 +2002,86 @@ extern "C" int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_fa
   } else rc = commit_state(s, d_x, cudaMemcpyDeviceToDevice);
   cudaFree(d_x); cudaFree(d_done); cudaFree(d_left);
   return rc;
+}
+
+// ---- checkpoints (DESIGN.md §2 "Checkpoints"; the image code is amwg_checkpoint.h) ---------------------------------------------
+extern "C" int amwg_model_fingerprint(const amwg_model* md, uint64_t* out) {
+  if (!out) return fail("amwg_model_fingerprint: out is NULL");
+  if (validate_model(md)) return -1;
+  *out = ckpt::model_fingerprint(md);
+  return 0;
+}
+
+extern "C" int amwg_checkpoint_size(amwg_sampler* s, int64_t* out) {
+  if (!s || !out) return fail("amwg_checkpoint_size: NULL argument");
+  *out = (int64_t)ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C).total;
+  return 0;
+}
+
+extern "C" int amwg_checkpoint_save(amwg_sampler* s, uint8_t* host_out, int64_t cap) {
+  if (!s || !host_out) return fail("amwg_checkpoint_save: NULL argument");
+  const ckpt::Layout L = ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C);
+  if (cap < (int64_t)L.total) return fail("amwg_checkpoint_save: the buffer holds " + std::to_string(cap) + " bytes, the image needs " + std::to_string(L.total));
+  CUDA_TRY(cudaSetDevice(s->device));
+  ckpt::Header h;
+  h.P = (uint32_t)s->P; h.D = (uint32_t)s->D; h.fingerprint = s->fingerprint; h.seed = s->a.seed; h.first_chain = s->a.first_chain; h.n_chains = s->a.C;
+  h.is_adapting.assign(s->is_adapting.begin(), s->is_adapting.end());
+  h.iter_since = s->iter_since; h.batch_count = s->batch_count;
+  ckpt::write_header(host_out, h);
+  const void* src[ckpt::kSections] = {s->a.state, s->a.pls, s->a.perm, s->a.rng_n, s->a.acc, s->a.perm_ext};
+  for (int k = 0; k < ckpt::kSections; ++k) {
+    const ckpt::Span sp = ckpt::span(L, s->D, s->P, (ckpt::Section)k);
+    if (sp.rows) CUDA_TRY(cudaMemcpyAsync(host_out + sp.off, src[k], (size_t)(sp.rows * s->a.C * sp.width), cudaMemcpyDeviceToHost, s->stream));
+  }
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  ckpt::seal(host_out, L);
+  return 0;
+}
+
+// Validate every image against the handle on the host; then (unless dry_run) upload the handle's chains from them, adopt the
+// images' seed and counters, and recompute what is not stored: psd from prop_log_scale, curr_lp and the term cache from the state.
+extern "C" int amwg_checkpoint_load(amwg_sampler* s, const uint8_t* const* images, const int64_t* sizes, int32_t n_images, int32_t dry_run) {
+  if (!s) return fail("restore: NULL handle");
+  if (n_images < 1 || !images || !sizes) return fail("restore: no image given");
+  std::vector<ckpt::View> views((size_t)n_images);
+  for (int k = 0; k < n_images; ++k) {
+    const std::string e = ckpt::parse(images[k], sizes[k], views[k]);
+    if (!e.empty()) return fail(e);
+  }
+  ckpt::Target t;
+  t.fingerprint = s->fingerprint; t.first_chain = s->a.first_chain; t.n_chains = s->a.C; t.D = s->D; t.P = s->P;
+  t.params = s->params;
+  t.batch_size.resize(s->D);
+  for (int c = 0; c < s->D; ++c) t.batch_size[c] = s->opts[c].batch_size;
+  std::vector<ckpt::Piece> pieces;
+  const std::string e = ckpt::check(views, t, pieces);
+  if (!e.empty()) return fail(e);
+  if (dry_run) return 0;
+
+  CUDA_TRY(cudaSetDevice(s->device));
+  const unsigned long long C = s->a.C;
+  void* dst[ckpt::kSections] = {s->a.state, s->a.pls, s->a.perm, s->a.rng_n, s->a.acc, s->a.perm_ext};
+  for (int k = 0; k < ckpt::kSections; ++k)
+    for (const ckpt::Piece& pc : pieces) {
+      const ckpt::View& v = views[pc.img];
+      const ckpt::Span sp = ckpt::span(v.L, s->D, s->P, (ckpt::Section)k);
+      if (!sp.rows) continue;
+      CUDA_TRY(cudaMemcpy2DAsync((uint8_t*)dst[k] + pc.dst * sp.width, C * sp.width, v.p + sp.off + pc.src * sp.width, v.h.n_chains * sp.width,
+                                 pc.count * sp.width, sp.rows, cudaMemcpyHostToDevice, s->stream));
+    }
+  const ckpt::Header& h = views[0].h;
+  s->a.seed = h.seed;
+  for (int c = 0; c < s->D; ++c) { s->is_adapting[c] = (unsigned char)h.is_adapting[c]; s->iter_since[c] = h.iter_since[c]; s->batch_count[c] = h.batch_count[c]; }
+  CUDA_TRY(cudaMemcpyAsync(s->d_adapting, s->is_adapting.data(), (size_t)s->D, cudaMemcpyHostToDevice, s->stream));
+  const unsigned long long DC = (unsigned long long)s->D * C;
+  amwg_psd_kernel<<<grid_for(DC, 256), 256, 0, s->stream>>>(s->a, DC);
+  CUDA_TRY(cudaGetLastError());
+  s->launches++;
+  amwg_relp_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, 1);
+  CUDA_TRY(cudaGetLastError());
+  s->launches++;
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return 0;
 }
 
 extern "C" int amwg_set_adapting(amwg_sampler* s, int32_t flag) {

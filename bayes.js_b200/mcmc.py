@@ -12,7 +12,8 @@ New, non-reference options (the many-chain setting needs them): ``chains`` (defa
 shaped exactly like the reference's), ``seed``, ``device``, ``distributed``, ``first_chain`` (global id of
 the first chain, default 0), ``faithful`` (no factorised likelihood plates: bit-faithful, slower),
 ``init_radius`` (over-dispersed starting points drawn on the device, DESIGN.md §2; default: every chain
-starts at the params' init). ``sampler.set_state(values)`` places the chains anywhere.
+starts at the params' init). ``sampler.set_state(values)`` places the chains anywhere; ``sampler.checkpoint()`` and
+``sampler.restore(images)`` stop and resume a run bit for bit.
 """
 from __future__ import annotations
 
@@ -261,6 +262,40 @@ def dispersal_failure_message(n_failed: int, n_chains: int, distributed: bool = 
         return None
     return "options.init_radius: %d of %d chains found no starting point with a finite log_post in %d attempts" % (
         n_failed, n_chains, DISPERSE_ATTEMPTS)
+
+
+RESTORE_REFUSED_ELSEWHERE = "restore: refused on another rank; no rank was changed"
+
+
+def restore_images(images) -> List[np.ndarray]:
+    """restore()'s argument -> one uint8 array per image, without copying: bytes, bytearray and memoryview are images, as is a
+    non-empty list or tuple of them. Anything else raises."""
+    kinds = (bytes, bytearray, memoryview)
+    if isinstance(images, kinds):
+        images = [images]
+    if not isinstance(images, (list, tuple)) or not images or not all(isinstance(x, kinds) for x in images):
+        raise JsThrow("restore expects a checkpoint image (bytes, bytearray or memoryview) or a list of them")
+    out = []
+    for x in images:
+        try:
+            out.append(np.frombuffer(x, dtype=np.uint8))
+        except (ValueError, BufferError):                      # a non-contiguous memoryview
+            out.append(np.frombuffer(memoryview(x).tobytes(), dtype=np.uint8))
+    return out
+
+
+def restore_with(load, distributed: bool = False, device: int = 0):
+    """The decision of a restore. load(dry_run) runs amwg_checkpoint_load and returns "" or its refusal. With `distributed` every rank
+    validates first and the refusals are counted over all ranks: if any rank refuses, no rank commits, the refusing ranks raise their
+    own message and the others RESTORE_REFUSED_ELSEWHERE."""
+    if distributed:
+        err = load(True)
+        from .parallel import total_over_ranks
+        if total_over_ranks(1 if err else 0, device) > 0:
+            raise JsThrow(err or RESTORE_REFUSED_ELSEWHERE)
+    err = load(False)
+    if err:
+        raise JsThrow(err)
 
 
 def _default_device() -> int:
@@ -571,6 +606,41 @@ class AmwgSampler(Sampler):
                 raise JsThrow("set_state: " + name + " is of dimension [" + _js_join(list(a.shape)) + "] but should be [" + _js_join(dim) +
                               "] or [" + _js_join(per_chain) + "]")
         return out
+
+    def checkpoint(self) -> bytes:
+        """Not in the reference: the image of this handle's chains (with options.distributed: this rank's shard), from which `restore`
+        resumes the run bit for bit, in this or another process, on any sharding (DESIGN.md §2 "Checkpoints"). thin and monitor are
+        not part of it."""
+        L = _ffi.lib()
+        n = C.c_int64(0)
+        _ffi.check(L.amwg_checkpoint_size(self._handle, C.byref(n)))
+        buf = np.empty(n.value, dtype=np.uint8)
+        if L.amwg_checkpoint_save(self._handle, buf.ctypes.data, n.value) != 0:
+            raise JsThrow(L.amwg_last_error().decode())
+        return buf.tobytes()
+
+    def restore(self, images):
+        """Not in the reference: resume the run `images` were taken from (one bytes-like image, or a list of them, e.g. every rank's
+        file of an earlier run). The sampler must have the same model, data and options; the images together must cover its chains
+        (more is fine). Afterwards every chain continues exactly as it would have without the interruption, and `self.seed` is the
+        images' seed. A refused restore raises "restore: ..." and changes nothing. With options.distributed every rank checks its
+        images first and no rank changes unless all of them can."""
+        imgs = restore_images(images)
+        L = _ffi.lib()
+        ptrs = (C.c_void_p * len(imgs))(*[a.ctypes.data for a in imgs])
+        sizes = (C.c_int64 * len(imgs))(*[a.size for a in imgs])
+
+        def load(dry_run: bool) -> str:
+            rc = L.amwg_checkpoint_load(self._handle, ptrs, sizes, len(imgs), 1 if dry_run else 0)
+            return L.amwg_last_error().decode() if rc != 0 else ""
+        restore_with(load, self.distributed, self.device)
+        self.seed = int.from_bytes(imgs[0][32:40].tobytes(), "little")
+
+    def model_fingerprint(self) -> int:
+        """amwg_model_fingerprint of this sampler's lowered model (no device needed): what checkpoint images are matched against."""
+        out = C.c_uint64(0)
+        _ffi.check(_ffi.lib().amwg_model_fingerprint(C.byref(self._model_keepalive[-1]), C.byref(out)))
+        return int(out.value)
 
     def log_post(self):
         """mcmc.js:958-960 -- `sampler.log_post()`: log_post at the current state (one number, or one per chain)."""

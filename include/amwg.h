@@ -249,6 +249,23 @@ AMWG_API int amwg_get_log_post(amwg_sampler* s, double* host_out);
 AMWG_API int amwg_set_state(amwg_sampler* s, const double* host_in);
 AMWG_API int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_failed);
 
+/* Checkpoints (not in the reference): save the whole run state of a handle and resume it later, bit for bit, in this or another
+ * process, on any sharding of the chains (DESIGN.md §2 "Checkpoints" has the image layout and the guarantee).
+ * amwg_model_fingerprint: the 64-bit hash of everything in `model` except init (params, options, programs, constants, data, plates
+ *   and every table). Needs no device. amwg_create stores it in the handle; an image is only restored into a handle of the same
+ *   fingerprint. It detects accidents (another data set, another option, another lowering); it is not a security measure.
+ * amwg_checkpoint_size / amwg_checkpoint_save: the image of the handle's chains (state, prop_log_scale, acceptance counts,
+ *   substepper orders, stream positions) with the seed, the chain range and the adaptation counters; host_out holds cap bytes.
+ * amwg_checkpoint_load: images[k] (sizes[k] bytes) together must cover the handle's chains [first_chain, first_chain + n_chains),
+ *   without overlap, from one point of one run of the same model. Everything is checked on the host first; a refused restore
+ *   returns an error starting "restore: " and leaves the handle unchanged. With dry_run nothing else happens. Otherwise the
+ *   handle's chains, its seed (the images' seed is adopted) and its adaptation counters become the images', and log_post and the
+ *   term cache are evaluated afresh from the restored state. */
+AMWG_API int amwg_model_fingerprint(const amwg_model* model, uint64_t* out);
+AMWG_API int amwg_checkpoint_size(amwg_sampler* s, int64_t* out);
+AMWG_API int amwg_checkpoint_save(amwg_sampler* s, uint8_t* host_out, int64_t cap);
+AMWG_API int amwg_checkpoint_load(amwg_sampler* s, const uint8_t* const* images, const int64_t* sizes, int32_t n_images, int32_t dry_run);
+
 /* sampler.start_adaptation() / stop_adaptation() -- mcmc.js:1060-1073 */
 AMWG_API int amwg_set_adapting(amwg_sampler* s, int32_t flag);
 

@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -293,6 +294,48 @@ BINDING(disperse_state)
   if (amwg_disperse_state(handle_of(env, a.at(0))->s, to_double(env, a.at(1)), &failed) != 0 && failed == 0) fail_from_library();
   return js_number(env, (double)failed);
 END_BINDING
+// model_fingerprint(descriptor) -> 16 hex digits                                amwg_model_fingerprint (no device needed)
+BINDING(model_fingerprint)
+  Model M;
+  marshal(env, a.at(0), M);
+  uint64_t fp = 0;
+  if (amwg_model_fingerprint(&M.m, &fp) != 0) fail_from_library();
+  char hex[17];
+  snprintf(hex, sizeof hex, "%016llx", (unsigned long long)fp);
+  return js_string(env, hex);
+END_BINDING
+// checkpoint(handle) -> Uint8Array image (js/mcmc.js hands it out as a Buffer)   amwg_checkpoint_size + amwg_checkpoint_save
+BINDING(checkpoint)
+  Handle* h = handle_of(env, a.at(0));
+  int64_t n = 0;
+  if (amwg_checkpoint_size(h->s, &n) != 0) fail_from_library();
+  void* data = nullptr;
+  napi_value buf, ta;
+  check(env, napi_create_arraybuffer(env, (size_t)n, &data, &buf), "arraybuffer");
+  if (amwg_checkpoint_save(h->s, (uint8_t*)data, n) != 0) fail_from_library();
+  check(env, napi_create_typedarray(env, napi_uint8_array, (size_t)n, buf, 0, &ta), "Uint8Array");
+  return ta;
+END_BINDING
+// restore(handle, [Buffer | Uint8Array, ...], dry_run) -> the images' seed (a number: exact up to 2^53)   amwg_checkpoint_load
+BINDING(restore)
+  Handle* h = handle_of(env, a.at(0));
+  std::vector<const uint8_t*> images;
+  std::vector<int64_t> sizes;
+  for (uint32_t i = 0, n = length_of(env, a.at(1)); i < n; ++i) {
+    napi_value v = elem(env, a.at(1), i);
+    bool is_ta = false;
+    napi_is_typedarray(env, v, &is_ta);
+    napi_typedarray_type ty; size_t len = 0; void* data = nullptr;
+    if (is_ta) check(env, napi_get_typedarray_info(env, v, &ty, &len, &data, nullptr, nullptr), "typed array");
+    if (!is_ta || ty != napi_uint8_array) throw Throw{"restore expects a Buffer or a list of Buffers"};
+    images.push_back((const uint8_t*)data);
+    sizes.push_back((int64_t)len);
+  }
+  if (amwg_checkpoint_load(h->s, images.data(), sizes.data(), (int32_t)images.size(), to_double(env, a.at(2)) != 0 ? 1 : 0) != 0) fail_from_library();
+  uint64_t seed = 0;
+  std::memcpy(&seed, images[0] + 32, 8);              // the checked images all carry this seed (DESIGN.md §2 layout)
+  return js_number(env, (double)seed);
+END_BINDING
 // set_adapting(handle, flag)                                                    amwg_set_adapting (mcmc.js:1060-1073)
 BINDING(set_adapting)
   if (amwg_set_adapting(handle_of(env, a.at(0))->s, to_double(env, a.at(1)) != 0 ? 1 : 0) != 0) fail_from_library();
@@ -453,7 +496,8 @@ END_BINDING
 NAPI_MODULE_INIT() {
   const struct { const char* name; napi_callback fn; } table[] = {
       {"create", create}, {"destroy", destroy}, {"burn", burn}, {"sample", sample}, {"sample_device", sample_device}, {"get_state", get_state},
-      {"get_log_post", get_log_post}, {"set_state", set_state}, {"disperse_state", disperse_state}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
+      {"get_log_post", get_log_post}, {"set_state", set_state}, {"disperse_state", disperse_state},
+      {"model_fingerprint", model_fingerprint}, {"checkpoint", checkpoint}, {"restore", restore}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},

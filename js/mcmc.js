@@ -12,7 +12,8 @@
 // New, non-reference options: `chains` (default 1: output shaped exactly like the reference's), `seed`, `device`, `first_chain`,
 // `faithful` (no factorised likelihood plates: bit-faithful sums, slower), `scope` ({name: value} for identifiers log_post uses
 // from an enclosing scope that a recording from source cannot see), `init_radius` (over-dispersed starting points drawn on the
-// device, DESIGN.md §2). New method: `sampler.set_state(values)` places the chains anywhere.
+// device, DESIGN.md §2). New methods: `sampler.set_state(values)` places the chains anywhere; `sampler.checkpoint()` and
+// `sampler.restore(images)` stop and resume a run bit for bit.
 (function (root, factory) {
   if (typeof define === "function" && define.amd) { define(["./amwg_trace", "./amwg_native"], factory); }
   else if (typeof module === "object" && module.exports) { module.exports = factory(require("./amwg_trace"), require("./amwg_native")); }
@@ -365,6 +366,16 @@
   // Not in the reference: place the chains (from a previous run, prior draws, an optimiser). Shapes as state() returns them, or one
   // chain's value for all chains; parameters not named keep their values; adaptation and the random streams carry on untouched.
   AmwgSampler.prototype.set_state = function (values) { this.model.set_state(values); };
+  // Not in the reference: checkpoints (DESIGN.md §2). checkpoint() -> the image of this sampler's chains (a Buffer under Node);
+  // restore(image or [image, ...]) resumes, bit for bit, the run the images were taken from: same model, data and options, and
+  // images that together cover this sampler's chains (from any number of samplers). The sampler adopts the images' seed.
+  AmwgSampler.prototype.checkpoint = function () {
+    var img = native.checkpoint(this.model.handle);
+    return typeof Buffer === "function" ? Buffer.from(img.buffer, img.byteOffset, img.length) : img;
+  };
+  AmwgSampler.prototype.restore = function (images) {
+    this.model.seed = native.restore(this.model.handle, is_array(images) ? images : [images], 0);
+  };
   AmwgSampler.prototype.log_post = function () { var lp = native.get_log_post(this.model.handle); return this.n_chains === 1 ? lp[0] : lp; };
   AmwgSampler.prototype.start_adaptation = function () { native.set_adapting(this.model.handle, 1); };
   AmwgSampler.prototype.stop_adaptation = function () { native.set_adapting(this.model.handle, 0); };
