@@ -515,10 +515,7 @@ static std::string choose_shape(Plan& pl, unsigned off, size_t per_thread, unsig
   int best_t = 0, best_r = 1, best_ws = 0;
   double best_eff = -1.0;
   const int cands[] = {128, 64, 96, 160, 192, 224, 256};
-  int forced_t = 0;
-  if (const char* e = getenv("AMWG_JIT_THREADS")) { int t = atoi(e); if (t >= 32 && t <= 1024 && t % 32 == 0) forced_t = t; }
   for (int t : cands) {
-    if (forced_t) t = forced_t;
     const size_t need = pad16(per_thread * (size_t)t);
     const int ws_smem = need <= kJitWsSmemLimit;
     const unsigned smem = std::max((unsigned)(pad16(base) + (ws_smem ? need : 0)), 16u);
@@ -532,14 +529,12 @@ static std::string choose_shape(Plan& pl, unsigned off, size_t per_thread, unsig
     // 128-thread CTAs are the default; another size has to fill the SMs a good deal more evenly (15 % in `eff`) to be chosen,
     // because more, smaller CTAs overlap the CTA-wide phases of a sweep better than a few larger ones balanced more evenly
     if (eff > best_eff + (best_t == 0 ? 0.0 : 0.15)) { best_eff = eff; best_t = t; best_r = r_need; best_ws = ws_smem; }
-    if (forced_t) break;
   }
   if (!best_t) return "no launch shape fits";
   pl.threads = best_t;
   if (best_ws) { pl.ws_smem = 1; pl.ws_off = (int)pad16(off); off = (unsigned)(pad16(off) + pad16(per_thread * (size_t)best_t)); }
   pl.smem_bytes = std::max(off, 16u);
   pl.minblocks = std::max(1, best_r);
-  if (const char* e = getenv("AMWG_JIT_MINBLOCKS")) { int v = atoi(e); if (v >= 1 && v <= 16) pl.minblocks = v; }
   return "";
 }
 
@@ -791,7 +786,6 @@ static std::string build_source(const amwg_model* md, const std::vector<double>&
       }
     if (indep) { jblock = p; best = pa.n_comp; }
   }
-  if (const char* e = getenv("AMWG_JIT_BLOCK")) { if (atoi(e) == 0) jblock = -1; }
   const bool jblock_free = jblock >= 0 && md->params[jblock].lower == -INFINITY && md->params[jblock].upper == INFINITY;
   std::ostringstream pre;
   pre << "#define JBLOCK " << jblock << "\n#define JBLOCK_FREE " << (jblock_free ? 1 : 0) << "\n";
@@ -802,10 +796,6 @@ static std::string build_source(const amwg_model* md, const std::vector<double>&
       << "#define JSTREAM " << (pl.stream_col >= 0 ? 1 : 0) << "\n#define JS_COL " << std::max(pl.stream_col, 0) << "\n#define JS_BEGIN " << s_begin << "\n#define JS_TOTAL " << s_total << "\n"
       << "#define JN_SSTAT " << s_entries.size() << "\n#define JRING_OFF " << pl.ring_off << "u\n#define JRING_STAGES " << pl.ring_stages << "\n#define JRING_TILE " << pl.ring_tile << "\n"
       << "#define JNORM_C0 " << lit(norm_c0) << "\n#define AMWG_REAL 0\n#define AMWG_INT 1\n#define AMWG_BINARY 2\n";
-  // accumulators of the plate loop: four by default (AMWG_JIT_NACC=8 selects eight, for A/B runs)
-  int nacc = 4;
-  if (const char* e = getenv("AMWG_JIT_NACC")) { int v = atoi(e); if (v == 4 || v == 8) nacc = v; }
-  pre << "#define AMWG_NACC " << nacc << "\n";
 
   src.prelude = pre.str();
   funcs << tables.str() << step.str() << extra.str() << dfun.str() << "}  // namespace amwg\n";
@@ -947,7 +937,7 @@ static std::string build_source_full(const amwg_model* md, const std::vector<dou
   pre << "#define JFULL 1\n#define JD " << D << "\n#define JP " << P << "\n#define JTHREADS " << pl.threads << "\n#define JMINB " << pl.minblocks
       << "\n#define JWS_SMEM " << pl.ws_smem << "\n#define JWS_OFF " << pl.ws_off << "\n#define JN_DERIVED " << md->n_derived << "\n#define JMAX_DIM0 " << max_dim0
       << "\n#define JMAXCOL " << kMaxColumns << "\n#define JN_BERN " << bm_plate.size() << "\n#define JN_RES " << pl.n_res << "\n#define JRES_TOTAL_BYTES " << res_total << "u\n#define JNORM_C0 " << lit(norm_c0)
-      << "\n#define AMWG_REAL 0\n#define AMWG_INT 1\n#define AMWG_BINARY 2\n#define AMWG_NACC 4\n";
+      << "\n#define AMWG_REAL 0\n#define AMWG_INT 1\n#define AMWG_BINARY 2\n";
   src.prelude = pre.str();
   // the generated header: parameter / staging tables and constants, tables the programs index, then the programs and their dispatch
   src.generated = "namespace amwg {\n#define LD(o) lds_f64_sa(smem_u32(smem) + (o))\n" + t2.str() + tables.str() + funcs.str() + "}  // namespace amwg\n";

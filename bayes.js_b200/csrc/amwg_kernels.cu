@@ -41,14 +41,8 @@ constexpr int kMaxParams = 255;      // substepper order: packed 4 bits per name
 constexpr int kMaxDim0 = 65535;      // top-level visit order of a multi-dim parameter: local bytes up to 256, 16-bit rows in global memory beyond
 constexpr int kMaxDerived = 32;
 constexpr int kStack = 32;          // operand stack of the interpreter; validate_model rejects programs that need more
-#ifndef AMWG_THREADS
-#define AMWG_THREADS 128
-#endif
-constexpr int kThreads = AMWG_THREADS;
-#ifndef AMWG_SYNC_THREADS
-#define AMWG_SYNC_THREADS 128
-#endif
-constexpr int kSyncThreads = AMWG_SYNC_THREADS;   // CTA size of the phase-synchronised sweep kernel
+constexpr int kThreads = 128;       // CTA size of the per-chain kernels (one thread per chain)
+constexpr int kMinBlocks = 7;       // resident CTAs per SM the sweep kernels are compiled for (register cap)
 constexpr int kAdaptChunk = 64;
 constexpr long long kHostChunkSweeps = 10;       // sample() to a host buffer: sweeps per launch, so copies overlap compute at this granularity
 constexpr unsigned kSmemBudget = 200u * 1024u;   // bytes of dynamic shared memory we are willing to fill with data
@@ -66,7 +60,6 @@ struct ModelDev {
   int block_params[AMWG_MAX_BLOCK_PARAMS];
   unsigned off_tbc;                // image offset of term_block_comp [n_block_params][n_terms]
   int stat_prog;                   // >= 0: sweeps run with pre-evaluated plate statistics (amwg_model.stat_prog), by amwg_stat_sweep_kernel
-  int stat_barriers;               // CTA barriers between the phases of a statistics sweep (instruction-cache locality)
   int scratch_smem_off;            // >= 0: byte offset in dynamic smem of the CTA's per-chain working set (amwg_stat_sweep_kernel), -1: global rows
   const double* col_global[kMaxColumns];
   unsigned col_bytes[kMaxColumns];     // padded to 16
@@ -841,11 +834,8 @@ __global__ void __launch_bounds__(kThreads) amwg_disperse_kernel(ModelDev m, Cha
 // scheduler then execute the same few hundred instructions together (instruction-cache hits instead of every warp streaming
 // the whole sweep body past the others), while the CTAs resident on one SM drift apart and overlap their fp64 loops with each
 // other's bookkeeping. Threads past the last chain shadow chain C-1 and write nothing, so they can take part in the barriers.
-#ifndef AMWG_MINBLOCKS
-#define AMWG_MINBLOCKS 7
-#endif
 template <bool CACHE>
-__global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
+__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -1070,7 +1060,7 @@ __global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_sweep_kerne
 // the whole launch, one column per thread (row stride = CTA size, conflict-free): state and term cache are read from HBM once
 // per launch and written back once, the per-sweep temporaries never leave the SM. Otherwise the rows are the global arrays
 // (row stride = C), which amwg_create lays out back to back in the same order.
-__global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_stat_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
+__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -1085,9 +1075,9 @@ __global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_stat_sweep_
   const bool in_smem = m.scratch_smem_off >= 0;
   // rows of the working set: wk[row * ws]; state rows: sp[c * ss]
   double* wk = in_smem ? reinterpret_cast<double*>(smem + m.scratch_smem_off) + threadIdx.x : a.tval + chain;
-  const unsigned long long ws = in_smem ? (unsigned long long)kSyncThreads : C;
+  const unsigned long long ws = in_smem ? (unsigned long long)kThreads : C;
   double* sp = in_smem ? wk + (unsigned long long)(2 * NT + 2 * D) * ws : a.state + chain;
-  unsigned short* vq = in_smem ? reinterpret_cast<unsigned short*>(smem + m.scratch_smem_off + (size_t)(2 * NT + 3 * D) * kSyncThreads * sizeof(double)) + threadIdx.x
+  unsigned short* vq = in_smem ? reinterpret_cast<unsigned short*>(smem + m.scratch_smem_off + (size_t)(2 * NT + 3 * D) * kThreads * sizeof(double)) + threadIdx.x
                                : a.vseq + chain;
   const int rTC = NT, rBP = 2 * NT, rBC = 2 * NT + D;           // first rows of tcand, bprop, bcoin
   if (in_smem) {
@@ -1126,7 +1116,7 @@ __global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_stat_sweep_
       if (rec_now) ++row;
     }
     // ---- (a) this sweep's random numbers, in the reference's order
-    if (m.stat_barriers) __syncthreads();
+    __syncthreads();
     for (int i = P - 1; i > 0; --i) {                           // shuffle_array(this.substeppers), in place (mcmc.js:887, 228-236)
       int j = (int)floor(g.next(a.seed, gchain) * (i + 1));
       perm_swap(a, perm, chain, i, j, valid);
@@ -1160,7 +1150,7 @@ __global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_stat_sweep_
       }
     }
     // ---- (b) one pass over the data: every plate statistic at the proposals -> candidate slots
-    if (m.stat_barriers) __syncthreads();
+    __syncthreads();
     {
       EvalState es{sp, ws, -1, 0.0};
       es.tval = wr ? wk : nullptr;                              // a shadow of a global column computes along (barriers) and stores nothing
@@ -1172,7 +1162,7 @@ __global__ void __launch_bounds__(kSyncThreads, AMWG_MINBLOCKS) amwg_stat_sweep_
     int c_next = (int)vq[0];
     double coin_next = wk[(unsigned long long)(rBC + c_next) * ws], prop_next = wk[(unsigned long long)(rBP + c_next) * ws];
     for (int i = 0; i < D; ++i) {
-      if (m.stat_barriers && D <= 8) __syncthreads();           // few steps: keep the CTA's warps in the same code (instruction cache)
+      if (D <= 8) __syncthreads();                              // few steps: keep the CTA's warps in the same code (instruction cache)
       const int c = c_next;
       const double coin = coin_next, prop = prop_next;
       if (i + 1 < D) {                                          // the next step's operands are on their way while this one is evaluated
@@ -1648,8 +1638,6 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
     if (const char* e = getenv("AMWG_STAT_SWEEP")) off = off || atoi(e) == 0;
     if (off) { m.stat_prog = -1; m.n_terms = 0; m.n_block_params = 0; }
   }
-  m.stat_barriers = 1;
-  if (const char* e = getenv("AMWG_STAT_BARRIERS")) m.stat_barriers = atoi(e) != 0;
   m.image_bytes = (unsigned)image.size();
   unsigned char* d_image = nullptr;
   if (dev_upload(s, image.data(), image.size(), &d_image)) return bail(-1);
@@ -1697,10 +1685,8 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
   m.scratch_smem_off = -1;
   if (m.stat_prog >= 0) {
     const size_t per_thread = sizeof(double) * (size_t)(2 * m.n_terms + 3 * md->n_comp) + sizeof(unsigned short) * (size_t)md->n_comp;
-    const size_t need = pad16(per_thread * kSyncThreads);
-    bool use = pad16(smem_used) + need <= (227u * 1024u) / 7u - 1024u;
-    if (const char* e = getenv("AMWG_STAT_SMEM")) use = use && atoi(e) != 0;
-    if (use) { m.scratch_smem_off = (int)pad16(smem_used); smem_used = (unsigned)(pad16(smem_used) + need); }
+    const size_t need = pad16(per_thread * kThreads);
+    if (pad16(smem_used) + need <= (227u * 1024u) / kMinBlocks - 1024u) { m.scratch_smem_off = (int)pad16(smem_used); smem_used = (unsigned)(pad16(smem_used) + need); }
   }
   s->smem_bytes = smem_used;
   if (cudaFuncSetAttribute(amwg_sweep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
@@ -1796,10 +1782,9 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
       void* kargs[] = {&ja};
       CUDA_TRY(cudaLaunchKernel((const void*)s->jit_kernel, dim3(grid_for(C, s->jit_threads)), dim3((unsigned)s->jit_threads), kargs, s->jit_smem, s->stream));
     } else {
-      const int threads = s->m.phase_sync ? kSyncThreads : kThreads;
-      if (s->m.stat_prog >= 0) amwg_stat_sweep_kernel<<<grid_for(C, kSyncThreads), kSyncThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
-      else if (s->m.n_terms > 0) amwg_sweep_kernel<true><<<grid_for(C, threads), threads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
-      else amwg_sweep_kernel<false><<<grid_for(C, threads), threads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
+      if (s->m.stat_prog >= 0) amwg_stat_sweep_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
+      else if (s->m.n_terms > 0) amwg_sweep_kernel<true><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
+      else amwg_sweep_kernel<false><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
     }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(s->ev_pool[n_events].second, s->stream));

@@ -95,24 +95,9 @@ __device__ __forceinline__ double2 lds_f64x2(unsigned saddr) {
 __device__ __forceinline__ double lds_f64_sa(unsigned saddr) { double v; asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(saddr)); return v; }
 
 // ---- plates: the O(N) likelihood sums -----------------------------------------------------------------------------
-// sum_i (x_i - mean)^2 : 2 fp64-pipe instructions per point (DADD + DFMA), AMWG_NACC independent accumulators, eight points
+// sum_i (x_i - mean)^2 : 2 fp64-pipe instructions per point (DADD + DFMA), four independent accumulators, eight points
 // per block read as four 16-byte warp-broadcast loads (ld.shared.v2.f64 when `saddr` != 0, i.e. the column sits in shared
-// memory; else the same loop over global/L2 addresses). AMWG_PREFETCH: the next block is loaded while the current one is summed.
-#ifndef AMWG_NACC
-#define AMWG_NACC 4
-#endif
-#ifndef AMWG_PREFETCH
-#define AMWG_PREFETCH 1
-#endif
-#if AMWG_NACC == 8
-#define AMWG_ACC8(P0, P1, P2, P3)                                                                              \
-  {                                                                                                            \
-    double d0 = P0.x - mean, d1 = P0.y - mean, d2 = P1.x - mean, d3 = P1.y - mean;                             \
-    double d4 = P2.x - mean, d5 = P2.y - mean, d6 = P3.x - mean, d7 = P3.y - mean;                             \
-    s0 = fma(d0, d0, s0); s1 = fma(d1, d1, s1); s2 = fma(d2, d2, s2); s3 = fma(d3, d3, s3);                     \
-    s4 = fma(d4, d4, s4); s5 = fma(d5, d5, s5); s6 = fma(d6, d6, s6); s7 = fma(d7, d7, s7);                     \
-  }
-#else
+// memory; else the same loop over global/L2 addresses). From shared memory the next block is loaded while the current one is summed.
 #define AMWG_ACC8(P0, P1, P2, P3)                                                                              \
   {                                                                                                            \
     double d0 = P0.x - mean, d1 = P0.y - mean, d2 = P1.x - mean, d3 = P1.y - mean;                             \
@@ -120,19 +105,14 @@ __device__ __forceinline__ double lds_f64_sa(unsigned saddr) { double v; asm vol
     s0 = fma(d0, d0, s0); s1 = fma(d1, d1, s1); s2 = fma(d2, d2, s2); s3 = fma(d3, d3, s3);                     \
     s0 = fma(d4, d4, s0); s1 = fma(d5, d5, s1); s2 = fma(d6, d6, s2); s3 = fma(d7, d7, s3);                     \
   }
-#endif
 __device__ __forceinline__ double sum_sq_dev(const double* __restrict__ x, unsigned saddr, int n, double mean) {
   double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-#if AMWG_NACC == 8
-  double s4 = 0.0, s5 = 0.0, s6 = 0.0, s7 = 0.0;
-#endif
   int i = 0;
   if ((reinterpret_cast<unsigned long long>(x) & 15ull) && n > 0) { double d = x[0] - mean; s3 = fma(d, d, s3); i = 1; }   // 16B-align the vector loads
   const int nb = (n - i) >> 3;                 // blocks of eight points
   if (nb > 0) {
     if (saddr) {
       unsigned a = saddr + 8u * (unsigned)i;
-#if AMWG_PREFETCH
       double2 p0 = lds_f64x2(a), p1 = lds_f64x2(a + 16u), p2 = lds_f64x2(a + 32u), p3 = lds_f64x2(a + 48u);
 #pragma unroll 2
       for (int b = 1; b < nb; ++b) {
@@ -142,13 +122,6 @@ __device__ __forceinline__ double sum_sq_dev(const double* __restrict__ x, unsig
         p0 = q0; p1 = q1; p2 = q2; p3 = q3;
       }
       AMWG_ACC8(p0, p1, p2, p3)
-#else
-#pragma unroll 2
-      for (int b = 0; b < nb; ++b, a += 64u) {
-        double2 p0 = lds_f64x2(a), p1 = lds_f64x2(a + 16u), p2 = lds_f64x2(a + 32u), p3 = lds_f64x2(a + 48u);
-        AMWG_ACC8(p0, p1, p2, p3)
-      }
-#endif
     } else {
       const double2* g = reinterpret_cast<const double2*>(x + i);
 #pragma unroll 2
@@ -160,11 +133,7 @@ __device__ __forceinline__ double sum_sq_dev(const double* __restrict__ x, unsig
     i += nb << 3;
   }
   for (; i < n; ++i) { double d = x[i] - mean; s0 = fma(d, d, s0); }
-#if AMWG_NACC == 8
-  return ((s0 + s1) + (s2 + s3)) + ((s4 + s5) + (s6 + s7));
-#else
   return (s0 + s1) + (s2 + s3);
-#endif
 }
 #undef AMWG_ACC8
 

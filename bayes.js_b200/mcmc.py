@@ -21,8 +21,6 @@ import copy
 import ctypes as C
 import math
 import os
-import sys
-import time
 from typing import Any, Dict, List, Optional
 
 import numpy as np
@@ -741,22 +739,15 @@ class AmwgSampler(Sampler):
             if need + 2 * len(entries) * self.local_chains * 8 + scratch > 0.9 * free:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
                               "device memory; raise thin() or lower n" % (need / 1e9, scratch / 1e9))
-        timing = os.environ.get("AMWG_SUMMARY_TIMING") == "1"
-        t0 = time.perf_counter()
         block = torch.empty((rows, len(entries), self.local_chains), dtype=torch.float64, device=dev)
         mon = np.asarray(entries, dtype=np.int32)
-        torch.cuda.current_stream(dev).synchronize()
-        t1 = time.perf_counter()
+        torch.cuda.current_stream(dev).synchronize()   # the library writes `block` on its own stream: torch's queued work goes first
         rc = L.amwg_sample_device(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(entries), block.data_ptr())
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
-        t2 = time.perf_counter()
         res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
         del block
-        if timing:
-            print("sample_summary: alloc %.2f ms, sweeps %.2f ms, reductions %.2f ms" %
-                  (1e3 * (t1 - t0), 1e3 * (t2 - t1), 1e3 * (time.perf_counter() - t2)), file=sys.stderr, flush=True)
         out = {}
         for name in monitored:
             s0, ln = spans[name]
