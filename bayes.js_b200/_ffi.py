@@ -68,7 +68,7 @@ EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_samp
            "amwg_last_error", "amwg_abi_version", "amwg_ld_eval", "amwg_primitive_eval",
            "amwg_summary_moments", "amwg_summary_digit_hist", "amwg_summary_autocov", "amwg_summary_rank_sort",
            "amwg_summary_rank_count", "amwg_summary_rank_z", "amwg_peak_fp64", "amwg_jit_status", "amwg_jit_compile_check",
-           "amwg_plate_sources"]
+           "amwg_plate_sources", "amwg_get_term_cache"]
 
 _lib = None
 
@@ -119,6 +119,7 @@ def lib():
     L.amwg_summary_rank_z.argtypes = [C.c_int, vp, vp, i64, i64, vp]; L.amwg_summary_rank_z.restype = C.c_int
     L.amwg_jit_status.argtypes = [vp, C.c_char_p, i64]; L.amwg_jit_status.restype = C.c_int
     L.amwg_plate_sources.argtypes = [vp, C.c_char_p, i64]; L.amwg_plate_sources.restype = C.c_int
+    L.amwg_get_term_cache.argtypes = [vp, vp, i64]; L.amwg_get_term_cache.restype = C.c_int
     L.amwg_jit_compile_check.argtypes = [C.POINTER(AmwgModel), u64, C.c_char_p, i64, C.c_char_p, i64]; L.amwg_jit_compile_check.restype = C.c_int
     L.amwg_peak_fp64.argtypes = [C.c_int, C.c_int, pd, pd]; L.amwg_peak_fp64.restype = C.c_int
     if L.amwg_abi_version() != ABI_VERSION:

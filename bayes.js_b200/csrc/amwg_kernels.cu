@@ -2106,6 +2106,20 @@ extern "C" int amwg_plate_sources(const amwg_sampler* s, char* out, int64_t cap)
   return s->plate_note.empty() ? 0 : 1 + (int)std::count(s->plate_note.begin(), s->plate_note.end(), ',');
 }
 
+// the term cache a.tval ([n_terms][C]) to the host; returns n_terms, 0 when the handle keeps no cache (amwg_get_term_cache)
+extern "C" int amwg_get_term_cache(amwg_sampler* s, double* host_out, int64_t cap) {
+  if (!s) return fail("amwg_get_term_cache: NULL handle");
+  const int NT = s->m.n_terms;
+  if (NT <= 0 || !s->a.tval) return 0;
+  const size_t n = (size_t)NT * (size_t)s->a.C;
+  if (!host_out || cap < 0 || (uint64_t)cap < n)
+    return fail("amwg_get_term_cache: the buffer holds " + std::to_string(cap) + " values, the cache has " + std::to_string(n));
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaMemcpyAsync(host_out, s->a.tval, sizeof(double) * n, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return NT;
+}
+
 // Generate and compile the specialised sweep of `model` without a GPU (NVRTC targets sm_90a from any host): 0 = compiled,
 // 1 = the model is not eligible (reason in `log`), -1 = generation or compilation failed (message in `log`). `src`, when given,
 // receives the generated source. Constants that the device would fold at create are left as they are in the model; the launch

@@ -830,6 +830,17 @@ class AmwgSampler(Sampler):
         n = _ffi.lib().amwg_plate_sources(self._handle, buf, len(buf))
         return buf.value.decode().split(",") if n > 0 else []
 
+    def _term_cache(self) -> np.ndarray:
+        """The term cache as the sweep kernels left it, [n_terms, chains] (amwg_get_term_cache; [0, chains] without one). Slots below
+        the program's n_sum_terms are terms of the sum, the rest plate statistics S, all at each chain's current state."""
+        nt = int(self._program.n_terms)
+        buf = np.empty((max(nt, 1), self.local_chains))
+        L = _ffi.lib()
+        got = L.amwg_get_term_cache(self._handle, buf.ctypes.data, buf.size)
+        if got < 0:
+            raise _ffi.AmwgError(L.amwg_last_error().decode("utf-8", "replace"))
+        return buf[:got]
+
     def jit_compile_check(self, n_chains=None):
         """Generate and compile the specialised sweep of this model without running it (works without a GPU).
         -> (rc, message, source): rc 0 compiled, 1 model not eligible, -1 error."""

@@ -354,6 +354,12 @@ AMWG_API int amwg_jit_compile_check(const amwg_model* model, uint64_t n_chains, 
  * order, comma-separated: "shared" (resident), "ring" (the TMA tile ring), "L2" (global loads) or "loop" (a bytecode plate).
  * Returns the number of plates. */
 AMWG_API int amwg_plate_sources(const amwg_sampler* s, char* out, int64_t cap);
+/* amwg_get_term_cache (read-only; for tests of the cached values): copies the term cache, host_out[t][chain] for t < n_terms
+ * (amwg_model.n_terms), to the host and returns n_terms; 0 for a handle that keeps no term cache. Slots 0 .. n_sum_terms-1 hold
+ * the terms of the sum at the chain's current state; with stat_prog, slots n_sum_terms .. n_terms-1 hold each plate statistic S
+ * at the current state. The sweep kernels write the cache back at the end of every launch, so it is current whenever
+ * amwg_burn / amwg_sample have returned. An error (with a message) when cap, the number of doubles host_out holds, is too small. */
+AMWG_API int amwg_get_term_cache(amwg_sampler* s, double* host_out, int64_t cap);
 
 /* ---- measurement ---------------------------------------------------------------------------------------------------------
  * The binding roof of this path is the non-tensor fp64 pipe (DADD + DFMA per data point), which MEASURED_PEAKS.json does not

@@ -478,6 +478,14 @@ BINDING(plate_sources)
   amwg_plate_sources(handle_of(env, a.at(0))->s, out, sizeof out);
   return js_string(env, out);
 END_BINDING
+// term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
+BINDING(term_cache)
+  Handle* h = handle_of(env, a.at(0));
+  std::vector<double> out((size_t)to_u64(env, a.at(1)) * (size_t)h->n_chains);
+  const int nt = amwg_get_term_cache(h->s, out.data(), (int64_t)out.size());
+  if (nt < 0) fail_from_library();
+  return f64_array(env, out.data(), (size_t)nt * (size_t)h->n_chains);
+END_BINDING
 // jit_compile_check(descriptor, n_chains) -> {rc, log}                           amwg_jit_compile_check
 BINDING(jit_compile_check)
   Model M;
@@ -502,7 +510,7 @@ NAPI_MODULE_INIT() {
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
-      {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources},
+      {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
     napi_value fn;

@@ -404,6 +404,7 @@ typedef struct orc_sampler {
   int64_t thinning_interval;
   int64_t n_logpost_calls;            /* instrumentation: how many evals the reference does */
   int* scratch;
+  double* trace; int64_t trace_cap, trace_len;   /* optional step trace (orc_trace) */
 } orc_sampler;
 
 static double call_log_post(orc_sampler* s) { s->n_logpost_calls++; return s->fn(s->state, s->data, s->user); }
@@ -414,6 +415,9 @@ static void onedim_step(orc_sampler* s, onedim_t* st) {
   /* generate_proposal: normal_proposal (:577-579) / discrete_normal_proposal (:596-598) */
   double param_proposal = rnorm_(&s->rng, param_state, orc_exp(st->prop_log_scale));
   if (st->is_int) param_proposal = orc_js_round(param_proposal);
+  double* rec = (s->trace && s->trace_len < s->trace_cap) ? s->trace + 6 * s->trace_len : NULL;
+  if (s->trace) s->trace_len++;
+  if (rec) { rec[0] = st->comp; rec[1] = param_state; rec[2] = param_proposal; rec[3] = -1.0; rec[4] = NAN; rec[5] = NAN; }
   if (param_proposal < st->lower || param_proposal > st->upper) {
     /* outside the limits: reject, no log_post, no accept uniform (:520-522) */
   } else {
@@ -421,7 +425,9 @@ static void onedim_step(orc_sampler* s, onedim_t* st) {
     s->state[st->comp] = param_proposal;
     double prop_log_dens = call_log_post(s);
     double accept_prob = orc_exp(prop_log_dens - curr_log_dens);
-    if (accept_prob > rng_next(&s->rng)) {
+    double u = rng_next(&s->rng);
+    if (rec) { rec[3] = u; rec[4] = curr_log_dens; rec[5] = prop_log_dens; }
+    if (accept_prob > u) {
       if (st->is_adapting) st->acceptance_count++;
     } else {
       s->state[st->comp] = param_state;
@@ -546,6 +552,16 @@ ORC_API void orc_destroy(orc_sampler* s) {
 }
 
 ORC_API void orc_set_replay(orc_sampler* s, const double* tape, uint64_t len) { s->rng.replay = tape; s->rng.replay_len = len; s->rng.n = 0; }
+/* Step trace (tests): from now on every OnedimMetropolisStepper step appends one row of six doubles to buf (room for cap rows):
+ * component, current value, proposal, accept uniform (-1 when the proposal is out of bounds and none is drawn), curr_log_dens,
+ * prop_log_dens (both NaN without evaluation). Steps beyond cap are counted but not written; buf NULL switches the trace off.
+ * Returns the number of rows so far. */
+ORC_API int64_t orc_trace(orc_sampler* s, double* buf, int64_t cap) {
+  if (buf != s->trace) s->trace_len = 0;
+  s->trace = buf; s->trace_cap = buf ? cap : 0;
+  return s->trace_len;
+}
+ORC_API int64_t orc_trace_len(const orc_sampler* s) { return s->trace_len; }
 ORC_API uint64_t orc_rng_position(const orc_sampler* s) { return s->rng.n; }
 ORC_API int64_t orc_logpost_calls(const orc_sampler* s) { return s->n_logpost_calls; }
 ORC_API void orc_thin(orc_sampler* s, int64_t k) { s->thinning_interval = k; }          /* mcmc.js:1053-1055 */
@@ -705,17 +721,19 @@ ORC_API double orc_model_hier_binom(double* st, const void* data, void* user) {
 }
 
 /* Many independent chains of one built-in model, optionally threaded by the caller (bench.py's CPU
- * baseline): runs chains [chain0, chain0+n_chains) burn + sample and writes out[chain][row][n_monitor]. */
+ * baseline): runs chains [chain0, chain0+n_chains) burn + sample and writes out[chain][row][n_monitor], and, when final is not
+ * NULL, each chain's state at the end, final[chain][D + n_derived]. */
 ORC_API void orc_run_chains(int n_params, const orc_param* params, const double* init, const orc_comp_options* opts,
                             int n_derived, orc_logpost_fn fn, const void* data, uint64_t seed,
                             uint64_t chain0, int64_t n_chains, int64_t n_burn, int64_t n_sample, int64_t thin,
-                            const int32_t* monitor, int n_monitor, double* out) {
+                            const int32_t* monitor, int n_monitor, double* out, double* final) {
   int64_t rows = (n_sample + thin - 1) / thin;
   for (int64_t c = 0; c < n_chains; c++) {
     orc_sampler* s = orc_create(n_params, params, init, opts, n_derived, fn, data, 0, seed, chain0 + (uint64_t)c);
     orc_thin(s, thin);
     orc_burn(s, n_burn);
     if (n_sample > 0) orc_sample(s, n_sample, monitor, n_monitor, out + (size_t)c * (size_t)rows * (size_t)n_monitor);
+    if (final) memcpy(final + (size_t)c * (size_t)(s->D + n_derived), s->state, sizeof(double) * (size_t)(s->D + n_derived));
     orc_destroy(s);
   }
 }
@@ -727,6 +745,7 @@ ORC_API void orc_run_chains(int n_params, const orc_param* params, const double*
 typedef struct {
   int n_params; const orc_param* params; const double* init; const orc_comp_options* opts; int n_derived; orc_logpost_fn fn;
   const void* data; uint64_t seed, chain0; int64_t c_lo, c_hi, n_burn, n_sample, thin; const int32_t* monitor; int n_monitor; double* out;
+  double* final; int width;
 } orc_mt_job;
 static void* orc_mt_worker(void* arg) {
   orc_mt_job* j = (orc_mt_job*)arg;
@@ -734,13 +753,16 @@ static void* orc_mt_worker(void* arg) {
   if (j->c_hi > j->c_lo)
     orc_run_chains(j->n_params, j->params, j->init, j->opts, j->n_derived, j->fn, j->data, j->seed, j->chain0 + (uint64_t)j->c_lo,
                    j->c_hi - j->c_lo, j->n_burn, j->n_sample, j->thin, j->monitor, j->n_monitor,
-                   j->out ? j->out + (size_t)j->c_lo * (size_t)rows * (size_t)j->n_monitor : NULL);
+                   j->out ? j->out + (size_t)j->c_lo * (size_t)rows * (size_t)j->n_monitor : NULL,
+                   j->final ? j->final + (size_t)j->c_lo * (size_t)j->width : NULL);
   return NULL;
 }
 ORC_API int orc_run_chains_mt(int n_params, const orc_param* params, const double* init, const orc_comp_options* opts,
                               int n_derived, orc_logpost_fn fn, const void* data, uint64_t seed,
                               uint64_t chain0, int64_t n_chains, int64_t n_burn, int64_t n_sample, int64_t thin,
-                              const int32_t* monitor, int n_monitor, double* out, int n_threads) {
+                              const int32_t* monitor, int n_monitor, double* out, double* final, int n_threads) {
+  int width = n_derived;
+  for (int p = 0; p < n_params; p++) width += params[p].n_comp;
   if (n_threads < 1) n_threads = 1;
   if ((int64_t)n_threads > n_chains) n_threads = (int)n_chains;
   pthread_t* th = (pthread_t*)malloc(sizeof(pthread_t) * (size_t)n_threads);
@@ -748,7 +770,8 @@ ORC_API int orc_run_chains_mt(int n_params, const orc_param* params, const doubl
   int started = 0;
   for (int t = 0; t < n_threads; t++) {
     orc_mt_job j = { n_params, params, init, opts, n_derived, fn, data, seed, chain0,
-                     n_chains * t / n_threads, n_chains * (t + 1) / n_threads, n_burn, n_sample, thin, monitor, n_monitor, out };
+                     n_chains * t / n_threads, n_chains * (t + 1) / n_threads, n_burn, n_sample, thin, monitor, n_monitor, out,
+                     final, width };
     jobs[t] = j;
     if (pthread_create(&th[t], NULL, orc_mt_worker, &jobs[t]) != 0) break;
     started++;

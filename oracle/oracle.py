@@ -89,9 +89,11 @@ def lib():
     L.orc_set_replay.restype = None; L.orc_set_replay.argtypes = [vp, vp, u64]
     L.orc_substepper_order.restype = None; L.orc_substepper_order.argtypes = [vp, vp]
     L.orc_run_chains.restype = None
-    L.orc_run_chains.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, u64, u64, i64, i64, i64, i64, vp, C.c_int, vp]
+    L.orc_run_chains.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, u64, u64, i64, i64, i64, i64, vp, C.c_int, vp, vp]
     L.orc_run_chains_mt.restype = C.c_int
-    L.orc_run_chains_mt.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, u64, u64, i64, i64, i64, i64, vp, C.c_int, vp, C.c_int]
+    L.orc_run_chains_mt.argtypes = [C.c_int, vp, vp, vp, C.c_int, vp, vp, u64, u64, i64, i64, i64, i64, vp, C.c_int, vp, vp, C.c_int]
+    L.orc_trace.restype = i64; L.orc_trace.argtypes = [vp, vp, i64]
+    L.orc_trace_len.restype = i64; L.orc_trace_len.argtypes = [vp]
     _lib = L
     return L
 
@@ -302,6 +304,21 @@ class OracleSampler:
     def logpost_calls(self) -> int:
         return int(lib().orc_logpost_calls(self.h))
 
+    TRACE_FIELDS = ("comp", "current", "proposal", "u", "curr_log_dens", "prop_log_dens")
+
+    def trace(self, cap: int):
+        """Record every Metropolis step from now on (orc_trace), up to `cap` steps: one row per step of TRACE_FIELDS -- the
+        component, its current value, the proposal, the accept uniform (-1: the proposal is out of bounds, no uniform drawn) and
+        log_post at the current state and at the proposal (NaN when not evaluated)."""
+        self._trace = np.full((int(cap), 6), np.nan)
+        lib().orc_trace(self.h, self._trace.ctypes.data, int(cap))
+
+    def trace_rows(self) -> np.ndarray:
+        """the rows recorded since trace(); fails if more steps were taken than it has room for"""
+        n = int(lib().orc_trace_len(self.h))
+        assert n <= self._trace.shape[0], f"{n} steps traced, room for {self._trace.shape[0]}"
+        return self._trace[:n].copy()
+
     def substepper_order(self) -> List[int]:
         out = np.empty(len(self.params), dtype=np.int32)
         lib().orc_substepper_order(self.h, out.ctypes.data)
@@ -310,9 +327,10 @@ class OracleSampler:
 
 def run_model(model: str, data, params: Dict[str, dict], chains: int = 1, seed: int = 0, burn: int = 0, sample: int = 0,
               thin: int = 1, first_chain: int = 0, comp_options: Optional[Dict[str, dict]] = None,
-              monitor: Optional[List[str]] = None, threads: int = 1) -> Dict[str, np.ndarray]:
+              monitor: Optional[List[str]] = None, threads: int = 1, final_state: bool = False):
     """`chains` independent oracle chains of a built-in model; output shaped like mcmc.AmwgSampler.sample():
-    [rows, *dim] for one chain, [rows, chains, *dim] otherwise."""
+    [rows, *dim] for one chain, [rows, chains, *dim] otherwise. With final_state, returns (that, [chains, D + n_derived] the state
+    each chain ends in)."""
     L = lib()
     cp, prm, init, opts, D = _layout(params, comp_options)
     cfn, st, keep, derived = _model(model, data)
@@ -334,9 +352,11 @@ def run_model(model: str, data, params: Dict[str, dict], chains: int = 1, seed: 
     mon = np.asarray(ent, dtype=np.int32)
     rows = (sample + thin - 1) // thin if sample > 0 else 0
     out = np.empty((chains, max(rows, 1), len(ent)))
+    final = np.empty((chains, D + len(derived))) if final_state else None
     args = (len(cp), C.cast(prm, C.c_void_p), init.ctypes.data, C.cast(opts, C.c_void_p), len(derived),
             C.cast(cfn, C.c_void_p), C.cast(C.pointer(st), C.c_void_p) if st is not None else None,
-            seed, first_chain, chains, burn, sample, thin, mon.ctypes.data, len(ent), out.ctypes.data)
+            seed, first_chain, chains, burn, sample, thin, mon.ctypes.data, len(ent), out.ctypes.data,
+            final.ctypes.data if final is not None else None)
     if threads > 1:
         L.orc_run_chains_mt(*args, int(threads))          # the C call releases the GIL; chains are dealt out to pthreads inside
     else:
@@ -349,7 +369,7 @@ def run_model(model: str, data, params: Dict[str, dict], chains: int = 1, seed: 
         a = np.moveaxis(out[:, :, s:s + ln], 0, 1)        # [rows, chains, entries]
         a = a.reshape(rows, chains) if list(dim) == [1] else a.reshape(rows, chains, *dim)
         res[nm] = a[:, 0] if chains == 1 else a
-    return res
+    return (res, final) if final_state else res
 
 
 def time_model(model: str, data, params, chains: int, burn: int, sample: int, seed: int = 0, threads: int = 1) -> float:

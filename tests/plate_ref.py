@@ -165,15 +165,50 @@ def pois_loglin(orc, y, X, beta, partials=2, chunk=64):
 
 
 # ---- PLATE_NORM_IID / PLATE_NORM_GROUPED ------------------------------------------------------------------------------------
-def norm_plate(x, mean, sd, n_groups=1, chunk=64):
+RING_TILE = 2048                # points per tile of the interpreter kernels' ring (csrc kRingStageBytes / 8)
+JRING_TILE = 1024               # points per tile of the specialised statistics sweep's ring (amwg_jit.cuh JRING_TILE)
+
+
+def ss_depth(n, tile, parts=1):
+    """How many fp64 roundings one d_i^2 of S = sum_i (x_i - mean_i)^2 can go through in csrc sum_sq_dev and its callers. A segment of
+    m points (a plate, a group, or the part of one inside a streamed tile) peels at most one point to align its 16-byte loads, sums
+    blocks of eight into four fma accumulators (two per block each) and the tail (<= 7 points) into the first, then adds
+    (s0 + s1) + (s2 + s3): at most (m - t) / 4 + t + 2 <= ceil(m / 4) + 8 roundings. The partial sums of the segments are then added
+    one by one: at most ceil(n / tile) tiles, plus one segment more per plate or group that starts inside a tile."""
+    return -(-n // 4) + -(-n // tile) + parts + 8
+
+
+def sum_sq(x, mean, tile=RING_TILE, chunk=64):
+    """S = sum_i (x_i - mean)^2 per chain -> Value (value, bound, median (x_i - mean)^2), for the statistic slots of the term cache.
+    x: [n]; mean: [C] (the value the kernel used, already rounded to fp64). Its error is at most
+      d   x_i - mean in fp64: relative u on d_i, so 2u + u^2 on d_i^2;
+      S   gamma_(ss_depth(n, tile)) sum_i d_i^2 (all summands are >= 0).
+    Value.check's sensitivity test (bound < 1e-3 x the median d_i^2) makes a dropped, duplicated or stale point, or S at another
+    mean, fail."""
+    x = np.asarray(x, dtype=np.float64)
+    mean = np.asarray(mean, dtype=np.float64).reshape(-1)
+    n, C = x.size, mean.size
+    xL = x.astype(LD)
+    value = np.empty(C, dtype=LD)
+    med = np.empty(C)
+    for a0 in range(0, C, chunk):
+        d = xL[:, None] - mean[None, a0:a0 + chunk].astype(LD)
+        d2 = d * d
+        value[a0:a0 + chunk] = d2.sum(axis=0)
+        med[a0:a0 + chunk] = np.median(d2.astype(np.float64), axis=0)
+    bound = (2 * U + U * U + gamma(ss_depth(n, tile))) * value.astype(np.float64)
+    return Value(value, bound, med)
+
+
+def norm_plate(x, mean, sd, n_groups=1, chunk=64, tile=RING_TILE):
     """sum_i ld.norm(x_i, mean_i, sd) per chain -> (value, bound, median (x_i - mean_i)^2 / (2 sd sd)). x: [n]; mean: [C] (NORM_IID) or [C, n] (the group
-    mean of each point, NORM_GROUPED); sd: [C].
+    mean of each point, NORM_GROUPED); sd: [C]; tile: the points per streamed tile of the kernel that formed S.
 
     The plate computes n (c0 - log sd) - S / (2 sd sd), S = sum_i (x_i - mean_i)^2 (csrc sum_sq_dev, norm_factorised). Its error is
     at most:
       d   x_i - mean_i in fp64: relative u on d_i, so 2u + u^2 on d_i^2;
       S   fma accumulation into four accumulators after a one-point alignment peel, blocks and tail, one partial sum per ring tile or
-          per group added in order: gamma_(n/4 + n/2048 + groups + 4) sum_i d_i^2;
+          per group added in order: gamma_(ss_depth(n, tile, groups)) sum_i d_i^2;
       q   S / (2 sd sd): two roundings, and S's error carried through;
       c   n (c0 - log sd): c0 and log sd within 1 ulp each and three roundings: 4 u n (|c0| + |log sd|);
       out the final difference: u |value|."""
@@ -185,7 +220,7 @@ def norm_plate(x, mean, sd, n_groups=1, chunk=64):
     per_point = mean.ndim == 2
     xL = x.astype(LD)
     c0 = LD(-0.5) * np.log(LD(2) * LD(JS_PI))
-    depth = -(-n // 4) + -(-n // 2048) + n_groups + 4
+    depth = ss_depth(n, tile, n_groups)
     value = np.empty(C, dtype=LD)
     bound = np.empty(C)
     med = np.empty(C)
@@ -207,6 +242,18 @@ def norm_plate(x, mean, sd, n_groups=1, chunk=64):
         bound[a0:a0 + chunk] = q_err + c_err + U * (np.abs(A.astype(np.float64)) + Sf / kf) + U * np.abs(v.astype(np.float64))
         med[a0:a0 + chunk] = np.median((d2 / k[None, :]).astype(np.float64), axis=0)    # a row changes S / (2 sd sd) by this
     return value, bound, med
+
+
+def oracle_norm_error(x, mean, sd, priors):
+    """The worst-case error of the oracle's own fp64 log_post for a Normal likelihood (orc_model_norm_readme / hier_norm, term by
+    term): per point -0.5 log(2 pi) - log(sd) - (x - mean)^2 / (2 sd sd): two logs within 1 ulp and six roundings; the priors' own
+    error (this module's bound for the same operations); the running sum over every term. mean: scalar or per point."""
+    c = abs(-0.5 * np.log(2 * np.pi))
+    q = (x - mean) ** 2 / (2 * sd * sd)
+    row = 6 * U * (c + abs(np.log(sd)) + q)
+    prior_mag = sum(float(np.sum(np.abs(v.astype(float)) + b)) for v, b in priors)
+    return float(np.sum(row) + sum(float(np.sum(b)) for _, b in priors) +
+                 gamma(x.size + len(priors)) * (np.sum(c + abs(np.log(sd)) + q) + prior_mag))
 
 
 def group_means(mu, g):

@@ -476,7 +476,11 @@ def _stat_kernel_text(generated):
 
 
 class HostStatKernel:
-    def __init__(self, pkg, orc, tmp_path, params, log_post, data, chains_hint=4096):
+    """`edit`: applied to the kernel's text before it is compiled (the self-checks of tests/stat_check.py plant a defect with it).
+    After run(), `work` holds the working set ([tval | tcand | bprop | bcoin][chain]; work[:NT] is the term cache) and `state` the
+    chains' components."""
+
+    def __init__(self, pkg, orc, tmp_path, params, log_post, data, chains_hint=4096, edit=None):
         self.s = s = pkg.mcmc.AmwgSampler(params, log_post, data, {"chains": chains_hint, "_model_only": True})
         self.prog, self.O = s._program, orc.lib()
         assert self.prog.stat_prog >= 0
@@ -489,7 +493,12 @@ class HostStatKernel:
         self.src = src
         cut = src.index("namespace amwg {")
         cpp = tmp_path / "stat_kernel.cpp"
-        cpp.write_text(src[:cut] + HOST_PRELUDE + STAT_SHIM + _tma_structs() + _sum_sq_text() + _stat_kernel_text(src[cut:]) + STAT_EXPORTS)
+        kernel = _stat_kernel_text(src[cut:])
+        if edit is not None:
+            edited = edit(kernel)
+            assert edited != kernel, "the edit did not change the kernel"
+            kernel = edited
+        cpp.write_text(src[:cut] + HOST_PRELUDE + STAT_SHIM + _tma_structs() + _sum_sq_text() + kernel + STAT_EXPORTS)
         so = tmp_path / "stat_kernel.so"
         r = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-I" + os.path.join(ROOT, "tests", "host_shim"),
                             "-I" + CSRC, str(cpp), "-o", str(so)], capture_output=True, text=True)
@@ -519,7 +528,7 @@ class HostStatKernel:
         cols = [np.ascontiguousarray(np.asarray(c, dtype=np.float64)) for c in self.prog.columns]
         colp = (C.POINTER(C.c_double) * max(len(cols), 1))(*[c.ctypes.data_as(C.POINTER(C.c_double)) for c in cols])
         adapting = np.ones(D, dtype=np.uint8) if adapting is None else np.asarray(adapting, dtype=np.uint8)
-        self.acc = acc
+        self.acc, self.work, self.state = acc, work, state
         p = lambda a, t: a.ctypes.data_as(C.POINTER(t))
         self.K.hs_sweep(p(state, C.c_double), p(psd, C.c_double), p(acc, C.c_int), p(work, C.c_double), p(vseq, C.c_ushort), p(perm, C.c_uint64),
                         p(rng_n, C.c_uint64), C.c_uint64(Cn), C.c_uint64(first_chain), C.c_uint64(seed), C.c_longlong(sweeps), int(mon.size), p(mon, C.c_int),

@@ -22,15 +22,7 @@ def _oracle_pois_error(orc, y, X, beta):
     return float(np.sum(row) + np.sum(prior[1]) + gamma(n_terms := K + y.size) * mag * (1 + gamma(n_terms)))
 
 
-def _oracle_norm_error(x, mean, sd, priors):
-    """per point -0.5 log(2 pi) - log(sd) - (x - mean)^2 / (2 sd sd): two logs within 1 ulp and six roundings; the priors' own
-    error (plate_ref's bound for the same operations); the running sum over every term"""
-    c = abs(-0.5 * np.log(2 * np.pi))
-    q = (x - mean) ** 2 / (2 * sd * sd)
-    row = 6 * U * (c + abs(np.log(sd)) + q)
-    prior_mag = sum(float(np.sum(np.abs(v.astype(float)) + b)) for v, b in priors)
-    return float(np.sum(row) + sum(float(np.sum(b)) for _, b in priors) +
-                 gamma(x.size + len(priors)) * (np.sum(c + abs(np.log(sd)) + q) + prior_mag))
+_oracle_norm_error = pr.oracle_norm_error
 
 
 def test_reference_has_an_extended_significand():
