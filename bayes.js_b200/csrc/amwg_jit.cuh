@@ -671,8 +671,15 @@ static std::string build_source(const amwg_model* md, const std::vector<double>&
   std::ostringstream step;
   step << "__device__ __forceinline__ bool jit_step(const int c, const double prop, const double coin, double* __restrict__ wk, const unsigned long long ws,\n"
           "                                         double* __restrict__ sp, const unsigned long long ss) {\n";
-  if (sig_order.size() > 1) step << "  switch (JCLS[c]) {\n";
   bool need_mem = false;
+  // Lanes of a warp step components of different classes at the same time (each chain visits its components in its own order), so a
+  // warp runs every class's case one after the other. With one Metropolis test per case it would also evaluate js_exp once per class.
+  // When every commit is a named value or a candidate slot, the cases only form dl and the values to commit (cv[]), and one js_exp
+  // after the switch serves all classes: the same operations on the same values, so the same bits and the same decisions.
+  struct ClassCode { std::string mem, body, stage, commit, hcommit; };
+  std::vector<ClassCode> cls_code;
+  bool hoist = sig_order.size() > 1;
+  int n_cv = 0;
   for (size_t k = 0; k < sig_order.size(); ++k) {
     const std::vector<int>& members = classes_by_sig[sig_order[k]];
     std::vector<Inst> inst;
@@ -681,20 +688,53 @@ static std::string build_source(const amwg_model* md, const std::vector<double>&
       inst.push_back(it);
       cls_of[members[m]] = (int)k; mem_of[members[m]] = (int)m;
     }
-    std::string body, commit, why;
-    if (!emit_step_class(gc, inst, body, commit, &total_insns, why)) return "component program: " + why;
+    ClassCode cc;
+    std::string why;
+    if (!emit_step_class(gc, inst, cc.body, cc.commit, &total_insns, why)) return "component program: " + why;
     if (total_insns > kMaxGeneratedInsns) return "the component programs are too long to specialise";
-    if (commit.empty()) return "a component touches no term";
+    if (cc.commit.empty()) return "a component touches no term";
+    if (inst.size() > 1) { cc.mem = "    const int m = JMEM[c];\n"; need_mem = true; }
+    std::istringstream lines(cc.commit);
+    std::ostringstream stage, commit;
+    int i = 0;
+    for (std::string ln; std::getline(lines, ln);) {
+      const size_t eq = ln.find(") = ");
+      const std::string rhs = eq == std::string::npos ? "" : ln.substr(eq + 4);
+      const bool named = rhs.size() > 2 && rhs[0] == 'v' && rhs.back() == ';' && rhs.find_first_not_of("0123456789", 1) == rhs.size() - 1;
+      if (ln.compare(0, 7, "    TV(") != 0 || eq == std::string::npos) { hoist = false; break; }
+      if (rhs.compare(0, 3, "TC(") == 0) { commit << ln << "\n"; continue; }
+      if (!named) { hoist = false; break; }
+      stage << "    cv[" << i << "] = " << rhs << "\n";
+      commit << ln.substr(0, eq + 4) << "cv[" << i << "];\n";
+      ++i;
+    }
+    n_cv = std::max(n_cv, i);
+    cc.stage = stage.str();
+    cc.hcommit = commit.str();
+    cls_code.push_back(cc);
+  }
+  if (hoist) {
+    step << "  double dl = 0.0;\n";
+    if (n_cv > 0) step << "  double cv[" << n_cv << "];\n";
+    step << "  switch (JCLS[c]) {\n";
+    for (size_t k = 0; k < cls_code.size(); ++k) step << "  case " << k << ": {\n" << cls_code[k].mem << cls_code[k].body << cls_code[k].stage << "    break;\n  }\n";
+    step << "  default: return false;\n  }\n";
+    step << "  if (!(js_exp(dl) > coin)) return false;              // Metropolis accept (mcmc.js:527-534): strict >, NaN rejects\n";
+    step << "  ST(c) = prop;\n  switch (JCLS[c]) {\n";
+    for (size_t k = 0; k < cls_code.size(); ++k) step << "  case " << k << ": {\n" << cls_code[k].mem << cls_code[k].hcommit << "    break;\n  }\n";
+    step << "  }\n  return true;\n}\n";
+  }
+  if (!hoist && sig_order.size() > 1) step << "  switch (JCLS[c]) {\n";
+  for (size_t k = 0; !hoist && k < cls_code.size(); ++k) {
     if (sig_order.size() > 1) step << "  case " << k << ": {\n";
     else step << "  {\n";
-    if (inst.size() > 1) { step << "    const int m = JMEM[c];\n"; need_mem = true; }
-    step << "    double dl = 0.0;\n" << body;
+    step << cls_code[k].mem << "    double dl = 0.0;\n" << cls_code[k].body;
     step << "    if (!(js_exp(dl) > coin)) return false;            // Metropolis accept (mcmc.js:527-534): strict >, NaN rejects\n";
-    step << "    ST(c) = prop;\n" << commit;
+    step << "    ST(c) = prop;\n" << cls_code[k].commit;
     step << "    return true;\n  }\n";
   }
-  if (sig_order.size() > 1) step << "  }\n  return false;\n";
-  step << "}\n";
+  if (!hoist && sig_order.size() > 1) step << "  }\n  return false;\n";
+  if (!hoist) step << "}\n";
 
   // ---- statistics whose mean is an expression
   std::ostringstream extra;
