@@ -17,8 +17,15 @@
 //                                     digits, stable; digit positions equal in all keys skipped) for the rank-normalised diagnostics
 //   K_r4  amwg_rank_count_kernel    : merge-path rank counts of a sorted key array against another (integer, exact)
 //   K_r5  amwg_rank_z_kernel        : normal scores of the average ranks, scattered into a [2h][1][chains] z-block
+//   K_h0  amwg_finite_range_kernel  : smallest / largest finite draw (as order-preserving keys: u64 atomicMin / Max, exact and
+//                                     order independent) and the counts of -inf, +inf and NaN, per entry
+//   K_h1  amwg_hist_kernel          : equal-width 1-D histogram per entry (numpy.histogram's bin rule, amwg_hist.cuh) plus the
+//                                     counts below / above the range and of NaN; 32-bit shared bins per CTA, 64-bit global flush
+//   K_h2  amwg_hist2d_kernel        : 2-D histogram of a pair of entries (numpy.histogramdd's rule), up to 128 x 128 shared bins
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
+
+#include "amwg_hist.cuh"
 
 namespace summary {
 
@@ -154,6 +161,186 @@ __global__ void __launch_bounds__(256) amwg_digit_hist_kernel(const double* __re
   __syncthreads();
   for (int i = threadIdx.x; i < n_prefix * 256; i += blockDim.x)
     if (hist[i]) atomicAdd(&counts[(size_t)e * n_prefix * 256 + i], (unsigned long long)hist[i]);
+}
+
+// CTAs per entry of the counting kernels (digit_hist, the histograms): at most kChainCtas, doubled while one CTA would see 2^32
+// values or more, because its shared bins are 32-bit (rows < 2^32 is checked by the callers).
+inline int64_t count_ctas(int64_t chains, int64_t rows) {
+  int64_t bx = std::min<int64_t>((chains + 255) / 256, kChainCtas);
+  while (bx < (chains + 255) / 256 && ((chains + bx - 1) / bx) * rows >= ((int64_t)1 << 32)) bx *= 2;
+  return bx;
+}
+
+// ---- posterior histograms (sample_summary(..., histogram=...)) -------------------------------------------------------------
+constexpr int kMaxHistBins = 4096;     // 1-D bins per entry: (4097 edges x 8 B) + (4099 bins x 4 B) = 48 KB of shared memory
+constexpr int kMaxPairBins = 128;      // bins per axis of a 2-D histogram: 128 x 128 x 4 B = 64 KB of shared memory
+constexpr int kMaxPairs = 64;
+constexpr unsigned long long kNoKey = ~0ull;     // above every finite value's key: "no finite draw" for the minimum
+
+__device__ __forceinline__ double key_to_double(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// K_h0: one thread per chain walking its rows. Keys, not doubles, so that -0 < +0 and the extremes do not depend on the order in
+// which the threads meet them. keys[entry][2] = {min, max} key of the finite draws; nonfinite[entry][3] = #-inf, #+inf, #NaN.
+__global__ void __launch_bounds__(256) amwg_finite_range_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                                unsigned long long* __restrict__ keys, unsigned long long* __restrict__ nonfinite) {
+  __shared__ unsigned long long sh[5][8];
+  const int e = blockIdx.y;
+  const size_t stride = (size_t)entries * C;
+  unsigned long long kmin = kNoKey, kmax = 0ull, n_lo = 0, n_hi = 0, n_nan = 0;
+  auto see = [&](double v) {
+    if (isfinite(v)) {
+      const unsigned long long k = ordered_key(v);
+      kmin = k < kmin ? k : kmin;
+      kmax = k > kmax ? k : kmax;
+    } else if (v != v) {
+      ++n_nan;
+    } else if (v < 0.0) {
+      ++n_lo;
+    } else {
+      ++n_hi;
+    }
+  };
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const double* p = x + (size_t)e * C + c;
+    long long r = 0;
+    for (; r + 8 <= rows; r += 8) {                          // eight loads in flight per thread
+      double v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) see(v[u]);
+    }
+    for (; r < rows; ++r) see(p[r * stride]);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long a = __shfl_xor_sync(0xffffffffu, kmin, o), b = __shfl_xor_sync(0xffffffffu, kmax, o);
+    kmin = a < kmin ? a : kmin;
+    kmax = b > kmax ? b : kmax;
+    n_lo += __shfl_xor_sync(0xffffffffu, n_lo, o);
+    n_hi += __shfl_xor_sync(0xffffffffu, n_hi, o);
+    n_nan += __shfl_xor_sync(0xffffffffu, n_nan, o);
+  }
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) { sh[0][w] = kmin; sh[1][w] = kmax; sh[2][w] = n_lo; sh[3][w] = n_hi; sh[4][w] = n_nan; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int v = 1; v < (int)(blockDim.x >> 5); ++v) {
+      kmin = sh[0][v] < kmin ? sh[0][v] : kmin;
+      kmax = sh[1][v] > kmax ? sh[1][v] : kmax;
+      n_lo += sh[2][v]; n_hi += sh[3][v]; n_nan += sh[4][v];
+    }
+    if (kmin != kNoKey) atomicMin(&keys[2 * e], kmin);
+    if (kmax != 0ull) atomicMax(&keys[2 * e + 1], kmax);
+    if (n_lo) atomicAdd(&nonfinite[3 * e], n_lo);
+    if (n_hi) atomicAdd(&nonfinite[3 * e + 1], n_hi);
+    if (n_nan) atomicAdd(&nonfinite[3 * e + 2], n_nan);
+  }
+}
+
+__global__ void amwg_range_init_kernel(unsigned long long* __restrict__ keys, unsigned long long* __restrict__ nonfinite, int entries) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < entries; i += gridDim.x * blockDim.x) {
+    keys[2 * i] = kNoKey; keys[2 * i + 1] = 0ull;
+    nonfinite[3 * i] = nonfinite[3 * i + 1] = nonfinite[3 * i + 2] = 0ull;
+  }
+}
+
+// in place: the keys become the doubles they stand for, +inf / -inf when the entry has no finite draw
+__global__ void amwg_range_final_kernel(unsigned long long* __restrict__ keys, int entries) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < entries; i += gridDim.x * blockDim.x) {
+    const unsigned long long lo = keys[2 * i], hi = keys[2 * i + 1];
+    reinterpret_cast<double*>(keys)[2 * i] = lo == kNoKey ? CUDART_INF : key_to_double(lo);
+    reinterpret_cast<double*>(keys)[2 * i + 1] = hi == 0ull ? -CUDART_INF : key_to_double(hi);
+  }
+}
+
+// K_h1: counts[entry][bins + 3] += the entry's 1-D histogram over edges[entry][bins + 1], then the draws below edges[0] (-inf
+// included), above edges[bins] (+inf included) and NaN. Grid and run counting as in amwg_digit_hist_kernel: a rejected step repeats
+// its value, so a chain's consecutive rows mostly share a bin and the shared bins are touched once per run. Dynamic shared memory:
+// edges (doubles), then the bins (u32). Bounded to 64 registers (four CTAs per SM, which 4096 bins' 48 KB also allow): without
+// the bound ptxas picks 64 registers anyway and spills.
+__global__ void __launch_bounds__(256, 4) amwg_hist_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                        const double* __restrict__ edges, int bins, unsigned long long* __restrict__ counts) {
+  extern __shared__ double hist_smem[];
+  double* ed = hist_smem;
+  unsigned* hist = reinterpret_cast<unsigned*>(ed + bins + 1);
+  const int e = blockIdx.y;
+  for (int i = threadIdx.x; i <= bins; i += blockDim.x) ed[i] = edges[(size_t)e * (bins + 1) + i];
+  for (int i = threadIdx.x; i < bins + 3; i += blockDim.x) hist[i] = 0u;
+  __syncthreads();
+  const double lo = ed[0], hi = ed[bins];
+  const size_t stride = (size_t)entries * C;
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const double* p = x + (size_t)e * C + c;
+    int last = -1;
+    unsigned int run = 0;
+    auto count = [&](double v) {
+      const int idx = v < lo ? bins : v > hi ? bins + 1 : v != v ? bins + 2 : hist_bin(v, ed, bins);
+      if (idx == last) { ++run; return; }
+      if (last >= 0) atomicAdd(&hist[last], run);
+      last = idx; run = 1;
+    };
+    long long r = 0;
+    for (; r + 8 <= rows; r += 8) {                          // eight loads in flight per thread
+      double v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) count(v[u]);
+    }
+    for (; r < rows; ++r) count(p[r * stride]);
+    if (last >= 0) atomicAdd(&hist[last], run);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < bins + 3; i += blockDim.x)
+    if (hist[i]) atomicAdd(&counts[(size_t)e * (bins + 3) + i], (unsigned long long)hist[i]);
+}
+
+struct PairList { int a[kMaxPairs], b[kMaxPairs]; };   // entry indices, passed by value (512 B of kernel parameters)
+
+// K_h2: counts[pair][bins][bins] += the 2-D histogram of entries (a, b) of the pair, a on axis 0; a draw counts only when both of
+// its values fall inside their axis's edges. Grid (chain blocks, pairs); runs as in K_h1. Dynamic shared memory: both axes'
+// edges (doubles), then bins * bins u32 cells (64 KB at 128 bins).
+__global__ void __launch_bounds__(256) amwg_hist2d_kernel(const double* __restrict__ x, long long rows, int entries, long long C, PairList pl,
+                                                          const double* __restrict__ edges, int bins, unsigned long long* __restrict__ counts) {
+  extern __shared__ double hist_smem[];
+  double* ea = hist_smem;
+  double* eb = ea + bins + 1;
+  unsigned* cell = reinterpret_cast<unsigned*>(eb + bins + 1);
+  const int pr = blockIdx.y, a = pl.a[pr], b = pl.b[pr];
+  const int cells = bins * bins;
+  for (int i = threadIdx.x; i <= bins; i += blockDim.x) { ea[i] = edges[(size_t)a * (bins + 1) + i]; eb[i] = edges[(size_t)b * (bins + 1) + i]; }
+  for (int i = threadIdx.x; i < cells; i += blockDim.x) cell[i] = 0u;
+  __syncthreads();
+  const size_t stride = (size_t)entries * C;
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const double* pa = x + (size_t)a * C + c;
+    const double* pb = x + (size_t)b * C + c;
+    int last = -1;
+    unsigned int run = 0;
+    auto count = [&](double va, double vb) {
+      const int ia = hist2d_axis(va, ea, bins), ib = hist2d_axis(vb, eb, bins);
+      const int idx = (ia < 0 || ib < 0) ? -1 : ia * bins + ib;
+      if (idx == last) { ++run; return; }
+      if (last >= 0) atomicAdd(&cell[last], run);
+      last = idx; run = 1;
+    };
+    long long r = 0;
+    for (; r + 8 <= rows; r += 8) {                          // eight rows (sixteen loads) in flight per thread
+      double va[8], vb[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) { va[u] = pa[(r + u) * stride]; vb[u] = pb[(r + u) * stride]; }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) count(va[u], vb[u]);
+    }
+    for (; r < rows; ++r) count(pa[r * stride], pb[r * stride]);
+    if (last >= 0) atomicAdd(&cell[last], run);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < cells; i += blockDim.x)
+    if (cell[i]) atomicAdd(&counts[(size_t)pr * cells + i], (unsigned long long)cell[i]);
 }
 
 // ---- split-chain autocovariances (effective sample size, split R-hat) ------------------------------------------------------
@@ -759,6 +946,68 @@ extern "C" int amwg_summary_rank_z(int device, const int64_t* dev_acc, const uin
   CUDA_TRY(cudaSetDevice(device));
   const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, summary::kChainCtas);
   summary::amwg_rank_z_kernel<<<grid, 256>>>(reinterpret_cast<const long long*>(dev_acc), dev_index, n, (double)total, dev_z);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+extern "C" int amwg_summary_finite_range(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                         double* dev_range, int64_t* dev_nonfinite) {
+  if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_finite_range: empty sample block");
+  if (!dev_samples || !dev_range || !dev_nonfinite) return fail("amwg_summary_finite_range: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_finite_range: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  auto* keys = reinterpret_cast<unsigned long long*>(dev_range);
+  auto* nonfinite = reinterpret_cast<unsigned long long*>(dev_nonfinite);
+  const unsigned small = (unsigned)std::min<int64_t>((entries + 255) / 256, 1024);
+  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  summary::amwg_range_init_kernel<<<small, 256>>>(keys, nonfinite, entries);
+  summary::amwg_finite_range_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, keys, nonfinite);
+  summary::amwg_range_final_kernel<<<small, 256>>>(keys, entries);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+extern "C" int amwg_summary_histogram(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                      const double* dev_edges, int32_t bins, int64_t* dev_counts) {
+  if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_histogram: empty sample block");
+  if (bins < 1 || bins > summary::kMaxHistBins) return fail("amwg_summary_histogram: bins must be 1.." + std::to_string(summary::kMaxHistBins));
+  if (rows >= (int64_t)1 << 32) return fail("amwg_summary_histogram: more than 2^32 rows");
+  if (!dev_samples || !dev_edges || !dev_counts) return fail("amwg_summary_histogram: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_histogram: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const size_t smem = (size_t)(bins + 1) * sizeof(double) + (size_t)(bins + 3) * sizeof(unsigned);
+  CUDA_TRY(cudaFuncSetAttribute(summary::amwg_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t bx = summary::count_ctas(chains, rows);
+  summary::amwg_hist_kernel<<<dim3((unsigned)bx, (unsigned)entries), 256, smem>>>(dev_samples, rows, entries, chains, dev_edges, bins,
+                                                                                  reinterpret_cast<unsigned long long*>(dev_counts));
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+extern "C" int amwg_summary_histogram2d(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                        const int32_t* host_pairs, int32_t n_pairs, const double* dev_edges, int32_t bins, int64_t* dev_counts) {
+  if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_histogram2d: empty sample block");
+  if (bins < 1 || bins > summary::kMaxPairBins) return fail("amwg_summary_histogram2d: bins must be 1.." + std::to_string(summary::kMaxPairBins));
+  if (n_pairs < 1 || n_pairs > summary::kMaxPairs) return fail("amwg_summary_histogram2d: n_pairs must be 1.." + std::to_string(summary::kMaxPairs));
+  if (rows >= (int64_t)1 << 32) return fail("amwg_summary_histogram2d: more than 2^32 rows");
+  if (!dev_samples || !host_pairs || !dev_edges || !dev_counts) return fail("amwg_summary_histogram2d: null pointer");
+  if (device < 0 || device >= 64) return fail("amwg_summary_histogram2d: device index out of range");
+  summary::PairList pl;
+  for (int i = 0; i < n_pairs; ++i) {
+    pl.a[i] = host_pairs[2 * i];
+    pl.b[i] = host_pairs[2 * i + 1];
+    if (pl.a[i] < 0 || pl.a[i] >= entries || pl.b[i] < 0 || pl.b[i] >= entries)
+      return fail("amwg_summary_histogram2d: pair " + std::to_string(i) + " names an entry outside [0, entries)");
+  }
+  CUDA_TRY(cudaSetDevice(device));
+  const size_t smem = (size_t)2 * (bins + 1) * sizeof(double) + (size_t)bins * bins * sizeof(unsigned);
+  CUDA_TRY(cudaFuncSetAttribute(summary::amwg_hist2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t bx = summary::count_ctas(chains, rows);
+  summary::amwg_hist2d_kernel<<<dim3((unsigned)bx, (unsigned)n_pairs), 256, smem>>>(dev_samples, rows, entries, chains, pl, dev_edges, bins,
+                                                                                    reinterpret_cast<unsigned long long*>(dev_counts));
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
   return 0;

@@ -690,7 +690,7 @@ class AmwgSampler(Sampler):
             raise JsThrow(L.amwg_last_error().decode())
         return buf
 
-    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False):
+    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -708,9 +708,22 @@ class AmwgSampler(Sampler):
         split chains) and "rhat_rank" (the larger split R-hat of the rank-normalised draws and of the rank-normalised folded draws
         |x - median|), ranked over the pooled draws of all chains on all GPUs (Vehtari et al. 2021, §4; the numbers Stan and
         ArviZ print). They stay finite with +-inf draws and catch chains that differ in scale only; see summary.rank_diagnostics.
-        Ranking needs 56 bytes of device scratch per ranked draw for one parameter entry at a time. Any other value raises."""
+        Ranking needs 56 bytes of device scratch per ranked draw for one parameter entry at a time. Any other value raises.
+        histogram=k (or {"bins": k}) adds equal-width posterior histograms, counted on the device and equal to numpy's on the raw
+        draws count for count. A dict may hold "bins" (1..4096 per entry; may be left out when only pairs are wanted), "range"
+        ({name: (lo, hi)}, finite lo < hi, for every component of that name), "pairs" (at most 64 (a, b), each selector a scalar's
+        name or (name, flat_index) for one component, row-major) and "pair_bins" (1..128 per axis, default 50). Each monitored
+        name gains, shaped like "quantiles" with the bins last ([k] or [*dim, k]): "hist" (int64 counts), "hist_edges" (k + 1
+        edges) and "hist_outside" (int64 [3]: draws < lo, > hi and NaN; infinities count as below or above), so hist.sum() +
+        hist_outside.sum() == n_draws. The range is range[name] when given, else the smallest and largest finite draw over all
+        chains, rows and GPUs (numpy.histogram's default on the finite draws), widened to (lo - 0.5, hi + 0.5) when lo == hi, and
+        (0, 1) when there is no finite draw. The edges are numpy.linspace(lo, hi, k + 1), and a draw lo <= x <= hi goes to the bin
+        numpy.histogram gives it (its equal-width arithmetic, in the same fp64 operations). Each pair adds a top-level entry keyed by
+        the pair as given: {"hist": int64 [pair_bins, pair_bins] (a on axis 0), "xedges", "yedges"}, the edges being linspace(lo,
+        hi, pair_bins + 1) of each selector's range; a draw counts when both values lie inside, binned as numpy.histogram2d bins
+        it. Every other key keeps its bits. A refused histogram raises ValueError before the chains move (summary.resolve_histogram)."""
         import torch
-        from .summary import CudaBlockReducer, check_diagnostics, summarise_block
+        from .summary import CudaBlockReducer, check_diagnostics, histogram_block, resolve_histogram, summarise_block
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
@@ -719,6 +732,8 @@ class AmwgSampler(Sampler):
             e = self._entries(name)
             spans[name] = (len(entries), len(e))
             entries.extend(e)
+        named = [name for name in monitored if spans[name][1] > 0]
+        plan = resolve_histogram(histogram, named, {name: list(self.params[name]["dim"]) if name in self.params else [1] for name in named})
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
@@ -727,6 +742,10 @@ class AmwgSampler(Sampler):
         L = _ffi.lib()
         dev = torch.device("cuda", self.device)
         need = rows * len(entries) * self.local_chains * 8
+        if plan is not None:
+            # edges and counts of the histograms, and the extremes (8 B each)
+            nb, pb = plan.bins or 0, plan.pair_bins
+            need += 8 * (len(entries) * (2 * nb + 4 + pb + 1 + 5) + len(plan.pairs) * pb * pb)
         free, _total = torch.cuda.mem_get_info(dev)
         if need + 2 * len(entries) * self.local_chains * 8 > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
@@ -747,6 +766,7 @@ class AmwgSampler(Sampler):
             raise JsThrow(L.amwg_last_error().decode())
         res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
+        hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
         del block
         out = {}
         for name in monitored:
@@ -761,6 +781,12 @@ class AmwgSampler(Sampler):
             if diagnostics:
                 for key, val in res[4][0].items():
                     out[name][key] = shape(val[s0:s0 + ln])
+            if hist is not None and plan.bins is not None:
+                for key in ("hist", "hist_edges", "hist_outside"):
+                    val = hist[key][s0:s0 + ln]
+                    out[name][key] = val[0] if dim == [1] else val.reshape(*dim, val.shape[-1])
+        if hist is not None:
+            out.update(hist["pairs"])
         return out
 
     def start_adaptation(self):

@@ -9,13 +9,15 @@ radix-select digit counts (integers) -- so every rank returns the same numbers a
 
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
 amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True, and
-amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank"). There is no
-CPU fallback: without the library or a GPU the reducer raises.
+amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank", and
+amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=...). There is no CPU fallback:
+without the library or a GPU the reducer raises.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Sequence, Tuple
+import numbers
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -198,6 +200,41 @@ class CudaBlockReducer:
         import torch
         torch.cuda.current_stream(acc.device).synchronize()
         self._ffi.check(self.L.amwg_summary_rank_z(self.device, acc.data_ptr(), index.data_ptr(), n, total, z.data_ptr()))
+
+    def finite_range(self, block):
+        """-> (float64 tensor [entries, 2]: smallest and largest finite draw, +inf / -inf when there is none; int64 tensor
+        [entries, 3]: the counts of -inf, +inf and NaN draws), this shard's, on the block's device."""
+        import torch
+        rows, entries, chains = block.shape
+        rng = torch.empty((entries, 2), dtype=torch.float64, device=block.device)
+        nonfinite = torch.empty((entries, 3), dtype=torch.int64, device=block.device)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_finite_range(self.device, block.data_ptr(), rows, entries, chains, rng.data_ptr(),
+                                                         nonfinite.data_ptr()))
+        return rng, nonfinite
+
+    def histogram(self, block, edges: np.ndarray, bins: int):
+        """-> int64 tensor [entries, bins + 3]: this shard's counts per bin over edges [entries, bins + 1], then below, above, NaN."""
+        import torch
+        rows, entries, chains = block.shape
+        ed = torch.from_numpy(np.ascontiguousarray(edges, dtype=np.float64)).to(block.device)
+        counts = torch.zeros((entries, bins + 3), dtype=torch.int64, device=block.device)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_histogram(self.device, block.data_ptr(), rows, entries, chains, ed.data_ptr(), bins,
+                                                      counts.data_ptr()))
+        return counts
+
+    def histogram2d(self, block, pairs: np.ndarray, edges: np.ndarray, bins: int):
+        """-> int64 tensor [n_pairs, bins, bins]: this shard's 2-D counts of the entry pairs [n_pairs, 2] over edges [entries, bins + 1]."""
+        import torch
+        rows, entries, chains = block.shape
+        pr = np.ascontiguousarray(pairs, dtype=np.int32)
+        ed = torch.from_numpy(np.ascontiguousarray(edges, dtype=np.float64)).to(block.device)
+        counts = torch.zeros((len(pr), bins, bins), dtype=torch.int64, device=block.device)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_histogram2d(self.device, block.data_ptr(), rows, entries, chains, pr.ctypes.data, len(pr),
+                                                        ed.data_ptr(), bins, counts.data_ptr()))
+        return counts
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -525,3 +562,174 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
         lo_min, lo_max = low[len(user_probs)], low[len(user_probs) + 3]
         diag[0].update(rank_diagnostics(reducer, block, rows, q[-1], lo_min, lo_max, distributed))
     return mean, sd, rhat, q[:len(user_probs)], diag
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# posterior histograms: equal-width 1-D bins per entry and 2-D counts of entry pairs, equal to numpy's on the raw draws
+MAX_HIST_BINS = 4096                   # include/amwg.h: amwg_summary_histogram, bins <= 4096
+MAX_PAIR_BINS = 128                    # amwg_summary_histogram2d: bins <= 128 per axis
+MAX_PAIRS = 64                         # amwg_summary_histogram2d: n_pairs <= 64
+PAIR_BINS = 50                         # default bins per axis of a 2-D histogram
+_HIST_KEYS = ("bins", "range", "pairs", "pair_bins")
+
+
+class HistogramPlan(NamedTuple):
+    """A checked `histogram=` argument. bins: 1-D bins per entry (None: pairs only); fixed: [entries, 2] user (lo, hi), NaN where
+    the range comes from the draws; pairs: (key as given, entry a, entry b); pair_bins: bins per axis of every pair."""
+    bins: Optional[int]
+    fixed: np.ndarray
+    pairs: List[Tuple[object, int, int]]
+    pair_bins: int
+
+
+def _is_int(v) -> bool:
+    return isinstance(v, numbers.Integral) and not isinstance(v, bool)
+
+
+def resolve_histogram(spec, names: Sequence[str], dims) -> Optional[HistogramPlan]:
+    """Checks the `histogram=` argument of sample_summary against the monitored names (in sample-block order, only those with
+    entries) and their dims ({name: dim list}; the entries of a name are prod(dim), row-major) and returns the plan, or None for
+    None. Pure: raises ValueError before any device work."""
+    if spec is None:
+        return None
+    if _is_int(spec):
+        spec = {"bins": spec}
+    elif not isinstance(spec, dict):
+        raise ValueError("histogram must be None, an int number of bins or a dict, not %r" % (spec,))
+    unknown = [k for k in spec if k not in _HIST_KEYS]
+    if unknown:
+        raise ValueError("histogram has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(_HIST_KEYS)))
+    span = {}
+    entries = 0
+    for name in names:                                        # a name listed twice in monitor: its last block, as sample_summary
+        n = int(np.prod(dims[name]))
+        span[name] = (entries, n)
+        entries += n
+
+    bins = spec.get("bins")
+    if "bins" in spec and not (_is_int(bins) and 1 <= bins <= MAX_HIST_BINS):
+        raise ValueError("histogram bins must be an int in 1..%d, not %r" % (MAX_HIST_BINS, bins))
+    pair_bins = spec.get("pair_bins", PAIR_BINS)
+    if not (_is_int(pair_bins) and 1 <= pair_bins <= MAX_PAIR_BINS):
+        raise ValueError("histogram pair_bins must be an int in 1..%d, not %r" % (MAX_PAIR_BINS, pair_bins))
+
+    fixed = np.full((entries, 2), np.nan)
+    ranges = spec.get("range", {})
+    if not isinstance(ranges, dict):
+        raise ValueError("histogram range must be a dict {name: (lo, hi)}, not %r" % (ranges,))
+    for name, r in ranges.items():
+        if name not in span:
+            raise ValueError("histogram range: %r is not a monitored parameter or derived quantity" % (name,))
+        ok = isinstance(r, (tuple, list)) and len(r) == 2 and all(isinstance(v, numbers.Real) and not isinstance(v, bool) for v in r)
+        if not ok or not (np.isfinite(r[0]) and np.isfinite(r[1])) or not r[0] < r[1]:
+            raise ValueError("histogram range of %r must be (lo, hi) with finite lo < hi, not %r" % (name, r))
+        s0, n = span[name]
+        fixed[s0:s0 + n] = (float(r[0]), float(r[1]))
+
+    def entry(sel) -> Tuple[object, int]:
+        if isinstance(sel, str):
+            if sel not in span:
+                raise ValueError("histogram pair: %r is not a monitored parameter or derived quantity" % (sel,))
+            if span[sel][1] != 1:
+                raise ValueError("histogram pair: %r has %d components; select one as (%r, flat_index)" % (sel, span[sel][1], sel))
+            return sel, span[sel][0]
+        if isinstance(sel, (tuple, list)) and len(sel) == 2 and isinstance(sel[0], str) and _is_int(sel[1]):
+            name, i = sel
+            if name not in span:
+                raise ValueError("histogram pair: %r is not a monitored parameter or derived quantity" % (name,))
+            if not 0 <= i < span[name][1]:
+                raise ValueError("histogram pair: component %d of %r is outside [0, %d)" % (i, name, span[name][1]))
+            return (name, int(i)) if isinstance(sel, list) else sel, span[name][0] + int(i)
+        raise ValueError("histogram pair selector must be a name or (name, flat_index), not %r" % (sel,))
+
+    given = spec.get("pairs", [])
+    if not isinstance(given, (tuple, list)):
+        raise ValueError("histogram pairs must be a list of (a, b) selectors, not %r" % (given,))
+    if len(given) > MAX_PAIRS:
+        raise ValueError("histogram pairs: %d pairs (max %d)" % (len(given), MAX_PAIRS))
+    pairs: List[Tuple[object, int, int]] = []
+    for p in given:
+        if not (isinstance(p, (tuple, list)) and len(p) == 2):
+            raise ValueError("histogram pair must be (a, b), not %r" % (p,))
+        (ka, ea), (kb, eb) = entry(p[0]), entry(p[1])
+        key = (ka, kb)                                       # the pair as given (a list selector becomes a tuple: keys must hash)
+        if all(key != q[0] for q in pairs):
+            pairs.append((key, ea, eb))
+    if bins is None and not pairs:
+        raise ValueError("histogram needs bins, pairs or both")
+    return HistogramPlan(bins, fixed, pairs, pair_bins)
+
+
+def _sortable(x: np.ndarray) -> np.ndarray:
+    """float64 -> int64 whose signed order is the order of the doubles (-0 below +0)."""
+    u = np.ascontiguousarray(x, dtype=np.float64).view(np.int64)
+    return np.where(u < 0, u ^ np.int64(0x7FFFFFFFFFFFFFFF), u)
+
+
+def _unsortable(k: np.ndarray) -> np.ndarray:
+    k = np.asarray(k, dtype=np.int64)
+    return np.where(k < 0, k ^ np.int64(0x7FFFFFFFFFFFFFFF), k).view(np.float64)
+
+
+def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed: bool) -> dict:
+    """-> {"hist" [entries, bins] int64, "hist_edges" [entries, bins + 1], "hist_outside" [entries, 3] int64 (when plan.bins),
+    "pairs": {key: {"hist" [pair_bins, pair_bins] int64, "xedges", "yedges"}}} over all shards; only reads the block.
+
+    Range of an entry: plan.fixed when given, else (lo, hi) = the smallest and largest finite draw over all rows, chains and
+    shards (numpy.histogram's default on the finite draws); lo == hi gives (lo - 0.5, hi + 0.5), no finite draw (0, 1). Edges:
+    numpy.linspace(lo, hi, bins + 1). A draw lo <= x <= hi goes to numpy.histogram's bin (csrc/amwg_hist.cuh); hist_outside counts
+    the draws < lo (-inf included), > hi (+inf included) and NaN, so hist.sum() + hist_outside.sum() is the number of draws.
+    A pair's axes are its two entries' ranges at plan.pair_bins; a draw counts when both values lie inside their axis's edges,
+    each binned as numpy.histogramdd bins it (searchsorted right, the last edge in the last bin).
+    Distributed: one MAX all-reduce of the extremes (as order-preserving integers, the minimum negated) and one SUM all-reduce of
+    all the counts, so every rank returns the same bits whatever the number of GPUs."""
+    import torch
+    entries = block.shape[1]
+    lo, hi = plan.fixed[:, 0].copy(), plan.fixed[:, 1].copy()
+    used = np.zeros(entries, dtype=bool)
+    used[:] = plan.bins is not None
+    for _key, a, b in plan.pairs:
+        used[a] = used[b] = True
+    auto = np.isnan(lo)
+    if np.any(auto & used):
+        rng = reducer.finite_range(block)[0].cpu().numpy()
+        if distributed:
+            import torch.distributed as dist
+            keys = np.concatenate([-_sortable(rng[:, 0]), _sortable(rng[:, 1])])
+            t = torch.from_numpy(keys)
+            if block.is_cuda:
+                t = t.to(block.device)
+            dist.all_reduce(t, op=dist.ReduceOp.MAX)
+            keys = t.cpu().numpy()
+            rng = np.stack([_unsortable(-keys[:entries]), _unsortable(keys[entries:])], axis=1)
+        for e in np.flatnonzero(auto):
+            a, b = rng[e]
+            lo[e], hi[e] = (0.0, 1.0) if not a <= b else (a - 0.5, b + 0.5) if a == b else (a, b)
+    lo[auto & ~used], hi[auto & ~used] = 0.0, 1.0
+
+    def edges(k: int) -> np.ndarray:
+        return np.stack([np.linspace(lo[e], hi[e], k + 1) for e in range(entries)])
+
+    parts = []
+    if plan.bins is not None:
+        e1 = edges(plan.bins)
+        parts.append(reducer.histogram(block, e1, plan.bins))
+    if plan.pairs:
+        e2 = edges(plan.pair_bins)
+        pair_idx = np.array([(a, b) for _k, a, b in plan.pairs], dtype=np.int32)
+        parts.append(reducer.histogram2d(block, pair_idx, e2, plan.pair_bins))
+    if distributed:
+        import torch.distributed as dist
+        flat = torch.cat([p.reshape(-1) for p in parts])
+        dist.all_reduce(flat)                                 # integer sums: exact, independent of the number of GPUs
+        parts = list(torch.split(flat, [p.numel() for p in parts]))
+    counts = [p.cpu().numpy().astype(np.int64, copy=False) for p in parts]
+    out = {"pairs": {}}
+    if plan.bins is not None:
+        c1 = counts.pop(0).reshape(entries, plan.bins + 3)
+        out.update(hist=c1[:, :plan.bins].copy(), hist_edges=e1, hist_outside=c1[:, plan.bins:].copy())
+    if plan.pairs:
+        c2 = counts.pop(0).reshape(len(plan.pairs), plan.pair_bins, plan.pair_bins)
+        for i, (key, a, b) in enumerate(plan.pairs):
+            out["pairs"][key] = {"hist": c2[i].copy(), "xedges": e2[a].copy(), "yedges": e2[b].copy()}
+    return out

@@ -331,7 +331,22 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   Errors: nq or nr < 1 or >= 2^32, null pointers.
  * amwg_summary_rank_z: dev_z[dev_index[i]] = Phi^-1((r - 3/8) / (total + 1/4)), r = (dev_acc[i] + 1) / 2, for i < n; total is the
  *   number of ranked draws over all shards. Sized [2h][chains], dev_z is a [2h][1][chains] block whose two halves
- *   amwg_summary_autocov splits exactly as they were ranked. Errors: n outside 1..2^32-1, total < n or >= 2^52, null pointers. */
+ *   amwg_summary_autocov splits exactly as they were ranked. Errors: n outside 1..2^32-1, total < n or >= 2^52, null pointers.
+ *
+ * Posterior histograms (sample_summary(..., histogram=...)): three reductions over the block, integers or exact extremes, so the
+ * results do not depend on the order of the atomics and sum (or min / max) across GPUs exactly.
+ * amwg_summary_finite_range: dev_range[entry][2] = { smallest, largest finite draw } (+inf / -inf when the entry has none; -0 counts
+ *   below +0) and dev_nonfinite[entry][3] = { #-inf, #+inf, #NaN }, both overwritten. Errors: an empty block, null pointers.
+ * amwg_summary_histogram: dev_counts[entry][bins + 3] += the counts of the bins over dev_edges[entry][bins + 1] (device memory),
+ *   then of the draws below edges[0] (-inf included), above edges[bins] (+inf included) and NaN; the caller zeroes the counts, as
+ *   for digit_hist. The edges are numpy.linspace(lo, hi, bins + 1) and a draw lo <= x <= hi gets numpy.histogram's bin (the
+ *   operations of its equal-width fast path: csrc/amwg_hist.cuh). Errors: bins outside 1..4096, rows >= 2^32, an empty block,
+ *   null pointers.
+ * amwg_summary_histogram2d: dev_counts[pair][bins][bins] += the 2-D histogram of entries host_pairs[pair][0] (axis 0) and
+ *   host_pairs[pair][1] (axis 1) over their rows of dev_edges[entry][bins + 1], by numpy.histogramdd's rule (per axis
+ *   searchsorted(edges, v, "right") - 1, the last edge in the last bin); a draw counts only when both values fall inside (NaN
+ *   never does). host_pairs is host memory. Errors: bins outside 1..128, n_pairs outside 1..64, a pair entry outside
+ *   [0, entries), rows >= 2^32, an empty block, null pointers. */
 AMWG_API int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats);
 AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t pass,
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
@@ -341,6 +356,12 @@ AMWG_API int amwg_summary_rank_sort(int device, const double* dev_samples, int64
                                     double centre, uint64_t* dev_keys, uint32_t* dev_index, int32_t* host_passes);
 AMWG_API int amwg_summary_rank_count(int device, const uint64_t* dev_q, int64_t nq, const uint64_t* dev_r, int64_t nr, int64_t* dev_acc);
 AMWG_API int amwg_summary_rank_z(int device, const int64_t* dev_acc, const uint32_t* dev_index, int64_t n, int64_t total, double* dev_z);
+AMWG_API int amwg_summary_finite_range(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                       double* dev_range, int64_t* dev_nonfinite);
+AMWG_API int amwg_summary_histogram(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                    const double* dev_edges, int32_t bins, int64_t* dev_counts);
+AMWG_API int amwg_summary_histogram2d(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                      const int32_t* host_pairs, int32_t n_pairs, const double* dev_edges, int32_t bins, int64_t* dev_counts);
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it

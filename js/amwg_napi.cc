@@ -478,6 +478,33 @@ BINDING(plate_sources)
   amwg_plate_sources(handle_of(env, a.at(0))->s, out, sizeof out);
   return js_string(env, out);
 END_BINDING
+// summary_finite_range(device, samples ptr, rows, entries, chains, range ptr, nonfinite ptr)          amwg_summary_finite_range
+BINDING(summary_finite_range)
+  if (amwg_summary_finite_range((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                                (int32_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), (double*)(uintptr_t)to_u64(env, a.at(5)),
+                                (int64_t*)(uintptr_t)to_u64(env, a.at(6))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// summary_histogram(device, samples ptr, rows, entries, chains, edges ptr, bins, counts ptr)             amwg_summary_histogram
+BINDING(summary_histogram)
+  if (amwg_summary_histogram((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                             (int32_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), (const double*)(uintptr_t)to_u64(env, a.at(5)),
+                             (int32_t)to_double(env, a.at(6)), (int64_t*)(uintptr_t)to_u64(env, a.at(7))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// summary_histogram2d(device, samples ptr, rows, entries, chains, pairs [n_pairs][2], edges ptr, bins, counts ptr)
+//                                                                                                         amwg_summary_histogram2d
+BINDING(summary_histogram2d)
+  const std::vector<int32_t> pairs = ints(env, a.at(5));
+  if (amwg_summary_histogram2d((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                               (int32_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), pairs.data(), (int32_t)(pairs.size() / 2),
+                               (const double*)(uintptr_t)to_u64(env, a.at(6)), (int32_t)to_double(env, a.at(7)),
+                               (int64_t*)(uintptr_t)to_u64(env, a.at(8))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
 // term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
 BINDING(term_cache)
   Handle* h = handle_of(env, a.at(0));
@@ -510,6 +537,7 @@ NAPI_MODULE_INIT() {
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
+      {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
