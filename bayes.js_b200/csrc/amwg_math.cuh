@@ -142,13 +142,29 @@ __device__ __forceinline__ Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint3
   return Philox4{c0, c1, c2, c3};
 }
 
-__device__ __forceinline__ double u53(uint32_t a, uint32_t b) {
-  return ((double)(a >> 5) * 67108864.0 + (double)(b >> 6)) * (1.0 / 9007199254740992.0);
+// (double)v for a 32-bit v without an integer-to-double conversion (a quarter-rate instruction on sm_90): the double whose high
+// word is 0x43300000 and whose low word is v is 2^52 + v, and subtracting 2^52 leaves v. Both steps are exact.
+__device__ __forceinline__ double u32_to_double(uint32_t v) {
+  return __hiloint2double(0x43300000, (int)v) - 4503599627370496.0;
 }
 
-// one Philox block = uniforms #2*blk and #2*blk+1 of chain (g0,g1). Kept out of line: it is ~80 instructions and
-// is needed at several points of a sweep; inlining it everywhere bloats the kernel past the instruction cache.
-__device__ __noinline__ double2 philox_uniform_pair(uint32_t blk_lo, uint32_t blk_hi, uint32_t g0, uint32_t g1, uint32_t k0, uint32_t k1) {
+__device__ __forceinline__ double u53(uint32_t a, uint32_t b) {
+  return (u32_to_double(a >> 5) * 67108864.0 + u32_to_double(b >> 6)) * (1.0 / 9007199254740992.0);
+}
+
+// one Philox block = uniforms #2*blk and #2*blk+1 of chain (g0,g1). Kept out of line by default: it is ~80 instructions and
+// is needed at several points of a sweep; inlining it everywhere bloats the kernel past the instruction cache. The specialised
+// statistics sweep defines AMWG_PHILOX_INLINE (amwg_jit.cuh): its step code is short, and there the call's overhead is the
+// larger cost (config 2: 6 % less per-sweep O(1) time on an H100, DESIGN.md section 4.1).
+#ifndef AMWG_PHILOX_INLINE
+#define AMWG_PHILOX_INLINE 0
+#endif
+#if AMWG_PHILOX_INLINE
+__device__ __forceinline__
+#else
+__device__ __noinline__
+#endif
+double2 philox_uniform_pair(uint32_t blk_lo, uint32_t blk_hi, uint32_t g0, uint32_t g1, uint32_t k0, uint32_t k1) {
   Philox4 p = philox4x32_10(blk_lo, blk_hi, g0, g1, k0, k1);
   return make_double2(u53(p.r0, p.r1), u53(p.r2, p.r3));
 }
