@@ -22,9 +22,15 @@
 //   K_h1  amwg_hist_kernel          : equal-width 1-D histogram per entry (numpy.histogram's bin rule, amwg_hist.cuh) plus the
 //                                     counts below / above the range and of NaN; 32-bit shared bins per CTA, 64-bit global flush
 //   K_h2  amwg_hist2d_kernel        : 2-D histogram of a pair of entries (numpy.histogramdd's rule), up to 128 x 128 shared bins
+//   K_c1  amwg_chain_means_kernel   : one thread per (chain, selected entry): the chain's mean over its rows (sequential sum)
+//   K_c2  amwg_shard_mean_kernel    : one CTA per selected entry: the mean of the chain means, summed in a fixed tree
+//   K_c3  amwg_gram_kernel          : upper-triangle 8 x 8 tiles of the Gram matrix of centred draws on the fp64 tensor core
+//                                     (mma.sync m8n8k4 f64), 32-chain stages in shared memory; addressing in amwg_comoments.cuh
+//   K_c4  amwg_sum_tiles_kernel     : sums the per-CTA partial tiles in CTA order
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
 
+#include "amwg_comoments.cuh"
 #include "amwg_hist.cuh"
 
 namespace summary {
@@ -737,6 +743,140 @@ __global__ void __launch_bounds__(256) amwg_rank_z_kernel(const long long* __res
   }
 }
 
+// ---- posterior covariance (sample_summary(..., covariance=...)) -------------------------------------------------------------
+// Record of a shard: chains, m[s] (mean of the chain means), B = sum_c (xbar_c - m)(xbar_c - m)^T and W = sum_c sum_r (x_rc -
+// xbar_c)(x_rc - xbar_c)^T over the selected entries. W is the Gram matrix of the block's draws centred by their chain means; B is
+// the same kernel's Gram matrix of the [1][sel][C] block of chain means centred by m.
+struct SelList { int e[kMaxSel]; };      // block entry of each selected slot, passed by value (512 B of kernel parameters)
+
+// K_c1: xbar[s][c] = the mean over rows of chain c of entry sel[s], summed sequentially as in K_m1
+__global__ void __launch_bounds__(256) amwg_chain_means_kernel(const double* __restrict__ x, long long rows, int entries, long long C, SelList sel,
+                                                               double* __restrict__ xbar) {
+  const int s = blockIdx.y;
+  const size_t stride = (size_t)entries * C;
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const double* p = x + (size_t)sel.e[s] * C + c;
+    double sum = 0.0;
+    long long r = 0;
+    for (; r + 8 <= rows; r += 8) {                          // eight loads in flight per thread, the sum stays sequential
+      double v[8];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) sum += v[u];
+    }
+    for (; r < rows; ++r) sum += p[r * stride];
+    xbar[(size_t)s * C + c] = sum / (double)rows;
+  }
+}
+
+// K_c2: m[s] = (sum over chains of xbar[s][c], in a fixed order) / C
+__global__ void __launch_bounds__(256) amwg_shard_mean_kernel(const double* __restrict__ xbar, long long C, double* __restrict__ m) {
+  __shared__ double sh[256];
+  const int s = blockIdx.x;
+  double acc = 0.0;
+#pragma unroll 8
+  for (long long c = threadIdx.x; c < C; c += 256) acc += xbar[(size_t)s * C + c];     // unrolled: eight loads in flight
+  const double tot = cta_sum<256>(sh, acc);
+  if (threadIdx.x == 0) m[s] = tot / (double)C;
+}
+
+__device__ __forceinline__ void dmma_8x8x4(double (&c)[2], double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};\n" : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
+}
+
+// *a when p, else 0 without touching memory: a predicated load, which the compiler schedules together with its neighbours (a load
+// under an `if` becomes a branch around it)
+__device__ __forceinline__ double load_if(bool p, const double* a) {
+  double v = 0.0;
+  asm("{\n .reg .pred q;\n setp.ne.b32 q, %2, 0;\n @q ld.global.nc.f64 %0, [%1];\n}" : "+d"(v) : "l"(a), "r"((int)p));
+  return v;
+}
+
+// stages values U0 .. U0 + 3 of this thread (value u is stage element i = threadIdx.x + u * kCoThreads; its chain is the lane,
+// kCoThreads and kCoChains being multiples of 32): eight loads in flight, then the stores to shared memory
+template <int U0>
+__device__ __forceinline__ void gram_stage_part(double* st, const double* __restrict__ x, long long rows, int entries, long long C,
+                                                const SelList& sel, int n_sel, const double* __restrict__ cen, long long cen_se,
+                                                long long cen_sc, int nb, int per_stage, long long c0, long long r0) {
+  double v[4];
+  int sm[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int i = threadIdx.x + (U0 + u) * kCoThreads;
+    const CoStageElem el = co_stage_elem(i, nb);
+    const long long r = r0 + el.rr, c = c0 + el.cc;
+    const bool p = i < per_stage && co_loads(r, el.s, c, rows, n_sel, C);
+    const int e = p ? sel.e[el.s] : 0;
+    v[u] = load_if(p, x + co_x_index(r, e, c, entries, C)) - load_if(p, cen + co_cen_index(el.s, c, cen_se, cen_sc));
+    sm[u] = i < per_stage ? co_smem_index(el.rr, el.s, el.cc, nb) : -1;
+  }
+#pragma unroll
+  for (int u = 0; u < 4; ++u)
+    if (sm[u] >= 0) st[sm[u]] = v[u];
+}
+
+// K_c3: partial[cta][rep][tile][8][8] = this CTA's share of the upper-triangle tiles of sum_k d[i][k] d[j][k], with d the draws
+// of x[row][sel[s]][chain] centred by cen[s * cen_se + chain * cen_sc]. Each CTA walks 32-chain groups (grid-stride) and, in each,
+// stages of co_stage_rows(nb) rows: the threads stage the centred values in shared memory (two parts of four values, each part's
+// eight loads in flight together; slots past n_sel and chains past C stage 0 and load nothing), then the warps add one DMMA per
+// (row, quad) to each of the <= 9 tiles they own (per rep, amwg_comoments.cuh). The accumulators stay in registers for the whole
+// walk: 128 registers, no spills, one 16-warp CTA per SM.
+__global__ void __launch_bounds__(kCoThreads, 1) amwg_gram_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                                  SelList sel, int n_sel, const double* __restrict__ cen, long long cen_se,
+                                                                  long long cen_sc, double* __restrict__ partial) {
+  __shared__ double st[kCoSmem];
+  const int nb = co_blocks(n_sel), srows = co_stage_rows(nb), reps = co_reps(nb);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, rep = co_warp_rep(warp, nb);
+  const int per_stage = srows * 8 * nb * kCoChains;
+  double acc[kCoSlots][2];
+  unsigned frag[kCoSlots];                                   // the slot's A and B fragment offsets (co_frag_lane < 2^16), packed
+  unsigned active = 0u;                                      // bit s: slot s holds a tile (warp-uniform)
+#pragma unroll
+  for (int s = 0; s < kCoSlots; ++s) {
+    acc[s][0] = acc[s][1] = 0.0;
+    const int t = co_slot_tile(warp, s, nb);
+    int bi = 0, bj = 0;
+    if (t >= 0) { co_tile(t, nb, bi, bj); active |= 1u << s; }
+    frag[s] = (unsigned)co_frag_lane(lane, bi) | ((unsigned)co_frag_lane(lane, bj) << 16);
+  }
+  static_assert(kCoStageValues == 8 * kCoThreads && kCoThreads % 32 == 0 && kCoChains == 32, "stage layout");
+  for (long long g = blockIdx.x; g * kCoChains < C; g += gridDim.x) {
+    const long long c0 = g * kCoChains;
+    const int nq = (int)((C - c0 < kCoChains ? C - c0 + 3 : kCoChains) / 4);     // quads holding at least one chain
+    for (long long r0 = 0; r0 < rows; r0 += srows) {
+      __syncthreads();                                       // every warp is done with the previous stage
+      gram_stage_part<0>(st, x, rows, entries, C, sel, n_sel, cen, cen_se, cen_sc, nb, per_stage, c0, r0);
+      gram_stage_part<4>(st, x, rows, entries, C, sel, n_sel, cen, cen_se, cen_sc, nb, per_stage, c0, r0);
+      __syncthreads();
+      const int nr = (int)(rows - r0 < srows ? rows - r0 : srows);
+      for (int k = rep; k < nr * nq; k += reps) {
+        const double* base = st + co_frag_base(k % nq, k / nq, nb);
+#pragma unroll
+        for (int s = 0; s < kCoSlots; ++s)
+          if (active & (1u << s)) dmma_8x8x4(acc[s], base[frag[s] & 0xffffu], base[frag[s] >> 16]);
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < kCoSlots; ++s) {
+    const int t = co_slot_tile(warp, s, nb);
+    if (t >= 0) {
+      partial[co_partial_index(blockIdx.x, rep, t, nb, lane, 0)] = acc[s][0];
+      partial[co_partial_index(blockIdx.x, rep, t, nb, lane, 1)] = acc[s][1];
+    }
+  }
+}
+
+// K_c4: out[v] = sum over the n_parts = CTAs * reps records, in that order, of partial[part][v] for v < n_vals (= tiles * 64)
+__global__ void __launch_bounds__(256) amwg_sum_tiles_kernel(const double* __restrict__ partial, int n_parts, int n_vals, double* __restrict__ out) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n_vals; v += gridDim.x * blockDim.x) {
+    double acc = 0.0;
+    for (int k = 0; k < n_parts; ++k) acc += partial[(size_t)k * n_vals + v];
+    out[v] = acc;
+  }
+}
+
 }  // namespace summary
 
 extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats) {
@@ -1010,5 +1150,85 @@ extern "C" int amwg_summary_histogram2d(int device, const double* dev_samples, i
                                                                                     reinterpret_cast<unsigned long long*>(dev_counts));
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+// bytes of device scratch amwg_summary_comoments uses (include/amwg.h states the formula; sample_summary counts it)
+static size_t comoments_scratch_bytes(int32_t n_sel, int64_t chains) {
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t tiles = (size_t)summary::co_tiles(summary::co_blocks(n_sel));
+  const size_t reps = (size_t)summary::co_reps(summary::co_blocks(n_sel));
+  return up((size_t)n_sel * chains * 8) + up((size_t)n_sel * 8) + up((size_t)summary::co_ctas(chains) * reps * tiles * 64 * 8) + up(2 * tiles * 64 * 8);
+}
+
+extern "C" int amwg_summary_comoments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                      const int32_t* host_sel, int32_t n_sel, double* host_out) {
+  if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_comoments: empty sample block");
+  if (n_sel < 1 || n_sel > summary::kMaxSel) return fail("amwg_summary_comoments: n_sel must be 1.." + std::to_string(summary::kMaxSel));
+  if (!dev_samples || !host_sel || !host_out) return fail("amwg_summary_comoments: null pointer");
+  summary::SelList sel{};
+  for (int i = 0; i < n_sel; ++i) {
+    if (host_sel[i] < 0 || host_sel[i] >= entries)
+      return fail("amwg_summary_comoments: selected entry " + std::to_string(i) + " is outside [0, entries)");
+    sel.e[i] = host_sel[i];
+  }
+  if (rows > (((int64_t)1 << 53) - 1) / chains) return fail("amwg_summary_comoments: rows * chains must be below 2^53");
+  if (device < 0 || device >= 64) return fail("amwg_summary_comoments: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const int nb = summary::co_blocks(n_sel), tiles = summary::co_tiles(nb), n_vals = tiles * 64;
+  const long long gx = summary::co_ctas(chains), parts = gx * summary::co_reps(nb);
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t b_xbar = up((size_t)n_sel * chains * 8), b_m = up((size_t)n_sel * 8), b_part = up((size_t)parts * n_vals * 8);
+  const size_t need = comoments_scratch_bytes(n_sel, chains);
+  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
+  struct Scratch { void* p = nullptr; size_t bytes = 0; };
+  static Scratch scratch[64];
+  static std::mutex scratch_mu;
+  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
+  Scratch& sc = scratch[device];
+  if (sc.bytes < need) {
+    if (sc.p) cudaFree(sc.p);
+    sc.p = nullptr; sc.bytes = 0;
+    CUDA_TRY(cudaMalloc(&sc.p, need));
+    sc.bytes = need;
+  }
+  char* base = reinterpret_cast<char*>(sc.p);
+  auto* xbar = reinterpret_cast<double*>(base);
+  auto* m = reinterpret_cast<double*>(base + b_xbar);
+  auto* part = reinterpret_cast<double*>(base + b_xbar + b_m);
+  auto* tw = reinterpret_cast<double*>(base + b_xbar + b_m + b_part);
+  double* tb = tw + n_vals;
+  summary::SelList ident{};
+  for (int i = 0; i < n_sel; ++i) ident.e[i] = i;
+  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned sx = (unsigned)((n_vals + 255) / 256);
+  summary::amwg_chain_means_kernel<<<dim3(bx, (unsigned)n_sel), 256>>>(dev_samples, rows, entries, chains, sel, xbar);
+  summary::amwg_shard_mean_kernel<<<(unsigned)n_sel, 256>>>(xbar, chains, m);
+  summary::amwg_gram_kernel<<<(unsigned)gx, summary::kCoThreads>>>(dev_samples, rows, entries, chains, sel, n_sel, xbar, chains, 1, part);
+  summary::amwg_sum_tiles_kernel<<<sx, 256>>>(part, (int)parts, n_vals, tw);
+  summary::amwg_gram_kernel<<<(unsigned)gx, summary::kCoThreads>>>(xbar, 1, n_sel, chains, ident, n_sel, m, 1, 0, part);
+  summary::amwg_sum_tiles_kernel<<<sx, 256>>>(part, (int)parts, n_vals, tb);
+  std::vector<double> hm(n_sel), ht(2 * (size_t)n_vals);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(hm.data(), m, hm.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(ht.data(), tw, ht.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return fail(std::string("amwg_summary_comoments: ") + cudaGetErrorString(e));
+  // host_out = { C, m[n], B[n][n], W[n][n] }: the upper triangle of each tile, mirrored, so both matrices are exactly symmetric
+  const size_t n = (size_t)n_sel;
+  double* oB = host_out + 1 + n;
+  double* oW = oB + n * n;
+  host_out[0] = (double)chains;
+  for (size_t i = 0; i < n; ++i) host_out[1 + i] = hm[i];
+  for (int t = 0; t < tiles; ++t) {
+    int bi = 0, bj = 0;
+    summary::co_tile(t, nb, bi, bj);
+    for (int r = 0; r < 8; ++r)
+      for (int c = 0; c < 8; ++c) {
+        const size_t i = 8 * (size_t)bi + r, j = 8 * (size_t)bj + c;
+        if (i > j || j >= n) continue;
+        oW[i * n + j] = oW[j * n + i] = ht[(size_t)t * 64 + r * 8 + c];
+        oB[i * n + j] = oB[j * n + i] = ht[(size_t)n_vals + (size_t)t * 64 + r * 8 + c];
+      }
+  }
   return 0;
 }

@@ -690,7 +690,7 @@ class AmwgSampler(Sampler):
             raise JsThrow(L.amwg_last_error().decode())
         return buf
 
-    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None):
+    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -721,9 +721,24 @@ class AmwgSampler(Sampler):
         numpy.histogram gives it (its equal-width arithmetic, in the same fp64 operations). Each pair adds a top-level entry keyed by
         the pair as given: {"hist": int64 [pair_bins, pair_bins] (a on axis 0), "xedges", "yedges"}, the edges being linspace(lo,
         hi, pair_bins + 1) of each selector's range; a draw counts when both values lie inside, binned as numpy.histogram2d bins
-        it. Every other key keeps its bits. A refused histogram raises ValueError before the chains move (summary.resolve_histogram)."""
+        it. Every other key keeps its bits. A refused histogram raises ValueError before the chains move (summary.resolve_histogram).
+        covariance=True adds the posterior covariance of every monitored entry, formed on the device (the cross-products of the
+        draws on the fp64 tensor core); a list of selectors (each a scalar's name or (name, flat_index), as for the histogram
+        pairs; at most 128 entries) covers those only, in the order given. The result gains the top-level key "covariance":
+        {"labels" (the selectors in matrix order; with True, every monitored name in order, a multi-dim one as (name, flat_index)
+        row-major), "mean" [k], "cov" [k, k] (ddof 1, over all rows and chains: numpy.cov of the pooled draws; its diagonal is
+        "sd" squared), "corr" [k, k] (numpy.corrcoef's), "within" (mean within-chain covariance, ddof 1), "between" (covariance
+        of the chain means, ddof 1), "rhat_multivariate" (Brooks & Gelman 1998: (n - 1)/n + (C + 1)/C lambda_max(within^-1
+        between), n kept rows, C chains; it flags chains that disagree on a combination of entries while every univariate R-hat
+        passes) and "n_draws"}. A NaN or +-inf draw makes its entry's rows and columns NaN, as numpy.cov does; rhat_multivariate
+        is NaN with fewer than 2 rows or chains, any non-finite entry, or a within matrix that is not positive definite (a
+        constant entry, or a derived quantity linear in others). The device scratch (summary.comoments_scratch_bytes) is counted
+        in the memory check. Every other key keeps its bits. A refused covariance (an unknown name, a component out of range,
+        more than 128 entries, anything but None / False / True / a list, or a monitored name "covariance") raises ValueError
+        before the chains move (summary.resolve_covariance); see summary.finalize_comoments for the arithmetic."""
         import torch
-        from .summary import CudaBlockReducer, check_diagnostics, histogram_block, resolve_histogram, summarise_block
+        from .summary import (CudaBlockReducer, check_diagnostics, comoments_scratch_bytes, covariance_block, histogram_block,
+                              resolve_covariance, resolve_histogram, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
@@ -733,7 +748,9 @@ class AmwgSampler(Sampler):
             spans[name] = (len(entries), len(e))
             entries.extend(e)
         named = [name for name in monitored if spans[name][1] > 0]
-        plan = resolve_histogram(histogram, named, {name: list(self.params[name]["dim"]) if name in self.params else [1] for name in named})
+        dims = {name: list(self.params[name]["dim"]) if name in self.params else [1] for name in named}
+        plan = resolve_histogram(histogram, named, dims)
+        cov_plan = resolve_covariance(covariance, named, dims)
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
@@ -746,6 +763,8 @@ class AmwgSampler(Sampler):
             # edges and counts of the histograms, and the extremes (8 B each)
             nb, pb = plan.bins or 0, plan.pair_bins
             need += 8 * (len(entries) * (2 * nb + 4 + pb + 1 + 5) + len(plan.pairs) * pb * pb)
+        if cov_plan is not None:
+            need += comoments_scratch_bytes(len(cov_plan.entries), self.local_chains)
         free, _total = torch.cuda.mem_get_info(dev)
         if need + 2 * len(entries) * self.local_chains * 8 > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
@@ -767,6 +786,7 @@ class AmwgSampler(Sampler):
         res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
         hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
+        cov = None if cov_plan is None else covariance_block(CudaBlockReducer(self.device), block, rows, cov_plan, self.distributed)
         del block
         out = {}
         for name in monitored:
@@ -787,6 +807,8 @@ class AmwgSampler(Sampler):
                     out[name][key] = val[0] if dim == [1] else val.reshape(*dim, val.shape[-1])
         if hist is not None:
             out.update(hist["pairs"])
+        if cov is not None:
+            out["covariance"] = cov
         return out
 
     def start_adaptation(self):

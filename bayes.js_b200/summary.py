@@ -10,7 +10,8 @@ radix-select digit counts (integers) -- so every rank returns the same numbers a
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
 amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True, and
 amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank", and
-amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=...). There is no CPU fallback:
+amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=..., and amwg_summary_comoments for
+the posterior covariance of covariance=...). There is no CPU fallback:
 without the library or a GPU the reducer raises.
 """
 from __future__ import annotations
@@ -235,6 +236,19 @@ class CudaBlockReducer:
         self._ffi.check(self.L.amwg_summary_histogram2d(self.device, block.data_ptr(), rows, entries, chains, pr.ctypes.data, len(pr),
                                                         ed.data_ptr(), bins, counts.data_ptr()))
         return counts
+
+    def comoments(self, block, sel) -> np.ndarray:
+        """-> flat record [1 + n + 2 n^2] {chains, m[n], B[n][n], W[n][n]} of the n selected entries of this shard; see
+        amwg_summary_comoments in include/amwg.h."""
+        import torch
+        rows, entries, chains = block.shape
+        s = np.ascontiguousarray(sel, dtype=np.int32)
+        n = len(s)
+        out = np.empty(1 + n + 2 * n * n, dtype=np.float64)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_comoments(self.device, block.data_ptr(), rows, entries, chains, s.ctypes.data, n,
+                                                      out.ctypes.data))
+        return out
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -732,4 +746,156 @@ def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed:
         c2 = counts.pop(0).reshape(len(plan.pairs), plan.pair_bins, plan.pair_bins)
         for i, (key, a, b) in enumerate(plan.pairs):
             out["pairs"][key] = {"hist": c2[i].copy(), "xedges": e2[a].copy(), "yedges": e2[b].copy()}
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# posterior covariance: cross-products of the draws on the fp64 tensor core, correlations, multivariate R-hat
+MAX_COV_ENTRIES = 128                  # include/amwg.h: amwg_summary_comoments, n_sel <= 128
+
+
+class CovariancePlan(NamedTuple):
+    """A checked `covariance=` argument: labels (the selectors in matrix order) and the block entry of each."""
+    labels: List[object]
+    entries: np.ndarray
+
+
+def resolve_covariance(spec, names: Sequence[str], dims) -> Optional[CovariancePlan]:
+    """Checks the `covariance=` argument of sample_summary against the monitored names (in sample-block order, only those with
+    entries) and their dims, as resolve_histogram does, and returns the plan, or None for None / False. True covers every
+    monitored entry (a scalar labelled by its name, a component of a multi-dim name by (name, flat_index), row-major); a list
+    covers the selectors it holds, in its order, each a scalar's name or (name, flat_index). Pure: raises ValueError before any
+    device work."""
+    if spec is None or spec is False:
+        return None
+    if "covariance" in names:
+        raise ValueError("covariance: a monitored parameter or derived quantity is named 'covariance', the key the result would use")
+    span = {}
+    entries = 0
+    for name in names:                                        # a name listed twice in monitor: its last block, as sample_summary
+        n = int(np.prod(dims[name]))
+        span[name] = (entries, n)
+        entries += n
+    if spec is True:
+        labels = [name if span[name][1] == 1 else (name, i) for name in span for i in range(span[name][1])]
+        idx = [span[name][0] + i for name in span for i in range(span[name][1])]
+    elif isinstance(spec, (list, tuple)):
+        labels, idx = [], []
+        for sel in spec:
+            if isinstance(sel, str):
+                if sel not in span:
+                    raise ValueError("covariance: %r is not a monitored parameter or derived quantity" % (sel,))
+                if span[sel][1] != 1:
+                    raise ValueError("covariance: %r has %d components; select one as (%r, flat_index)" % (sel, span[sel][1], sel))
+                label, e = sel, span[sel][0]
+            elif isinstance(sel, (tuple, list)) and len(sel) == 2 and isinstance(sel[0], str) and _is_int(sel[1]):
+                name, i = sel
+                if name not in span:
+                    raise ValueError("covariance: %r is not a monitored parameter or derived quantity" % (name,))
+                if not 0 <= i < span[name][1]:
+                    raise ValueError("covariance: component %d of %r is outside [0, %d)" % (i, name, span[name][1]))
+                label, e = (name, int(i)), span[name][0] + int(i)
+            else:
+                raise ValueError("covariance selector must be a name or (name, flat_index), not %r" % (sel,))
+            if e in idx:
+                raise ValueError("covariance: %r selects an entry already selected" % (sel,))
+            labels.append(label)
+            idx.append(e)
+        if not idx:
+            raise ValueError("covariance: the selector list is empty")
+    else:
+        raise ValueError("covariance must be None, True or a list of selectors, not %r" % (spec,))
+    if len(idx) > MAX_COV_ENTRIES:
+        raise ValueError("covariance: %d entries (max %d)" % (len(idx), MAX_COV_ENTRIES))
+    return CovariancePlan(labels, np.asarray(idx, dtype=np.int32))
+
+
+def comoments_scratch_bytes(n_sel: int, chains: int) -> int:
+    """Device scratch of amwg_summary_comoments (include/amwg.h)."""
+    up = lambda b: -(-b // 256) * 256
+    nb = -(-n_sel // 8)
+    tiles = nb * (nb + 1) // 2
+    reps = 1 if tiles >= 16 else 16 // tiles
+    ctas = min(-(-chains // 32), 264)
+    return up(8 * n_sel * chains) + up(8 * n_sel) + up(8 * 64 * tiles * ctas * reps) + up(8 * 128 * tiles)
+
+
+def split_comoment_record(rec: np.ndarray):
+    """flat record [1 + n + 2 n^2] -> (chains, m [n], B [n, n], W [n, n])."""
+    rec = np.asarray(rec, dtype=np.float64)
+    n = int(round((np.sqrt(8.0 * (rec.size - 1) + 1.0) - 1.0) / 4.0))
+    assert 1 + n + 2 * n * n == rec.size, rec.size
+    return rec[0], rec[1:1 + n], rec[1 + n:1 + n + n * n].reshape(n, n), rec[1 + n + n * n:].reshape(n, n)
+
+
+def merge_comoment_records(records: Sequence[np.ndarray]) -> np.ndarray:
+    """Chan merge of per-shard flat records {C, m[n], B[n][n], W[n][n]} in the order given (rank order), in matrix form:
+    B = B_a + B_b + (n_a n_b / n) d d^T with d = m_b - m_a, W adds. The arithmetic of merge_moment_records."""
+    na, ma, Ba, Wa = split_comoment_record(records[0])
+    ma, Ba, Wa = ma.copy(), Ba.copy(), Wa.copy()
+    for rec in records[1:]:
+        nb, mb, Bb, Wb = split_comoment_record(rec)
+        if nb == 0:
+            continue
+        if na == 0:
+            na, ma, Ba, Wa = nb, mb.copy(), Bb.copy(), Wb.copy()
+            continue
+        n = na + nb
+        d = mb - ma
+        ma = ma + d * (nb / n)
+        Ba = Ba + Bb + np.outer(d, d) * (na * nb / n)
+        Wa = Wa + Wb
+        na = n
+    return np.concatenate([[na], ma, Ba.ravel(), Wa.ravel()])
+
+
+def finalize_comoments(rec: np.ndarray, rows: int) -> dict:
+    """{"mean", "cov", "corr", "within", "between", "rhat_multivariate", "n_draws"} from the merged record. With C chains and
+    M = C rows draws: cov = (W + rows B) / (M - 1) (ddof 1; its diagonal is finalize_moments' sd squared), corr = cov / (sd sd^T)
+    in numpy.corrcoef's operations (clipped to [-1, 1]), within = W / (C (rows - 1)), between = B / (C - 1) and Brooks & Gelman's
+    (1998) multivariate potential scale reduction (n - 1)/n + (C + 1)/C lambda_max(within^-1 between), n = rows, from a Cholesky
+    factor of within and eigvalsh. The R-hat is NaN when rows < 2, C < 2, any entry is non-finite, or within is not positive
+    definite (a constant entry, or one that is linear in others)."""
+    G, m, B, W = split_comoment_record(rec)
+    M = G * rows
+    with np.errstate(invalid="ignore", divide="ignore"):
+        cov = (W + rows * B) / (M - 1)
+        sd = np.sqrt(np.diag(cov))
+        corr = cov / sd[:, None]
+        corr /= sd[None, :]
+        np.clip(corr, -1, 1, out=corr)
+        within = W / (G * (rows - 1))
+        between = B / (G - 1)
+    rhat = np.nan
+    if rows >= 2 and G >= 2 and np.all(np.isfinite(within)) and np.all(np.isfinite(between)):
+        try:
+            L = np.linalg.cholesky(within)
+        except np.linalg.LinAlgError:
+            L = None
+        if L is not None:
+            Li = np.linalg.inv(L)
+            S = Li @ between @ Li.T
+            lam = np.linalg.eigvalsh((S + S.T) / 2).max()
+            rhat = float((rows - 1) / rows + (G + 1) / G * lam)
+    return {"mean": m.copy(), "cov": cov, "corr": corr, "within": within, "between": between, "rhat_multivariate": rhat,
+            "n_draws": int(M)}
+
+
+def covariance_block(reducer, block, rows: int, plan: CovariancePlan, distributed: bool) -> dict:
+    """-> finalize_comoments' dict plus "labels", over all shards; only reads the block. Each shard's record comes from
+    reducer.comoments; distributed: one all_gather_into_tensor of the fixed-size records, merged on the host in rank order,
+    so every rank returns the same bits."""
+    rec = reducer.comoments(block, plan.entries)
+    if distributed:
+        import torch
+        import torch.distributed as dist
+        ws = dist.get_world_size()
+        mine = torch.from_numpy(np.ascontiguousarray(rec))
+        if block.is_cuda:
+            mine = mine.to(block.device)
+        gathered = torch.empty(ws * rec.size, dtype=mine.dtype, device=mine.device)
+        dist.all_gather_into_tensor(gathered, mine)
+        rec = merge_comoment_records(list(gathered.cpu().numpy().reshape(ws, rec.size)))
+    out = {"labels": list(plan.labels)}
+    out.update(finalize_comoments(rec, rows))
     return out

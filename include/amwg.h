@@ -346,7 +346,20 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   host_pairs[pair][1] (axis 1) over their rows of dev_edges[entry][bins + 1], by numpy.histogramdd's rule (per axis
  *   searchsorted(edges, v, "right") - 1, the last edge in the last bin); a draw counts only when both values fall inside (NaN
  *   never does). host_pairs is host memory. Errors: bins outside 1..128, n_pairs outside 1..64, a pair entry outside
- *   [0, entries), rows >= 2^32, an empty block, null pointers. */
+ *   [0, entries), rows >= 2^32, an empty block, null pointers.
+ *
+ * Posterior covariance (sample_summary(..., covariance=...)): the matrix form of amwg_summary_moments' record, for the n_sel
+ * entries host_sel[0 .. n_sel) (host memory).
+ * amwg_summary_comoments: host_out[1 + n_sel + 2 n_sel^2] = { C (chains), m[n_sel] (mean of the chain means),
+ *   B[n_sel][n_sel] = sum_c (xbar_c - m)(xbar_c - m)^T (co-M2 of the chain means), W[n_sel][n_sel] = sum_c sum_r (x_rc - xbar_c)
+ *   (x_rc - xbar_c)^T (summed within-chain co-M2) }, row-major and exactly symmetric. xbar_c is a sequential sum over the rows
+ *   divided by rows; m sums the chain means in a fixed order. B and W are Gram matrices of the centred values, formed on the fp64
+ *   tensor core (mma.sync m8n8k4) by a grid whose size depends on chains only and summed in a fixed order: two calls give the
+ *   same bits. A NaN or +-inf draw of an entry makes that entry's rows and columns of B and W NaN. Records of shards merge like
+ *   amwg_summary_moments' (Chan, in matrix form). Device scratch, from a per-device pool grown on demand: with T = nb (nb + 1) / 2
+ *   tiles, nb = ceil(n_sel / 8), R = 1 when T >= 16 else floor(16 / T) warps per tile and G = min(ceil(chains / 32), 264) CTAs,
+ *   8 (n_sel chains + n_sel + 64 T R G + 128 T) bytes, each of the four parts rounded up to 256 bytes. Errors (nothing is touched): an empty block, n_sel outside 1..128, null
+ *   pointers, a selected entry outside [0, entries), rows * chains >= 2^53. */
 AMWG_API int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats);
 AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t pass,
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
@@ -362,6 +375,8 @@ AMWG_API int amwg_summary_histogram(int device, const double* dev_samples, int64
                                     const double* dev_edges, int32_t bins, int64_t* dev_counts);
 AMWG_API int amwg_summary_histogram2d(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
                                       const int32_t* host_pairs, int32_t n_pairs, const double* dev_edges, int32_t bins, int64_t* dev_counts);
+AMWG_API int amwg_summary_comoments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                    const int32_t* host_sel, int32_t n_sel, double* host_out);
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it

@@ -505,6 +505,16 @@ BINDING(summary_histogram2d)
     fail_from_library();
   return js_undefined(env);
 END_BINDING
+// summary_comoments(device, samples ptr, rows, entries, chains, selected entries [n_sel]) -> Float64Array [1 + n_sel + 2 n_sel^2]
+//                                                                                                         amwg_summary_comoments
+BINDING(summary_comoments)
+  const std::vector<int32_t> sel = ints(env, a.at(5));
+  std::vector<double> out(1 + sel.size() + 2 * sel.size() * sel.size());
+  if (amwg_summary_comoments((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                             (int32_t)to_double(env, a.at(3)), (int64_t)to_double(env, a.at(4)), sel.data(), (int32_t)sel.size(), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
 // term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
 BINDING(term_cache)
   Handle* h = handle_of(env, a.at(0));
@@ -538,6 +548,7 @@ NAPI_MODULE_INIT() {
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
+      {"summary_comoments", summary_comoments},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
