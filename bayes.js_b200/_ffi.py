@@ -69,7 +69,7 @@ EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_samp
            "amwg_summary_moments", "amwg_summary_digit_hist", "amwg_summary_autocov", "amwg_summary_rank_sort",
            "amwg_summary_rank_count", "amwg_summary_rank_z", "amwg_peak_fp64", "amwg_jit_status", "amwg_jit_compile_check",
            "amwg_plate_sources", "amwg_get_term_cache", "amwg_summary_finite_range", "amwg_summary_histogram", "amwg_summary_histogram2d",
-           "amwg_summary_comoments"]
+           "amwg_summary_comoments", "amwg_disperse_state_superchains", "amwg_summary_nested"]
 
 _lib = None
 
@@ -99,6 +99,7 @@ def lib():
     L.amwg_get_log_post.argtypes = [vp, vp]; L.amwg_get_log_post.restype = C.c_int
     L.amwg_set_state.argtypes = [vp, vp]; L.amwg_set_state.restype = C.c_int
     L.amwg_disperse_state.argtypes = [vp, dbl, C.POINTER(i64)]; L.amwg_disperse_state.restype = C.c_int
+    L.amwg_disperse_state_superchains.argtypes = [vp, dbl, i64, C.POINTER(i64)]; L.amwg_disperse_state_superchains.restype = C.c_int
     L.amwg_model_fingerprint.argtypes = [C.POINTER(AmwgModel), C.POINTER(u64)]; L.amwg_model_fingerprint.restype = C.c_int
     L.amwg_checkpoint_size.argtypes = [vp, C.POINTER(i64)]; L.amwg_checkpoint_size.restype = C.c_int
     L.amwg_checkpoint_save.argtypes = [vp, vp, i64]; L.amwg_checkpoint_save.restype = C.c_int
@@ -122,6 +123,7 @@ def lib():
     L.amwg_summary_histogram.argtypes = [C.c_int, vp, i64, i32, i64, vp, i32, vp]; L.amwg_summary_histogram.restype = C.c_int
     L.amwg_summary_histogram2d.argtypes = [C.c_int, vp, i64, i32, i64, vp, i32, vp, i32, vp]; L.amwg_summary_histogram2d.restype = C.c_int
     L.amwg_summary_comoments.argtypes = [C.c_int, vp, i64, i32, i64, vp, i32, vp]; L.amwg_summary_comoments.restype = C.c_int
+    L.amwg_summary_nested.argtypes = [C.c_int, vp, i64, i32, i64, i64, i64, vp]; L.amwg_summary_nested.restype = C.c_int
     L.amwg_jit_status.argtypes = [vp, C.c_char_p, i64]; L.amwg_jit_status.restype = C.c_int
     L.amwg_plate_sources.argtypes = [vp, C.c_char_p, i64]; L.amwg_plate_sources.restype = C.c_int
     L.amwg_get_term_cache.argtypes = [vp, vp, i64]; L.amwg_get_term_cache.restype = C.c_int

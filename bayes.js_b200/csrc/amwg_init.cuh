@@ -12,6 +12,14 @@ namespace amwg {
 constexpr int kDisperseAttempts = 100;                 // attempts per chain before amwg_disperse_state gives up
 constexpr uint64_t kInitStreamBase = 1ull << 63;       // uniform #(2^63 + a*n_comp + c): Math.random() never gets there
 
+// The chain whose stream draws the attempts of global chain `chain` when superchains of `superchain_size` consecutive chains
+// start together (amwg_disperse_state_superchains): the superchain's first chain, superchain_size * floor(chain /
+// superchain_size). Every chain of a superchain then draws the same attempts and keeps the same point; superchain_size = 1 is
+// the chain itself.
+__device__ __forceinline__ uint64_t superchain_leader(uint64_t chain, uint64_t superchain_size) {
+  return chain - chain % superchain_size;
+}
+
 // uniform of attempt `attempt` for component `c` of global chain `chain`
 __device__ __forceinline__ double disperse_uniform(uint64_t seed, uint64_t chain, int attempt, int n_comp, int c) {
   RandomStream g;

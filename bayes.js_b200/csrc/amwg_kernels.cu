@@ -791,8 +791,8 @@ __global__ void __launch_bounds__(kThreads) amwg_relp_kernel(ModelDev m, ChainAr
 // stores nothing. It stays CTA-uniform: chains that are done evaluate their kept point, shadow threads chain C-1's, and neither
 // writes. `remaining` receives the number of chains still without a point (one atomic per CTA).
 __global__ void __launch_bounds__(kThreads) amwg_disperse_kernel(ModelDev m, ChainArrays a, const double* __restrict__ init, double radius,
-                                                                int attempt, double* __restrict__ scratch, unsigned char* __restrict__ done,
-                                                                unsigned long long* __restrict__ remaining) {
+                                                                unsigned long long superchain_size, int attempt, double* __restrict__ scratch,
+                                                                unsigned char* __restrict__ done, unsigned long long* __restrict__ remaining) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -803,11 +803,12 @@ __global__ void __launch_bounds__(kThreads) amwg_disperse_kernel(ModelDev m, Cha
   const bool todo = valid && !done[chain];
   bool ok = true;
   if (todo) {
+    const unsigned long long leader = superchain_leader(a.first_chain + chain, superchain_size);
     for (int p = 0; p < m.n_params; ++p) {
       const amwg_param& pa = ctx.params[p];
       for (int k = 0; k < pa.n_comp; ++k) {
         const int c = pa.comp_offset + k;
-        const double U = disperse_uniform(a.seed, a.first_chain + chain, attempt, m.D, c);
+        const double U = disperse_uniform(a.seed, leader, attempt, m.D, c);
         double x;
         ok = disperse_component(pa.type, pa.lower, pa.upper, init[c], radius, U, &x) && ok;
         scratch[(unsigned long long)c * a.C + chain] = x;
@@ -1952,9 +1953,14 @@ extern "C" int amwg_set_state(amwg_sampler* s, const double* host_in) {
 }
 
 extern "C" int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_failed) {
+  return amwg_disperse_state_superchains(s, radius, 1, n_failed);
+}
+
+extern "C" int amwg_disperse_state_superchains(amwg_sampler* s, double radius, int64_t superchain_size, int64_t* n_failed) {
   if (n_failed) *n_failed = 0;
   if (!s) return fail("amwg_disperse_state: NULL handle");
   if (!(radius > 0.0) || radius == INFINITY) return fail("amwg_disperse_state: radius must be finite and > 0");
+  if (superchain_size < 1) return fail("amwg_disperse_state: superchain_size must be >= 1");
   CUDA_TRY(cudaSetDevice(s->device));
   const unsigned long long C = s->a.C;
   double* d_x = nullptr;
@@ -1969,7 +1975,8 @@ extern "C" int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_fa
     for (int attempt = 0; e == cudaSuccess && left > 0 && attempt < kDisperseAttempts; ++attempt) {
       e = cudaMemsetAsync(d_left, 0, sizeof(unsigned long long), s->stream);
       if (e != cudaSuccess) break;
-      amwg_disperse_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, s->d_init, radius, attempt, d_x, d_done, d_left);
+      amwg_disperse_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, s->d_init, radius, (unsigned long long)superchain_size,
+                                                                                           attempt, d_x, d_done, d_left);
       s->launches++;
       e = cudaGetLastError();
       if (e == cudaSuccess) e = cudaMemcpyAsync(&left, d_left, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s->stream);

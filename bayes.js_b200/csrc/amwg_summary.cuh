@@ -27,11 +27,15 @@
 //   K_c3  amwg_gram_kernel          : upper-triangle 8 x 8 tiles of the Gram matrix of centred draws on the fp64 tensor core
 //                                     (mma.sync m8n8k4 f64), 32-chain stages in shared memory; addressing in amwg_comoments.cuh
 //   K_c4  amwg_sum_tiles_kernel     : sums the per-CTA partial tiles in CTA order
+//   K_n1  amwg_nested_chain_kernel  : one thread per (chain, entry): mean and M2 of the chain over its rows (as K_m1), stored
+//   K_n2  amwg_nested_seg_kernel    : one thread per superchain segment: its chains merged in chain order; complete superchains
+//                                     as unit records into a fixed CTA tree (then K_m2), cut ones stored for the host
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
 
 #include "amwg_comoments.cuh"
 #include "amwg_hist.cuh"
+#include "amwg_nested.cuh"      // Moments and merge
 
 namespace summary {
 
@@ -39,24 +43,11 @@ constexpr int kMaxPrefixes = 32;      // distinct prefixes per entry and pass (o
 // CTAs per entry of the chain-wise kernels (fewer when there are fewer 256-chain groups): a fixed number, not the device's SM
 // count, because it sets the merge order of the moments and so their last bits; ~9 CTAs per SM of an H100.
 constexpr long long kChainCtas = 1184;
+static_assert(kNestedCtas == kChainCtas, "amwg_nested.cuh caps the segment kernel's grid like the chain-wise kernels");
 
 __device__ __forceinline__ unsigned long long ordered_key(double x) {
   unsigned long long u = (unsigned long long)__double_as_longlong(x);
   return (u >> 63) ? ~u : (u | 0x8000000000000000ull);      // ascending keys == ascending doubles (-0 < +0, NaN on top)
-}
-
-struct Moments { double n, mean, m2, sum_w; };     // n chain means merged so far; sum_w = sum of the within-chain M2
-
-__device__ __forceinline__ Moments merge(const Moments& a, const Moments& b) {
-  if (b.n == 0.0) return a;
-  if (a.n == 0.0) return b;
-  Moments r;
-  r.n = a.n + b.n;
-  const double d = b.mean - a.mean;
-  r.mean = a.mean + d * (b.n / r.n);
-  r.m2 = a.m2 + b.m2 + d * d * (a.n * b.n / r.n);
-  r.sum_w = a.sum_w + b.sum_w;
-  return r;
 }
 
 template <int THREADS>
@@ -80,29 +71,7 @@ __global__ void __launch_bounds__(256) amwg_chain_moments_kernel(const double* _
   const size_t stride = (size_t)entries * C;
   Moments acc{0.0, 0.0, 0.0, 0.0};
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
-    const double* p = x + (size_t)e * C + c;
-    double s = 0.0;
-    long long r = 0;
-    for (; r + 8 <= rows; r += 8) {                          // eight loads in flight per thread, the sum stays sequential
-      double v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) s += v[u];
-    }
-    for (; r < rows; ++r) s += p[r * stride];
-    const double m = s / (double)rows;
-    double m2 = 0.0;
-    r = 0;
-    for (; r + 8 <= rows; r += 8) {
-      double v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) { double d = v[u] - m; m2 = fma(d, d, m2); }
-    }
-    for (; r < rows; ++r) { double d = p[r * stride] - m; m2 = fma(d, d, m2); }
-    acc = merge(acc, Moments{1.0, m, 0.0, m2});
+    acc = merge(acc, chain_record(x + (size_t)e * C + c, rows, stride));
   }
   const Moments tot = cta_merge<256>(sh, acc);
   if (threadIdx.x == 0) partial[(size_t)e * gridDim.x + blockIdx.x] = tot;
@@ -877,6 +846,40 @@ __global__ void __launch_bounds__(256) amwg_sum_tiles_kernel(const double* __res
   }
 }
 
+// ---- nested R-hat (sample_summary(..., nested=M), DESIGN.md §4.6); addressing and merges in amwg_nested.cuh -------------------
+// K_n1: cm[e][c], cw[e][c] = mean and M2 of chain c of entry e over its rows (two sequential passes, as in K_m1)
+__global__ void __launch_bounds__(256) amwg_nested_chain_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                                double* __restrict__ cm, double* __restrict__ cw) {
+  const int e = blockIdx.y;
+  const size_t stride = (size_t)entries * C;
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    const Moments r = chain_record(x + (size_t)e * C + c, rows, stride);
+    cm[(size_t)e * C + c] = r.mean;
+    cw[(size_t)e * C + c] = r.sum_w;
+  }
+}
+
+// K_n2: one thread per segment (grid-stride): its chains merged in chain order. A complete segment becomes its superchain's unit
+// record, merged into the thread's accumulator and then in the fixed CTA tree into partial[e][cta]; a cut one goes to cut[e][slot]
+// as its chain-level record. The grid depends on the number of segments only, so the merge order is fixed.
+__global__ void __launch_bounds__(256) amwg_nested_seg_kernel(const double* __restrict__ cm, const double* __restrict__ cw, long long C,
+                                                              long long first_chain, long long M, long long rows, long long n_seg,
+                                                              Moments* __restrict__ partial, Moments* __restrict__ cut) {
+  __shared__ Moments sh[256];
+  const int e = blockIdx.y;
+  Moments acc{0.0, 0.0, 0.0, 0.0};
+  for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < n_seg; s += (long long)gridDim.x * blockDim.x) {
+    long long c0, c1;
+    nested_range(s, first_chain, C, M, c0, c1);
+    const Moments r = nested_chain_merge(cm + (size_t)e * C, cw + (size_t)e * C, c0, c1);
+    const int slot = nested_cut_slot(s, first_chain, C, M);
+    if (slot < 0) acc = merge(acc, nested_unit(r, M, rows));
+    else cut[(size_t)e * 2 + slot] = r;
+  }
+  const Moments tot = cta_merge<256>(sh, acc);
+  if (threadIdx.x == 0) partial[(size_t)e * gridDim.x + blockIdx.x] = tot;
+}
+
 }  // namespace summary
 
 extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats) {
@@ -1229,6 +1232,75 @@ extern "C" int amwg_summary_comoments(int device, const double* dev_samples, int
         oW[i * n + j] = oW[j * n + i] = ht[(size_t)t * 64 + r * 8 + c];
         oB[i * n + j] = oB[j * n + i] = ht[(size_t)n_vals + (size_t)t * 64 + r * 8 + c];
       }
+  }
+  return 0;
+}
+
+// bytes of device scratch amwg_summary_nested uses (include/amwg.h states the formula; sample_summary counts it)
+static size_t nested_scratch_bytes(int32_t entries, int64_t chains, int64_t n_seg) {
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t bx = (size_t)summary::nested_seg_ctas(n_seg);
+  return up((size_t)entries * chains * 16) + up((size_t)entries * bx * 32) + up((size_t)entries * 32) + up((size_t)entries * 64);
+}
+
+extern "C" int amwg_summary_nested(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int64_t first_chain,
+                                   int64_t superchain_size, double* host_out) {
+  if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_nested: empty sample block");
+  if (!dev_samples || !host_out) return fail("amwg_summary_nested: null pointer");
+  if (superchain_size < 1) return fail("amwg_summary_nested: superchain_size must be >= 1");
+  if (first_chain < 0) return fail("amwg_summary_nested: first_chain must be >= 0");
+  if (first_chain > ((int64_t)1 << 53) - chains) return fail("amwg_summary_nested: first_chain + chains must be at most 2^53");
+  if (device < 0 || device >= 64) return fail("amwg_summary_nested: device index out of range");
+  CUDA_TRY(cudaSetDevice(device));
+  const long long M = superchain_size, n_seg = summary::nested_segments(first_chain, chains, M);
+  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned sx = (unsigned)summary::nested_seg_ctas(n_seg);     // depends on n_seg only: a fixed merge order
+  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
+  const size_t b_chain = up((size_t)entries * chains * 16), b_part = up((size_t)entries * sx * sizeof(summary::Moments));
+  const size_t b_out = up((size_t)entries * 4 * sizeof(double));
+  const size_t need = nested_scratch_bytes(entries, chains, n_seg);
+  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
+  struct Scratch { void* p = nullptr; size_t bytes = 0; };
+  static Scratch scratch[64];
+  static std::mutex scratch_mu;
+  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
+  Scratch& sc = scratch[device];
+  if (sc.bytes < need) {
+    if (sc.p) cudaFree(sc.p);
+    sc.p = nullptr; sc.bytes = 0;
+    CUDA_TRY(cudaMalloc(&sc.p, need));
+    sc.bytes = need;
+  }
+  char* base = reinterpret_cast<char*>(sc.p);
+  auto* cm = reinterpret_cast<double*>(base);
+  auto* cw = cm + (size_t)entries * chains;
+  auto* part = reinterpret_cast<summary::Moments*>(base + b_chain);
+  auto* d_out = reinterpret_cast<double*>(base + b_chain + b_part);
+  auto* cut = reinterpret_cast<summary::Moments*>(base + b_chain + b_part + b_out);
+  summary::amwg_nested_chain_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, cm, cw);
+  summary::amwg_nested_seg_kernel<<<dim3(sx, (unsigned)entries), 256>>>(cm, cw, chains, first_chain, M, rows, n_seg, part, cut);
+  summary::amwg_merge_moments_kernel<<<(unsigned)entries, 1024>>>(part, (int)sx, d_out);
+  std::vector<double> tot((size_t)entries * 4), cr((size_t)entries * 8);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(tot.data(), d_out, tot.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(cr.data(), cut, cr.size() * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return fail(std::string("amwg_summary_nested: ") + cudaGetErrorString(e));
+  // host_out[entry][14] = { complete record (4), then per cut slot { superchain id (-1: none), chains, mean, M2, sum_w } }
+  long long slot_seg[2] = {-1, -1};
+  for (long long s : {0LL, n_seg - 1}) {
+    const int slot = summary::nested_cut_slot(s, first_chain, chains, M);
+    if (slot >= 0) slot_seg[slot] = s;
+  }
+  for (int32_t en = 0; en < entries; ++en) {
+    double* o = host_out + (size_t)en * summary::kNestedRecord;
+    for (int i = 0; i < 4; ++i) o[i] = tot[(size_t)en * 4 + i];
+    for (int slot = 0; slot < 2; ++slot) {
+      double* q = o + 4 + 5 * slot;
+      const double* r = cr.data() + ((size_t)en * 2 + slot) * 4;
+      if (slot_seg[slot] < 0) { q[0] = -1.0; q[1] = q[2] = q[3] = q[4] = 0.0; continue; }
+      q[0] = (double)summary::nested_superchain(slot_seg[slot], first_chain, M);
+      for (int i = 0; i < 4; ++i) q[1 + i] = r[i];
+    }
   }
   return 0;
 }

@@ -12,7 +12,8 @@ New, non-reference options (the many-chain setting needs them): ``chains`` (defa
 shaped exactly like the reference's), ``seed``, ``device``, ``distributed``, ``first_chain`` (global id of
 the first chain, default 0), ``faithful`` (no factorised likelihood plates: bit-faithful, slower),
 ``init_radius`` (over-dispersed starting points drawn on the device, DESIGN.md §2; default: every chain
-starts at the params' init). ``sampler.set_state(values)`` places the chains anywhere; ``sampler.checkpoint()`` and
+starts at the params' init), ``superchain_size`` (chains per superchain: with ``init_radius`` the chains of a
+superchain start at one point, and ``sample_summary(n, nested=True)`` uses it; DESIGN.md §4.6). ``sampler.set_state(values)`` places the chains anywhere; ``sampler.checkpoint()`` and
 ``sampler.restore(images)`` stop and resume a run bit for bit.
 """
 from __future__ import annotations
@@ -390,6 +391,13 @@ class AmwgSampler(Sampler):
         if radius is not None and not (is_number(radius) and math.isfinite(radius) and radius > 0):
             raise JsThrow("options.init_radius must be a finite number > 0")
         self.init_radius = None if radius is None else float(radius)
+        size = get_option("superchain_size", options, None)               # chains per superchain (nested R-hat, DESIGN.md §4.6)
+        if size is not None:
+            if not (is_number(size) and math.isfinite(size) and size >= 1 and size == math.floor(size)):
+                raise JsThrow("options.superchain_size must be an integer >= 1")
+            if self.n_chains % int(size):
+                raise JsThrow("options.superchain_size must divide options.chains")
+        self.superchain_size = None if size is None else int(size)
 
         # flat component layout: Object.keys(params) order, row-major inside a parameter
         self._offsets: Dict[str, int] = {}
@@ -500,11 +508,12 @@ class AmwgSampler(Sampler):
             self._disperse(self.init_radius)
 
     def _disperse(self, radius: float):
-        """options.init_radius: every chain to its first valid point of the device's dispersal (amwg_disperse_state). With
-        options.distributed the failed chains are counted over all ranks, so that every rank raises the same message or none."""
+        """options.init_radius: every chain to its first valid point of the device's dispersal (amwg_disperse_state_superchains; with
+        options.superchain_size the chains of a superchain share one point). With options.distributed the failed chains are counted
+        over all ranks, so that every rank raises the same message or none."""
         L = _ffi.lib()
         failed = C.c_int64(0)
-        rc = L.amwg_disperse_state(self._handle, float(radius), C.byref(failed))
+        rc = L.amwg_disperse_state_superchains(self._handle, float(radius), self.superchain_size or 1, C.byref(failed))
         err = L.amwg_last_error().decode() if rc != 0 else ""
         msg = dispersal_failure_message(failed.value, self.n_chains, self.distributed, self.device)
         if rc != 0 or msg:
@@ -690,7 +699,8 @@ class AmwgSampler(Sampler):
             raise JsThrow(L.amwg_last_error().decode())
         return buf
 
-    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None):
+    def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None,
+                       nested=None):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -735,10 +745,23 @@ class AmwgSampler(Sampler):
         constant entry, or a derived quantity linear in others). The device scratch (summary.comoments_scratch_bytes) is counted
         in the memory check. Every other key keeps its bits. A refused covariance (an unknown name, a component out of range,
         more than 128 entries, anything but None / False / True / a list, or a monitored name "covariance") raises ValueError
-        before the chains move (summary.resolve_covariance); see summary.finalize_comoments for the arithmetic."""
+        before the chains move (summary.resolve_covariance); see summary.finalize_comoments for the arithmetic.
+        nested=M adds "rhat_nested" to every monitored name, shaped like "mean": the nested R-hat of Margossian et al. (Bayesian
+        Analysis 2024) for superchains of M chains, superchain k being the global chains [kM, (k + 1)M). It is built for many
+        short chains: it compares the superchain means with the variance inside the superchains, is defined for one kept row, and
+        tends to 1 once the ensemble of chains is stationary, whether or not each chain is long. nested=True takes M from
+        options.superchain_size, which with options.init_radius also starts the chains of each superchain at one point; nested=M
+        sets it for this call (for chains placed with set_state). With N kept rows, K superchains, chain means xbar_km,
+        superchain means xbar_k and xbar their mean: B^ = sum_k (xbar_k - xbar)^2 / (K - 1), B~_k = sum_m (xbar_km - xbar_k)^2 /
+        (M - 1) (0 when M = 1), W-_k = (1/M) sum_m sum_n (x_nmk - xbar_km)^2 / (N - 1) (0 when N = 1), W^ = (1/K) sum_k (B~_k +
+        W-_k), rhat_nested = sqrt(1 + B^ / W^); NaN when K < 2, W^ = 0 or any draw of the entry is not finite. The chains
+        summarised (this handle's, or all of them with options.distributed) must be whole superchains. The device scratch
+        (summary.nested_scratch_bytes) is counted in the memory check. Every other key keeps its bits. A refused nested (True
+        without options.superchain_size, anything but None / False / True / an int >= 1, or chains that are not whole
+        superchains) raises ValueError before the chains move (summary.resolve_nested); see summary.finalize_nested."""
         import torch
-        from .summary import (CudaBlockReducer, check_diagnostics, comoments_scratch_bytes, covariance_block, histogram_block,
-                              resolve_covariance, resolve_histogram, summarise_block)
+        from .summary import (CudaBlockReducer, check_diagnostics, comoments_scratch_bytes, covariance_block, histogram_block, nested_block,
+                              nested_scratch_bytes, resolve_covariance, resolve_histogram, resolve_nested, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
@@ -751,6 +774,8 @@ class AmwgSampler(Sampler):
         dims = {name: list(self.params[name]["dim"]) if name in self.params else [1] for name in named}
         plan = resolve_histogram(histogram, named, dims)
         cov_plan = resolve_covariance(covariance, named, dims)
+        first, held = (0, self.n_chains) if self.distributed else (self.first_chain, self.local_chains)
+        superchain = resolve_nested(nested, self.superchain_size, first, held)
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
@@ -765,6 +790,8 @@ class AmwgSampler(Sampler):
             need += 8 * (len(entries) * (2 * nb + 4 + pb + 1 + 5) + len(plan.pairs) * pb * pb)
         if cov_plan is not None:
             need += comoments_scratch_bytes(len(cov_plan.entries), self.local_chains)
+        if superchain is not None:
+            need += nested_scratch_bytes(len(entries), self.local_chains, self.first_chain, superchain)
         free, _total = torch.cuda.mem_get_info(dev)
         if need + 2 * len(entries) * self.local_chains * 8 > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
@@ -787,6 +814,8 @@ class AmwgSampler(Sampler):
         mean, sd, rhat, q = res[:4]
         hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
         cov = None if cov_plan is None else covariance_block(CudaBlockReducer(self.device), block, rows, cov_plan, self.distributed)
+        rn = None if superchain is None else nested_block(CudaBlockReducer(self.device), block, rows, self.first_chain, superchain,
+                                                          self.distributed)
         del block
         out = {}
         for name in monitored:
@@ -805,6 +834,8 @@ class AmwgSampler(Sampler):
                 for key in ("hist", "hist_edges", "hist_outside"):
                     val = hist[key][s0:s0 + ln]
                     out[name][key] = val[0] if dim == [1] else val.reshape(*dim, val.shape[-1])
+            if rn is not None:
+                out[name]["rhat_nested"] = shape(rn[s0:s0 + ln])
         if hist is not None:
             out.update(hist["pairs"])
         if cov is not None:

@@ -10,8 +10,8 @@ radix-select digit counts (integers) -- so every rank returns the same numbers a
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
 amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True, and
 amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank", and
-amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=..., and amwg_summary_comoments for
-the posterior covariance of covariance=...). There is no CPU fallback:
+amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=..., amwg_summary_comoments for
+the posterior covariance of covariance=..., and amwg_summary_nested for the nested R-hat of nested=...). There is no CPU fallback:
 without the library or a GPU the reducer raises.
 """
 from __future__ import annotations
@@ -248,6 +248,17 @@ class CudaBlockReducer:
         torch.cuda.current_stream(block.device).synchronize()
         self._ffi.check(self.L.amwg_summary_comoments(self.device, block.data_ptr(), rows, entries, chains, s.ctypes.data, n,
                                                       out.ctypes.data))
+        return out
+
+    def nested(self, block, first_chain: int, superchain_size: int) -> np.ndarray:
+        """-> [entries, 14]: this shard's complete-superchain record and its two cut records; see amwg_summary_nested in
+        include/amwg.h."""
+        import torch
+        rows, entries, chains = block.shape
+        out = np.empty((entries, NESTED_RECORD), dtype=np.float64)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_nested(self.device, block.data_ptr(), rows, entries, chains, first_chain, superchain_size,
+                                                   out.ctypes.data))
         return out
 
 
@@ -899,3 +910,105 @@ def covariance_block(reducer, block, rows: int, plan: CovariancePlan, distribute
     out = {"labels": list(plan.labels)}
     out.update(finalize_comoments(rec, rows))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# nested R-hat (Margossian et al., "Nested R-hat", Bayesian Analysis 2024): superchains of M chains that start together
+NESTED_RECORD = 14                     # include/amwg.h: amwg_summary_nested, doubles per entry
+
+
+def resolve_nested(spec, superchain_size: Optional[int], first_chain: int, chains: int) -> Optional[int]:
+    """Checks the `nested=` argument of sample_summary and returns the superchain size M, or None for None / False. True takes
+    options.superchain_size (`superchain_size`, None when it was not set); an int >= 1 is M itself. Superchain k is the global
+    chains [kM, (k + 1)M), and the chains summarised, [first_chain, first_chain + chains) (all of them with options.distributed),
+    must be whole superchains. Pure: raises ValueError before any device work."""
+    if spec is None or spec is False:
+        return None
+    if spec is True:
+        if superchain_size is None:
+            raise ValueError("nested=True needs options.superchain_size")
+        M = int(superchain_size)
+    elif _is_int(spec) and spec >= 1:
+        M = int(spec)
+    else:
+        raise ValueError("nested must be None, False, True or an int superchain size >= 1, not %r" % (spec,))
+    if first_chain % M or (first_chain + chains) % M:
+        raise ValueError("nested: the chains summarised, [%d, %d), are not whole superchains of %d chains"
+                         % (first_chain, first_chain + chains, M))
+    return M
+
+
+def nested_scratch_bytes(entries: int, chains: int, first_chain: int, superchain_size: int) -> int:
+    """Device scratch of amwg_summary_nested (include/amwg.h)."""
+    up = lambda b: -(-b // 256) * 256
+    n_seg = (first_chain + chains - 1) // superchain_size - first_chain // superchain_size + 1
+    ctas = min(-(-n_seg // 256), 1184)
+    return up(16 * entries * chains) + up(32 * entries * ctas) + up(32 * entries) + up(64 * entries)
+
+
+def nested_unit(rec: np.ndarray, M: int, rows: int) -> np.ndarray:
+    """Chain-level records [..., 4] of whole superchains (M chains, mean of the chain means, M2 of the chain means, sum of the
+    within-chain M2) -> their units (1, superchain mean, 0, B~_k + W-_k) of the superchain-to-total level: B~_k = M2 / (M - 1)
+    (0 when M = 1), W-_k = sum / (M (rows - 1)) (0 when rows = 1). The arithmetic of nested_unit in csrc/amwg_nested.cuh."""
+    rec = np.asarray(rec, dtype=np.float64)
+    b = rec[..., 2] / float(M - 1) if M > 1 else np.zeros_like(rec[..., 2])
+    w = rec[..., 3] / (float(M) * float(rows - 1)) if rows > 1 else np.zeros_like(rec[..., 3])
+    return np.stack([np.ones_like(rec[..., 0]), rec[..., 1], np.zeros_like(rec[..., 0]), b + w], axis=-1)
+
+
+def merge_nested_records(records: Sequence[np.ndarray], M: int, rows: int) -> np.ndarray:
+    """Per-shard [entries, 14] records of amwg_summary_nested in rank order -> one [entries, 4] superchain-to-total record
+    (superchains, mean of the superchain means, M2 of the superchain means, sum over superchains of B~_k + W-_k). The complete
+    records merge in rank order (merge_moment_records). The cut records are grouped by superchain id and merged in rank order
+    into chain-level records, which must then hold all M chains; each becomes its unit (nested_unit) and is folded in, in the
+    order of the superchain ids."""
+    recs = [np.asarray(r, dtype=np.float64) for r in records]
+    total = merge_moment_records([r[:, :4] for r in recs])
+    cut = {}
+    for r in recs:
+        for slot in range(2):
+            part = r[:, 4 + 5 * slot:9 + 5 * slot]
+            if part[0, 0] < 0:
+                continue
+            k = int(part[0, 0])
+            cut[k] = part[:, 1:] if k not in cut else merge_moment_records([cut[k], part[:, 1:]])
+    for k in sorted(cut):
+        if not np.all(cut[k][:, 0] == M):
+            raise RuntimeError("nested: superchain %d has %d of its %d chains over all shards" % (k, int(cut[k][0, 0]), M))
+        total = merge_moment_records([total, nested_unit(cut[k], M, rows)])
+    return total
+
+
+def finalize_nested(rec: np.ndarray) -> np.ndarray:
+    """rhat_nested per entry from the merged [entries, 4] superchain-to-total record (K, mean of the superchain means, M2 of the
+    superchain means, sum over superchains of B~_k + W-_k): with B^ = M2 / (K - 1) and W^ = sum / K,
+    rhat_nested = sqrt(1 + B^ / W^). NaN when K < 2, when W^ = 0, or when any value of the record is not finite (a NaN or +-inf
+    draw of the entry)."""
+    rec = np.asarray(rec, dtype=np.float64)
+    K, mean, m2, sw = rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        B = m2 / (K - 1)
+        W = sw / K
+        rhat = np.sqrt(1.0 + B / W)
+    ok = (K >= 2) & (W > 0) & np.isfinite(mean) & np.isfinite(B) & np.isfinite(W)
+    return np.where(ok, rhat, np.nan)
+
+
+def nested_block(reducer, block, rows: int, first_chain: int, M: int, distributed: bool) -> np.ndarray:
+    """-> rhat_nested per entry over all shards; only reads the block. Each shard's record comes from reducer.nested;
+    distributed: one all_gather_into_tensor of the fixed-size records, merged on the host in rank order (merge_nested_records),
+    so every rank returns the same bits."""
+    rec = reducer.nested(block, first_chain, M)
+    if distributed:
+        import torch
+        import torch.distributed as dist
+        ws = dist.get_world_size()
+        mine = torch.from_numpy(np.ascontiguousarray(rec))
+        if block.is_cuda:
+            mine = mine.to(block.device)
+        gathered = torch.empty((ws * rec.shape[0], NESTED_RECORD), dtype=mine.dtype, device=mine.device)
+        dist.all_gather_into_tensor(gathered, mine)
+        recs = list(gathered.cpu().numpy().reshape(ws, rec.shape[0], NESTED_RECORD))
+    else:
+        recs = [rec]
+    return finalize_nested(merge_nested_records(recs, M, rows))

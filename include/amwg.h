@@ -245,9 +245,17 @@ AMWG_API int amwg_get_log_post(amwg_sampler* s, double* host_out);
  *   of its init on the unconstrained scale (uniform #(2^63 + a*n_comp + c) of the chain's Philox stream, so the draws do not
  *   depend on sharding and never meet Math.random()'s); a chain keeps its first attempt whose components are valid and whose
  *   log_post is finite. The points are then committed as by amwg_set_state. radius must be finite and > 0. If some chains find no
- *   point in 100 attempts, *n_failed (when not null) receives their number, an error is returned and the handle is unchanged. */
+ *   point in 100 attempts, *n_failed (when not null) receives their number, an error is returned and the handle is unchanged.
+ * amwg_disperse_state_superchains: the same with superchains of superchain_size consecutive global chains (superchain k holds the
+ *   chains [k superchain_size, (k + 1) superchain_size)) that start together, for nested R-hat (DESIGN.md §4.6). Global chain g
+ *   draws its attempts from the stream of its superchain's first chain, superchain_size * floor(g / superchain_size), instead of
+ *   its own, so every chain of a superchain keeps the same point, whichever handles hold them; superchain_size = 1 is
+ *   amwg_disperse_state. The sampling streams stay keyed by g. Errors, before anything on the device changes: superchain_size < 1,
+ *   and those of amwg_disperse_state. A handle holds a range of the global chains and does not know how many there are in all:
+ *   that superchain_size divides the chain count is the caller's check (the hosts' options.superchain_size). */
 AMWG_API int amwg_set_state(amwg_sampler* s, const double* host_in);
 AMWG_API int amwg_disperse_state(amwg_sampler* s, double radius, int64_t* n_failed);
+AMWG_API int amwg_disperse_state_superchains(amwg_sampler* s, double radius, int64_t superchain_size, int64_t* n_failed);
 
 /* Checkpoints (not in the reference): save the whole run state of a handle and resume it later, bit for bit, in this or another
  * process, on any sharding of the chains (DESIGN.md §2 "Checkpoints" has the image layout and the guarantee).
@@ -359,7 +367,21 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   amwg_summary_moments' (Chan, in matrix form). Device scratch, from a per-device pool grown on demand: with T = nb (nb + 1) / 2
  *   tiles, nb = ceil(n_sel / 8), R = 1 when T >= 16 else floor(16 / T) warps per tile and G = min(ceil(chains / 32), 264) CTAs,
  *   8 (n_sel chains + n_sel + 64 T R G + 128 T) bytes, each of the four parts rounded up to 256 bytes. Errors (nothing is touched): an empty block, n_sel outside 1..128, null
- *   pointers, a selected entry outside [0, entries), rows * chains >= 2^53. */
+ *   pointers, a selected entry outside [0, entries), rows * chains >= 2^53.
+ *
+ * Nested R-hat (sample_summary(..., nested=M), DESIGN.md §4.6): superchain k is the global chains [k M, (k + 1) M); the block
+ * holds the global chains [first_chain, first_chain + chains).
+ * amwg_summary_nested: host_out[entry][14]. Per chain, its mean and M2 over the rows (two sequential passes); per superchain the
+ *   shard touches, its chains' records (1, mean, 0, M2) merged in chain order into (chains, mean of the chain means, M2 of the chain
+ *   means, sum of the within-chain M2). host_out[entry][0..3] = the complete superchains, each as the unit (1, superchain mean, 0,
+ *   B~_k + W-_k) with B~_k = M2 of its chain means / (M - 1) (0 when M = 1) and W-_k = its within-chain M2 / (M (rows - 1)) (0 when
+ *   rows = 1), Chan-merged in a fixed order; then two cut records { superchain id, chains, mean of the chain means, M2 of the chain
+ *   means, sum of the within-chain M2 } for the first and the last superchain when the range cuts them (id -1 and zeros when not).
+ *   The grid depends on chains and the number of superchains touched only: two calls give the same bits. Records of shards merge
+ *   like amwg_summary_moments' (summary.merge_nested_records). Device scratch, from a per-device pool grown on demand, with S the
+ *   superchains touched and G = min(ceil(S / 256), 1184): 16 entries chains + 32 entries G + 32 entries + 64 entries bytes, each
+ *   part rounded up to 256 bytes. Errors (nothing is touched): an empty block, null pointers, superchain_size < 1,
+ *   first_chain < 0, first_chain + chains > 2^53. */
 AMWG_API int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats);
 AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t pass,
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
@@ -377,6 +399,8 @@ AMWG_API int amwg_summary_histogram2d(int device, const double* dev_samples, int
                                       const int32_t* host_pairs, int32_t n_pairs, const double* dev_edges, int32_t bins, int64_t* dev_counts);
 AMWG_API int amwg_summary_comoments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
                                     const int32_t* host_sel, int32_t n_sel, double* host_out);
+AMWG_API int amwg_summary_nested(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int64_t first_chain,
+                                 int64_t superchain_size, double* host_out);
 
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it

@@ -288,10 +288,14 @@ BINDING(set_state)
   if (amwg_set_state(h->s, x.data()) != 0) fail_from_library();
   return js_undefined(env);
 END_BINDING
-// disperse_state(handle, radius) -> chains without a starting point (0: all placed)   amwg_disperse_state
+// disperse_state(handle, radius[, superchain_size]) -> chains without a starting point (0: all placed)
+//                                                                       amwg_disperse_state, amwg_disperse_state_superchains
 BINDING(disperse_state)
   int64_t failed = 0;
-  if (amwg_disperse_state(handle_of(env, a.at(0))->s, to_double(env, a.at(1)), &failed) != 0 && failed == 0) fail_from_library();
+  amwg_sampler* s = handle_of(env, a.at(0))->s;
+  const double radius = to_double(env, a.at(1));
+  const int rc = a.n > 2 ? amwg_disperse_state_superchains(s, radius, (int64_t)to_double(env, a.at(2)), &failed) : amwg_disperse_state(s, radius, &failed);
+  if (rc != 0 && failed == 0) fail_from_library();
   return js_number(env, (double)failed);
 END_BINDING
 // model_fingerprint(descriptor) -> 16 hex digits                                amwg_model_fingerprint (no device needed)
@@ -515,6 +519,16 @@ BINDING(summary_comoments)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// summary_nested(device, samples ptr, rows, entries, chains, first_chain, superchain_size) -> Float64Array [entries][14]
+//                                                                                                            amwg_summary_nested
+BINDING(summary_nested)
+  const int32_t entries = (int32_t)to_double(env, a.at(3));
+  std::vector<double> out((size_t)(entries > 0 ? entries : 0) * 14);
+  if (amwg_summary_nested((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)), entries,
+                          (int64_t)to_double(env, a.at(4)), (int64_t)to_double(env, a.at(5)), (int64_t)to_double(env, a.at(6)), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
 // term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
 BINDING(term_cache)
   Handle* h = handle_of(env, a.at(0));
@@ -548,7 +562,7 @@ NAPI_MODULE_INIT() {
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
-      {"summary_comoments", summary_comoments},
+      {"summary_comoments", summary_comoments}, {"summary_nested", summary_nested},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {

@@ -12,7 +12,7 @@
 // New, non-reference options: `chains` (default 1: output shaped exactly like the reference's), `seed`, `device`, `first_chain`,
 // `faithful` (no factorised likelihood plates: bit-faithful sums, slower), `scope` ({name: value} for identifiers log_post uses
 // from an enclosing scope that a recording from source cannot see), `init_radius` (over-dispersed starting points drawn on the
-// device, DESIGN.md §2). New methods: `sampler.set_state(values)` places the chains anywhere; `sampler.checkpoint()` and
+// device, DESIGN.md §2), `superchain_size` (chains per superchain that start at one point, DESIGN.md §4.6). New methods: `sampler.set_state(values)` places the chains anywhere; `sampler.checkpoint()` and
 // `sampler.restore(images)` stop and resume a run bit for bit.
 (function (root, factory) {
   if (typeof define === "function" && define.amd) { define(["./amwg_trace", "./amwg_native"], factory); }
@@ -178,7 +178,7 @@
 
   // ---------------------------------------------------------------------------------------------- the device model
   function DeviceModel(params, names, log_post, data, options, resolved) {
-    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed, radius, failed;
+    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed, radius, size, failed;
     this.params = params; this.names = names; this.offsets = {};
     for (i = 0; i < names.length; i++) { this.offsets[names[i]] = n_comp; n_comp += product(params[names[i]].dim); }
     this.n_comp = n_comp;
@@ -190,6 +190,12 @@
     this.first_chain = get_option("first_chain", options, 0);
     radius = get_option("init_radius", options, null);            // over-dispersed starting points (DESIGN.md §2)
     if (radius !== null && !(typeof radius === "number" && isFinite(radius) && radius > 0)) { throw "options.init_radius must be a finite number > 0"; }
+    size = get_option("superchain_size", options, null);           // chains per superchain (nested R-hat, DESIGN.md §4.6)
+    if (size !== null) {
+      if (!(typeof size === "number" && isFinite(size) && size >= 1 && size === Math.floor(size))) { throw "options.superchain_size must be an integer >= 1"; }
+      if (this.n_chains % size !== 0) { throw "options.superchain_size must divide options.chains"; }
+    }
+    this.superchain_size = size;
     prog =tracer.trace(log_post, names, params, this.offsets, n_comp, data, {faithful: !!get_option("faithful", options, false), scope: get_option("scope", options, null),
                                                                                 base_state: get_option("base_state", options, null)});
     this.program = prog;
@@ -218,7 +224,7 @@
     }
     this.handle = native.create(desc, this.n_chains, this.first_chain, this.seed, this.device);
     if (radius !== null) {
-      failed = native.disperse_state(this.handle, radius);
+      failed = size === null ? native.disperse_state(this.handle, radius) : native.disperse_state(this.handle, radius, size);
       if (failed > 0) {
         native.destroy(this.handle);
         this.handle = null;
