@@ -706,7 +706,10 @@ class AmwgSampler(Sampler):
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
         statistics with numpy.quantile's linear rule; a long grid such as numpy.linspace(0, 1, 41) gives an equal-mass histogram and
         runs as several radix selects of 16 probabilities each). With options.distributed every rank returns the all-GPU summary
-        (two small collectives, summary.py). Advances the chains exactly as sample(n) does.
+        (two small collectives, summary.py). Advances the chains exactly as sample(n) does. A NaN or +-inf draw (a derived quantity
+        such as Math.log(mu) or 1/x) is summarised as numpy summarises it: a NaN draw makes the entry's mean and every quantile NaN;
+        +inf draws alone make the mean +inf, -inf draws alone -inf, both NaN; sd and rhat are NaN. Only an entry whose finite
+        draws overflow the sum can differ from numpy.mean (summary.nonfinite_as_numpy).
         diagnostics=True adds, per parameter and shaped like "mean": "ess_mean" and "ess_tail" (split-chain effective sample
         sizes of the draws and of the 5 % / 95 % tail indicators, Vehtari et al. 2021), "mcse_mean" (sd / sqrt(ess_mean)) and
         "rhat_split" (split-chain R-hat, not rank-normalised); the other keys keep their values bit for bit. Fewer than 10 kept

@@ -540,7 +540,9 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
     the collectives run on the tensors it returns (NCCL for CUDA tensors, gloo for the CPU stand-in used in the tests).
     diagnostics=True appends (split_chain_diagnostics' dict, lag windows used): the select also forms the minimum, q05, q95 and
     the maximum (each quantile is its own order statistics, so the requested ones are unchanged). diagnostics="rank" also forms
-    the median and adds rank_diagnostics' "ess_bulk" and "rhat_rank" to that dict; every other value is the same bits."""
+    the median and adds rank_diagnostics' "ess_bulk" and "rhat_rank" to that dict; every other value is the same bits. The mean
+    and the returned quantiles of an entry with NaN or infinite draws are numpy's (nonfinite_as_numpy); the internal order
+    statistics that feed the diagnostics keep their bits."""
     import torch
     check_diagnostics(diagnostics)
     entries = block.shape[1]
@@ -566,27 +568,64 @@ def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequenc
     for first in range(0, len(probs), per_select):            # long probability grids (equal-mass histograms): several selects
         chunk = probs[first:first + per_select]
         ranks, plan = quantile_targets(rows * total_chains, chunk)
-        sel = RadixSelect(entries, ranks)
-        for npass in range(8):
-            table, which = sel.prefixes()
-            counts = reducer.digit_counts(block, npass, table)
-            if distributed:
-                import torch.distributed as dist
-                dist.all_reduce(counts)                       # integer sums: exact, independent of the number of GPUs
-            sel.advance(counts.cpu().numpy(), which)
+        sel = _select(reducer, block, ranks, distributed)
         vals = sel.values()                                   # [entries, T]
         for i, (lo, hi, g) in enumerate(plan):
             q[first + i] = _lerp(vals[:, lo], vals[:, hi], g)
             low[first + i] = vals[:, lo]
+    mean, q_user = nonfinite_as_numpy(reducer, block, mean, q[:len(user_probs)], rows * total_chains, distributed)
     if not diagnostics:
-        return mean, sd, rhat, q
+        return mean, sd, rhat, q_user
     vmin, q05, q95, vmax = q[len(user_probs):len(user_probs) + len(DIAGNOSTIC_PROBS)]
     diag = split_chain_diagnostics(reducer, block, rows, sd, q05, q95, vmin, vmax, distributed)
     if diagnostics == "rank":
         # the exact minimum and maximum: interpolating an infinite extreme with itself gives NaN, and these must tell +-inf from NaN
         lo_min, lo_max = low[len(user_probs)], low[len(user_probs) + 3]
         diag[0].update(rank_diagnostics(reducer, block, rows, q[-1], lo_min, lo_max, distributed))
-    return mean, sd, rhat, q[:len(user_probs)], diag
+    return mean, sd, rhat, q_user, diag
+
+
+def _select(reducer, block, ranks: np.ndarray, distributed: bool) -> RadixSelect:
+    """The 8 passes of the radix select of the sorted 0-based `ranks` over all shards; -> the finished RadixSelect."""
+    sel = RadixSelect(block.shape[1], ranks)
+    for npass in range(8):
+        table, which = sel.prefixes()
+        counts = reducer.digit_counts(block, npass, table)
+        if distributed:
+            import torch.distributed as dist
+            dist.all_reduce(counts)                           # integer sums: exact, independent of the number of GPUs
+        sel.advance(counts.cpu().numpy(), which)
+    return sel
+
+
+_KEY_NEG_INF, _KEY_POS_INF = double_to_key(np.array([-np.inf, np.inf]))
+
+
+def nonfinite_as_numpy(reducer, block, mean: np.ndarray, q_user: np.ndarray, M: int, distributed: bool):
+    """-> (mean, quantiles) with the entries that hold NaN or infinite draws summarised as numpy.mean / numpy.quantile
+    summarise them; M: the draws per entry over all shards. The merged mean of such an entry is not finite, but not always
+    numpy's: once a record's mean is +inf, the Chan merge with a finite record forms inf + (x - inf) w = NaN. And the select
+    orders NaN by its sign bit (below -inf or above +inf), so only one end of an entry with a NaN draw comes out NaN.
+    So when some mean is not finite, one more radix select finds the smallest and the largest key of every entry (ranks 0 and
+    M - 1; distributed: its counts are all-reduced like the quantiles', and every rank takes this branch because the merged mean
+    is the same on all of them). The key order puts every NaN outside [-inf, +inf], so an entry holds a NaN exactly when one of
+    its extreme keys lies outside, and otherwise holds -inf (+inf) exactly when its smallest (largest) draw is -inf (+inf).
+    An entry with a NaN draw gets mean NaN and NaN at every probability; +inf and -inf both: mean NaN; +inf only: mean +inf;
+    -inf only: mean -inf. sd and R-hat of all of these are NaN already, and so are their quantiles where numpy.quantile's
+    interpolation meets an infinity. An entry with finite draws only whose sum overflowed keeps its merged mean (numpy may differ
+    there). When every mean is finite nothing runs and nothing changes."""
+    if np.all(np.isfinite(mean)):
+        return mean, q_user
+    keys = _select(reducer, block, np.unique([0, M - 1]), distributed).prefix
+    kmin, kmax = keys[:, 0], keys[:, -1]
+    nan = (kmin < _KEY_NEG_INF) | (kmax > _KEY_POS_INF)
+    mean, q_user = mean.copy(), q_user.copy()
+    mean[(kmin == _KEY_NEG_INF) & (kmax == _KEY_POS_INF)] = np.nan
+    mean[(kmax == _KEY_POS_INF) & (kmin != _KEY_NEG_INF)] = np.inf
+    mean[(kmin == _KEY_NEG_INF) & (kmax != _KEY_POS_INF)] = -np.inf
+    mean[nan] = np.nan
+    q_user[:, nan] = np.nan
+    return mean, q_user
 
 
 # ---------------------------------------------------------------------------------------------------------------------

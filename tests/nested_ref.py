@@ -29,10 +29,11 @@ def gamma(k) -> float:
     return k * U / (1.0 - k * U)
 
 
-def _chan_bound(means, e_v, m2_leaf, m2_err, sw_leaf, sw_err):
-    """Bounds (mean, M2, sum_w) of the Chan merge of len(means) records, as derived in the module docstring."""
+def _chan_bound(means, e_v, m2_leaf, m2_err, sw_leaf, sw_err, steps=None):
+    """Bounds (mean, M2, sum_w) of the Chan merge of len(means) records, as derived in the module docstring; `steps`: the most
+    merge steps a mean passes through, when fewer than L = n + 20 are known."""
     n = len(means)
-    L = n + 20
+    L = n + 20 if steps is None else steps
     A = float(np.max(np.abs(means)))
     D = float(np.max(means) - np.min(means))
     E = float(np.max(e_v)) + 3 * L * gamma(4) * A

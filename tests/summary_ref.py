@@ -34,6 +34,31 @@ class NumpyBlockReducer:
         return torch.from_numpy(counts)
 
 
+class ChanBlockReducer(NumpyBlockReducer):
+    """NumpyBlockReducer whose moments merge per-chain records (1, chain mean, 0, within-chain M2) in a fixed binary tree with
+    the Chan merge of the device (merge_moment_records), as amwg_summary_moments' CTA tree does: a chain whose mean is +inf
+    merged with a finite one gives the mean NaN there too, where numpy.mean gives +inf."""
+
+    def moments(self, block):
+        from bayes_js_b200.summary import merge_moment_records
+        x = block.numpy()
+        rows, entries, chains = x.shape
+        m = x.sum(axis=0) / rows
+        with np.errstate(invalid="ignore"):
+            m2 = ((x - m[None]) ** 2).sum(axis=0)
+        w = 1
+        while w < chains:
+            w *= 2
+        rec = np.zeros((w, entries, 4))
+        rec[:chains, :, 0] = 1.0
+        rec[:chains, :, 1] = m.T
+        rec[:chains, :, 3] = m2.T
+        while w > 1:                                         # sh[t] = merge(sh[t], sh[t + w]) for t < w, w halving
+            w //= 2
+            rec[:w] = merge_moment_records([rec[:w].reshape(-1, 4), rec[w:2 * w].reshape(-1, 4)]).reshape(w, entries, 4)
+        return rec[0]
+
+
 def numpy_summary(x, probs):
     """x [rows, entries, chains] -> (mean, sd, rhat, quantiles) straight from numpy, as a user of sample() would compute them."""
     rows, entries, chains = x.shape
