@@ -1548,8 +1548,12 @@ static void try_jit(amwg_sampler* s, const amwg_model* md) {
   cudaDeviceProp prop{};
   if (cudaGetDeviceProperties(&prop, s->device) != cudaSuccess) { s->jit_note = "cudaGetDeviceProperties failed"; cudaGetLastError(); return; }
   jit::Source src;
+  // the model as this handle steps it: with AMWG_TERM_CACHE=0 (or AMWG_STAT_SWEEP=0) amwg_create dropped the term cache and every
+  // step runs the full program, which is what the full-program specialisation does
+  amwg_model stepped = *md;
+  if (s->m.n_terms == 0) stepped.n_terms = 0;
   std::string why = stat_model ? jit::build_source(md, consts, s->a.C, prop.multiProcessorCount, c0, src)
-                               : jit::build_source_full(md, consts, s->a.C, prop.multiProcessorCount, c0, src);
+                               : jit::build_source_full(&stepped, consts, s->a.C, prop.multiProcessorCount, c0, src);
   if (!why.empty()) { s->jit_note = "not specialised: " + why; return; }
   if (src.plan.smem_bytes > (unsigned)prop.sharedMemPerBlockOptin) { s->jit_note = "not specialised: shared-memory plan does not fit"; return; }
   const unsigned long long key = jit::fnv1a(src.generated, jit::fnv1a(src.prelude));

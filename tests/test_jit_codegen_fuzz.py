@@ -6,6 +6,8 @@ binary / vector parameters -- lowers it with the product's tracer, specialises i
 the host and compares jit_logpost() / jit_derived() with the bytecode run on the oracle's arithmetic at random states, bit for bit.
 Half of the models are lowered as with AMWG_TERM_CACHE=0 (every step runs the full program); of the others, those the generator
 turns down (they step with a term cache) are counted, not failed."""
+import os
+
 import numpy as np
 import pytest
 
@@ -426,3 +428,78 @@ def test_statistics_sweep_bounded_block_derived_thinning_and_acceptance_counts(p
     assert np.array_equal(hs.acc[:, same], hf.acc[:, same]) and hs.acc[1::2].sum() > 0 and hs.acc[0::2].sum() == 0
     # the bounds bind: some proposals were refused without a uniform, so the chains consumed different numbers of Math.random() calls
     assert np.unique(rng_s).size > 4 and out_s[:, :J, :].min() >= 8.5 and out_s[:, :J, :].max() <= 11.5
+
+
+# ---- the seeds tests/test_gpu_fuzz.py runs on the device: each one is cleared here first, on the emulated kernels it reaches there, under
+#      the strict shim (bulk copies, mbarrier accounting, declared shared memory, device-shaped columns) and, in a subprocess, ASan -------
+GPU_SEEDS = (("generic", 3), ("generic", 7), ("stat", 4), ("stat", 51), ("shapes", 2), ("shapes", 7))
+
+
+def gpu_model(pkg, kind, seed):
+    """(params, log_post, data) of one of the builders above"""
+    if kind == "generic":
+        return _build(pkg, seed)
+    if kind == "stat":
+        return _build_stat(pkg, seed)
+    params, log_post = _build_shapes(pkg, seed)
+    return params, log_post, None
+
+
+@pytest.mark.parametrize("kind,seed", GPU_SEEDS)
+def test_gpu_fuzz_seeds_on_the_emulated_kernels(pkg, orc, tmp_path, kind, seed):
+    """The full-program sweep of the faithful lowering (what AMWG_JIT=1 runs for a faithful handle, with AMWG_TERM_CACHE=0 where that
+    lowering keeps a term cache) against the oracle stepping the same program, bit for bit, with the stream positions; for a model the
+    tracer gives the statistics lowering, also the statistics sweep against that full-program sweep (one chain in sixteen may differ)."""
+    import prog_eval
+    from test_jit_codegen_semantics import HostKernel, HostStatKernel
+    params, log_post, data = gpu_model(pkg, kind, seed)
+    (tmp_path / "full").mkdir()
+    hk = HostKernel(pkg, orc, tmp_path / "full", params, log_post, data, faithful=True, _force_full=True)
+    chains, first, sd, sweeps = 4, 30 + seed, 11 + seed, 25
+    hk.start(chains, first, sd)
+    out = hk.sweeps(sweeps)
+    prog, consts, O = hk.prog, hk.consts, hk.O
+    for c in range(chains):
+        o = orc.OracleSampler(lambda st: prog_eval.logpost(prog, consts, st, O), None, params, seed=sd, chain=first + c)
+        refd = o.sample(sweeps)
+        e = 0
+        for name in hk.s.params:
+            n = int(np.prod(hk.s.params[name]["dim"]))
+            want = np.asarray(refd[name], np.float64).reshape(sweeps, n)
+            assert np.array_equal(out[:, e:e + n, c].view(np.uint64), want.view(np.uint64)), (kind, seed, name, c)
+            e += n
+        assert int(hk.rng_n[c]) == o.rng_position()
+    if kind == "stat":
+        probe = pkg.mcmc.AmwgSampler(params, log_post, data, {"chains": 4096, "_model_only": True})
+        assert probe._program.stat_prog >= 0
+        hs = HostStatKernel(pkg, orc, tmp_path, params, log_post, data)
+        out_s, rng_s = hs.run(16, first, sd, sweeps, thin=2)
+        hk.start(16, first, sd)
+        out_f = hk.sweeps(sweeps, thin=2)
+        same = (out_s.view(np.uint64) == out_f.view(np.uint64)).all(axis=(0, 1))
+        assert same.mean() >= 15 / 16, same.mean()
+        assert np.array_equal(rng_s[same], hk.rng_n[same])
+
+
+def test_gpu_fuzz_seeds_under_address_sanitizer(tmp_path):
+    """The cleared seeds again, every emulated kernel built with -fsanitize=address, in a pytest subprocess with g++'s libasan preloaded
+    (the test process itself cannot load an instrumented library). Any heap overflow, use after free or misaligned access ends that
+    run with a report under `log_path`."""
+    import subprocess
+    import sys
+    lib = subprocess.run(["g++", "-print-file-name=libasan.so"], capture_output=True, text=True).stdout.strip()
+    if not os.path.isabs(lib) or not os.path.exists(lib):
+        pytest.skip("g++ has no libasan.so here")
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    log = tmp_path / "asan"
+    env = dict(os.environ, LD_PRELOAD=lib, ASAN_OPTIONS=f"detect_leaks=0:log_path={log}", AMWG_HOST_SANITIZE="address",
+               PYTHONDONTWRITEBYTECODE="1")
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [
+        "-m", "pytest", "-q", "-p", "no:cacheprovider", f"--basetemp={tmp_path / 'run'}",
+        os.path.join(root, "tests", "test_jit_codegen_fuzz.py"), "-k", "test_gpu_fuzz_seeds_on_the_emulated_kernels"]
+    r = subprocess.run(cmd, cwd=root, env=env, capture_output=True, text=True, timeout=1800)
+    reports = sorted(tmp_path.glob("asan*"))
+    text = "".join(p.read_text(errors="replace")[:6000] for p in reports)
+    assert not reports, text
+    assert r.returncode == 0, (r.stdout[-4000:], r.stderr[-4000:])
+    assert f"{len(GPU_SEEDS)} passed" in r.stdout, r.stdout[-2000:]

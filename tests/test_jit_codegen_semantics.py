@@ -11,6 +11,7 @@ Constants that the library folds on the device at create (log(2*pi), lbeta(2,2) 
 arithmetic and written into the model descriptor before the generator sees it, exactly what try_jit() reads back from the device."""
 import ctypes as C
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -26,11 +27,28 @@ CSRC = os.path.join(ROOT, "bayes.js_b200", "csrc")
 HOST_PRELUDE = r'''
 #include "cuda_runtime.h"      // tests/host_shim
 #include "math_constants.h"
+#include <cstdarg>
+#include <cstdio>
 #define __constant__
 static unsigned char* g_smem_base = nullptr;                    // "shared memory": a host buffer, addressed by offset
+static unsigned g_smem_limit = 0;                               // its size: every load must lie below it
+static char g_fault[2048];                                      // the first breach of the device's rules; the harness reads it after each call
+static void hs_fault(const char* fmt, ...) {
+  if (g_fault[0]) return;
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(g_fault, sizeof g_fault, fmt, ap);
+  va_end(ap);
+}
 namespace amwg {
 static inline unsigned smem_u32(const void* p) { return (unsigned)((const unsigned char*)p - g_smem_base); }
-static inline double lds_f64_sa(unsigned a) { double v; std::memcpy(&v, g_smem_base + a, 8); return v; }
+// an n-byte ld.shared at offset a: aligned to n (a misaligned one faults on the device) and inside the CTA's shared memory
+static inline bool lds_ok(unsigned a, unsigned n) {
+  if (a % n) { hs_fault("misaligned %u-byte shared-memory load at offset %u", n, a); return false; }
+  if ((unsigned long long)a + n > g_smem_limit) { hs_fault("%u-byte shared-memory load at offset %u, past the %u bytes declared", n, a, g_smem_limit); return false; }
+  return true;
+}
+static inline double lds_f64_sa(unsigned a) { double v = 0.0; if (lds_ok(a, 8)) std::memcpy(&v, g_smem_base + a, 8); return v; }
 }
 #include "amwg_math.cuh"
 #include "amwg_ld.cuh"
@@ -38,7 +56,8 @@ static inline double lds_f64_sa(unsigned a) { double v; std::memcpy(&v, g_smem_b
 
 HOST_EXPORTS = r'''
 extern "C" {
-void hs_set_smem(unsigned char* p) { g_smem_base = p; }
+void hs_set_smem(unsigned char* p, unsigned n) { g_smem_base = p; g_smem_limit = n; }
+const char* hs_fault_msg() { return g_fault; }
 int hs_n_res() { return JN_RES; }
 unsigned hs_res_off(int k) { return amwg::JRES_OFF[k]; }
 int hs_res_col(int k) { return amwg::JRES_COL[k]; }
@@ -56,6 +75,18 @@ void hs_derived(const double* state, double* der) {
 }
 }
 '''
+
+
+def _compile(cpp, so):
+    """g++ for the host. AMWG_HOST_SANITIZE=address builds with AddressSanitizer (the process must then preload libasan: see
+    test_jit_codegen_fuzz.py's ASan run)."""
+    extra = ["-fsanitize=address", "-fno-omit-frame-pointer", "-g"] if os.environ.get("AMWG_HOST_SANITIZE") == "address" else []
+    r = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-w", *extra, "-I" + os.path.join(ROOT, "tests", "host_shim"),
+                        "-I" + CSRC, str(cpp), "-o", str(so)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-4000:]
+    lib = C.CDLL(str(so))
+    lib.hs_fault_msg.restype = C.c_char_p
+    return lib
 
 
 def _skeleton_helpers():
@@ -82,15 +113,12 @@ class HostProgram:
         rc, msg, src = s.jit_compile_check()
         assert rc == 0, msg
         assert "#define JFULL 1" in src
+        self.src, self.msg = src, msg
         cpp = tmp_path / "gen.cpp"
         # the generated text = the #define prelude (up to the first namespace block), then tables and programs
         cut = src.index("namespace amwg {")
         cpp.write_text(src[:cut] + HOST_PRELUDE + _skeleton_helpers() + src[cut:] + HOST_EXPORTS)
-        so = tmp_path / "gen.so"
-        r = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-I" + os.path.join(ROOT, "tests", "host_shim"),
-                            "-I" + CSRC, str(cpp), "-o", str(so)], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        self.lib = L = C.CDLL(str(so))
+        self.lib = L = _compile(cpp, tmp_path / "gen.so")
         L.hs_logpost.restype, L.hs_logpost.argtypes = C.c_double, [C.POINTER(C.c_double), C.c_int, C.c_double]
         L.hs_derived.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double)]
         for f in ("hs_res_off", "hs_bern_data", "hs_bern_mask"):
@@ -110,7 +138,7 @@ class HostProgram:
                     words[i >> 5] |= np.uint32(1 << (i & 31))
             words[-1] = 1 if np.any(~((y == 1.0) | (y == 0.0))) else 0
             self.smem[m0:m0 + 4 * words.size] = words.view(np.uint8)
-        L.hs_set_smem(self.smem.ctypes.data_as(C.POINTER(C.c_ubyte)))
+        L.hs_set_smem(self.smem.ctypes.data_as(C.POINTER(C.c_ubyte)), self.smem.size)
         self.D = self.prog.n_comp if hasattr(self.prog, "n_comp") else int(m.n_comp)
         self.types = []                                             # per component: (type, lower, upper)
         for p in range(m.n_params):
@@ -153,6 +181,7 @@ class HostProgram:
                     pc = self.prog.variant_derived[v]
                 prog_eval.run(self.prog, self.consts, st, pc, self.O, der=ref)
                 assert [np.float64(x).view(np.uint64) for x in der] == [np.float64(x).view(np.uint64) for x in ref]
+        assert not self.lib.hs_fault_msg(), self.lib.hs_fault_msg().decode()
 
 
 def _cases(pkg):
@@ -195,6 +224,9 @@ def test_generated_log_post_equals_the_program(pkg, orc, tmp_path, name):
 
 # ---- the whole specialised kernel on the host: skeleton + generated code, one emulated thread per CTA -----------------------------
 KERNEL_SHIM = r'''
+#include <cstdlib>
+#include <map>
+#include <vector>
 #define __global__
 #define __launch_bounds__(...)
 #define __grid_constant__
@@ -204,17 +236,108 @@ struct hs_dim3 { unsigned x = 0, y = 0, z = 0; };
 static hs_dim3 threadIdx, blockIdx, blockDim;
 static inline void __syncthreads() {}
 namespace amwg {
-alignas(16) unsigned char smem[1 << 18];                         // the CTA's dynamic shared memory (`extern __shared__ ... smem[]` in the kernel)
-static inline void mbar_init(unsigned long long*, unsigned) {}
-static inline void mbar_expect_tx(unsigned long long*, unsigned) {}
-static inline void mbar_wait(unsigned long long*, unsigned) {}
-static inline void tma_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long*) { std::memcpy(dst, src, bytes); }
+// The CTA's dynamic shared memory (`extern __shared__ ... smem[]` in the kernel): exactly the bytes the launch declares, allocated
+// on its own so that AddressSanitizer bounds it too, and filled with 0xff (NaN) before every CTA: the device hands no CTA another
+// one's contents. `hs_presets` are what the harness writes in place of code the host cannot run (the ballot loop).
+static unsigned char* smem = nullptr;
+static unsigned smem_bytes = 0;
+static std::vector<std::pair<unsigned, std::vector<unsigned char>>> hs_presets;
+// The device allocations a bulk copy may read: the data columns, laid out as amwg_create's dev_upload lays them out.
+struct HsAlloc { const unsigned char* p; unsigned long long n; };
+static std::vector<HsAlloc> hs_allocs;
+// One mbarrier: arrivals still pending in its current phase, transaction bytes announced (expect_tx) and delivered (bulk copies).
+struct HsBar { unsigned count, pending, phase; unsigned long long expect, delivered; };
+static std::map<const void*, HsBar> hs_bars;
+
+static HsBar* hs_bar(const unsigned long long* bar, const char* what) {
+  auto it = hs_bars.find(bar);
+  if (it == hs_bars.end()) { hs_fault("%s on an mbarrier that was never initialised", what); return nullptr; }
+  return &it->second;
+}
+static inline void mbar_init(unsigned long long* bar, unsigned count) { hs_bars[bar] = HsBar{count, count, 0u, 0ull, 0ull}; }
+static inline void mbar_expect_tx(unsigned long long* bar, unsigned bytes) {        // mbarrier.arrive.expect_tx: one arrival + bytes
+  HsBar* b = hs_bar(bar, "mbar_expect_tx");
+  if (!b) return;
+  if (b->pending == 0) { hs_fault("mbar_expect_tx: an arrival on an mbarrier whose %u arrival(s) of this phase have all happened", b->count); return; }
+  b->pending -= 1;
+  b->expect += bytes;
+  if (b->expect > 0xfffffull) hs_fault("mbar_expect_tx: %llu transaction bytes in one phase, beyond the 2^20 - 1 an mbarrier counts", b->expect);
+}
+static inline void mbar_wait(unsigned long long* bar, unsigned parity) {
+  HsBar* b = hs_bar(bar, "mbar_wait");
+  if (!b) return;
+  if (parity != b->phase)
+    hs_fault("mbar_wait on parity %u while the mbarrier is in phase %u: on the device the wait returns before the data lands", parity, b->phase);
+  else if (b->pending != 0 || b->delivered != b->expect)
+    hs_fault("mbar_wait would hang on the device: %llu transaction bytes expected, %llu delivered, %u arrival(s) pending",
+             b->expect, b->delivered, b->pending);
+  b->phase ^= 1u;                                                 // the phase completes: one thread per CTA has nobody to wait for
+  b->pending = b->count;
+  b->expect = b->delivered = 0;
+}
+static inline void tma_bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* bar) {      // cp.async.bulk global -> shared
+  const uintptr_t d = (uintptr_t)dst, s = (uintptr_t)src, lo = (uintptr_t)smem;
+  const long long doff = (long long)(d - lo);
+  HsBar* b = hs_bar(bar, "tma_bulk_g2s");
+  if (!b) return;
+  if (s % 16 || d % 16) { hs_fault("tma_bulk_g2s: %u bytes from %p to shared offset %lld: source and destination must be 16-byte aligned", bytes, src, doff); return; }
+  if (bytes == 0 || bytes % 16) { hs_fault("tma_bulk_g2s: %u bytes to shared offset %lld: the size must be a positive multiple of 16", bytes, doff); return; }
+  if (d < lo || d + bytes > lo + smem_bytes) {
+    hs_fault("tma_bulk_g2s: %u bytes to shared offset %lld, outside the %u bytes of dynamic shared memory the launch declares", bytes, doff, smem_bytes);
+    return;
+  }
+  const HsAlloc* a = nullptr;
+  for (const HsAlloc& x : hs_allocs) if (s >= (uintptr_t)x.p && s < (uintptr_t)x.p + x.n) a = &x;
+  if (!a) { hs_fault("tma_bulk_g2s: %u bytes from %p, which lies in no device allocation", bytes, src); return; }
+  if (s + bytes > (uintptr_t)a->p + a->n) {
+    hs_fault("tma_bulk_g2s: %u bytes from %llu bytes into a %llu-byte device allocation: the copy runs past its end", bytes,
+             (unsigned long long)(s - (uintptr_t)a->p), a->n);
+    return;
+  }
+  std::memcpy(dst, src, bytes);
+  b->delivered += bytes;
+}
 }
 '''
 
-KERNEL_EXPORTS = r'''
+# What both kernels' exports share: the declared shared memory, the device allocations, the first fault, and the shim's own functions
+# (test_the_strict_shim_refuses_* calls them directly).
+CONTRACT_EXPORTS = r'''
 extern "C" {
+void hs_set_dyn_smem(unsigned bytes) {
+  std::free(amwg::smem);
+  void* p = nullptr;
+  if (posix_memalign(&p, 16, bytes ? bytes : 1) != 0) std::abort();
+  amwg::smem = (unsigned char*)p;
+  amwg::smem_bytes = bytes;
+  std::memset(amwg::smem, 0xff, bytes);
+  amwg::hs_presets.clear();
+  g_smem_base = amwg::smem; g_smem_limit = bytes;
+}
 unsigned char* hs_kernel_smem() { return amwg::smem; }
+void hs_preset(unsigned off, const unsigned char* p, unsigned n) { amwg::hs_presets.emplace_back(off, std::vector<unsigned char>(p, p + n)); }
+void hs_clear_allocs() { amwg::hs_allocs.clear(); }
+void hs_register_alloc(const void* p, unsigned long long n) { amwg::hs_allocs.push_back(amwg::HsAlloc{(const unsigned char*)p, n}); }
+const char* hs_fault_msg() { return g_fault; }
+void hs_clear_fault() { g_fault[0] = 0; }
+void hs_mbar_init(unsigned long long* bar, unsigned count) { amwg::mbar_init(bar, count); }
+void hs_mbar_expect_tx(unsigned long long* bar, unsigned bytes) { amwg::mbar_expect_tx(bar, bytes); }
+void hs_mbar_wait(unsigned long long* bar, unsigned parity) { amwg::mbar_wait(bar, parity); }
+void hs_tma_bulk_g2s(unsigned long long dst_off, const void* src, unsigned bytes, unsigned long long* bar) {
+  amwg::tma_bulk_g2s(amwg::smem + dst_off, src, bytes, bar);
+}
+}
+// a fresh CTA: nothing in its shared memory but what the harness presets
+static void hs_cta_begin(unsigned x) {
+  std::memset(amwg::smem, 0xff, amwg::smem_bytes);
+  for (const auto& pr : amwg::hs_presets) std::memcpy(amwg::smem + pr.first, pr.second.data(), pr.second.size());
+  g_smem_base = amwg::smem; g_smem_limit = amwg::smem_bytes;
+  blockDim.x = 1; threadIdx.x = 0; blockIdx.x = x;
+}
+'''
+
+KERNEL_EXPORTS = CONTRACT_EXPORTS + r'''
+extern "C" {
 double hs_exp_of(double x) { return amwg::js_exp(x); }
 void hs_sweep(double* state, double* psd, int* acc, double* curr_lp, unsigned long long* perm, unsigned long long* rng_n,
               unsigned long long C, unsigned long long first_chain, unsigned long long seed, long long n_sweeps, long long sample_i0,
@@ -228,12 +351,60 @@ void hs_sweep(double* state, double* psd, int* acc, double* curr_lp, unsigned lo
   A.sa.monitor = monitor; A.sa.out = out;
   for (int k = 0; k < n_cols; ++k) A.col[k] = cols[k];
   A.adapting = adapting;
-  g_smem_base = amwg::smem;
-  blockDim.x = 1; threadIdx.x = 0;
-  for (unsigned long long c = 0; c < C; ++c) { blockIdx.x = (unsigned)c; amwg::amwg_jit_sweep(A); }   // one thread per CTA: chain = blockIdx.x
+  for (unsigned long long c = 0; c < C && !g_fault[0]; ++c) { hs_cta_begin((unsigned)c); amwg::amwg_jit_sweep(A); }   // one thread per CTA: chain = blockIdx.x
 }
 }
 '''
+
+
+def _smem_bytes(msg):
+    """the dynamic shared memory a launch of the compiled specialisation declares (amwg_jit_compile_check's message)"""
+    m = re.search(r"(\d+) B shared memory", msg)
+    assert m, msg
+    return int(m.group(1))
+
+
+def device_columns(columns):
+    """the model's data columns as amwg_create uploads them (dev_upload): 16-byte aligned, zero-padded to a multiple of 16 bytes and
+    to at least 16"""
+    out = []
+    for c in columns:
+        v = np.asarray(c, dtype=np.float64).ravel()
+        n = max(2 * ((v.size + 1) // 2), 2)
+        raw = np.zeros(n + 1)
+        a = raw[(-raw.ctypes.data % 16) // 8:][:n]
+        a[:v.size] = v
+        out.append(a)
+    return out
+
+
+class StrictShim:
+    """What the kernel harnesses share: the kernel `K` compiled with the strict shim, the dynamic shared memory its launch declares,
+    its device columns, and the check after every launch, which fails with the kernel's staging tables when the shim saw a breach."""
+
+    def _shim_setup(self, K, src, msg):
+        K.hs_kernel_smem.restype = C.POINTER(C.c_ubyte)
+        K.hs_register_alloc.argtypes = [C.c_void_p, C.c_ulonglong]
+        K.hs_preset.argtypes = [C.c_uint, C.c_void_p, C.c_uint]
+        self.K, self.src, self.smem_bytes = K, src, _smem_bytes(msg)
+        K.hs_set_dyn_smem(self.smem_bytes)
+
+    def _upload(self, columns):
+        cols = device_columns(columns)
+        self.K.hs_clear_allocs()
+        for c in cols:
+            self.K.hs_register_alloc(c.ctypes.data, c.nbytes)
+        colp = (C.POINTER(C.c_double) * max(len(cols), 1))(*[c.ctypes.data_as(C.POINTER(C.c_double)) for c in cols])
+        return cols, colp
+
+    def _contract(self, cols):
+        msg = self.K.hs_fault_msg()
+        if msg:
+            tables = [ln for ln in self.src.splitlines()
+                      if re.match(r"#define (JN_RES|JRES_TOTAL_BYTES|JSTREAM|JS_COL|JS_BEGIN|JS_TOTAL|JRING_\w+|JWS_\w+|JTHREADS|JN_BERN)\b", ln)
+                      or re.search(r"\b(JRES|JBERN)_\w+\[", ln)]
+            raise AssertionError(f"{msg.decode()}\n  declared dynamic shared memory: {self.smem_bytes} B; device columns: "
+                                 f"{[c.nbytes for c in cols]} B\n  " + "\n  ".join(tables))
 
 
 def _tma_structs():
@@ -245,48 +416,47 @@ def _tma_structs():
 
 def _kernel_text(generated):
     """csrc/amwg_jit_full_kernel.cuh as the host compiles it: the generated header spliced in where it is included, the one PTX fence
-    dropped (no mbarrier on the host), and the Bernoulli bit masks taken as given (the test builds them; the kernel's builder is a
+    dropped (the shim's mbarriers need none), the dynamic shared memory declaration dropped (the shim's `smem` of the declared size
+    stands for it), and the Bernoulli bit masks taken as given (the test builds them; the kernel's builder is a
     warp-wide ballot, and the host runs one thread per CTA)."""
     text = open(os.path.join(CSRC, "amwg_jit_full_kernel.cuh")).read()
     lines = []
-    n_asm = 0
+    n_asm = n_smem = 0
     for ln in text.splitlines():
         if "asm volatile(" in ln:
             assert "fence.mbarrier_init" in ln, ln
             n_asm += 1
             continue
+        if "extern __shared__" in ln:
+            assert ln.strip() == "extern __shared__ __align__(16) unsigned char smem[];", ln
+            n_smem += 1
+            continue
         lines.append(ln)
-    assert n_asm == 1
+    assert n_asm == 1 and n_smem == 1
     text = "\n".join(lines)
     inc = '#include "amwg_jit_generated.inc"'
     assert text.count(inc) == 1
     return text.replace(inc, generated + "\n#undef JN_BERN\n#define JN_BERN 0\n").replace("#pragma once", "")
 
 
-class HostKernel(HostProgram):
+class HostKernel(HostProgram, StrictShim):
     def __init__(self, pkg, orc, tmp_path, params, log_post, data, _opts=None, **opts):
         self._tmp = tmp_path
         super().__init__(pkg, orc, tmp_path, params, log_post, data, _opts=_opts, **opts)
         s = self.s
         m = s._model_keepalive[-1]
-        rc, msg, src = s.jit_compile_check()
-        assert rc == 0, msg
+        src = self.src
         cut = src.index("namespace amwg {")
         cpp = tmp_path / "kernel.cpp"
         cpp.write_text(src[:cut] + HOST_PRELUDE + KERNEL_SHIM + _tma_structs() + _kernel_text(src[cut:]) + KERNEL_EXPORTS)
-        so = tmp_path / "kernel.so"
-        r = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-I" + os.path.join(ROOT, "tests", "host_shim"),
-                            "-I" + CSRC, str(cpp), "-o", str(so)], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        self.K = K = C.CDLL(str(so))
-        K.hs_kernel_smem.restype = C.POINTER(C.c_ubyte)
+        K = _compile(cpp, tmp_path / "kernel.so")
+        self._shim_setup(K, src, self.msg)
         K.hs_exp_of.restype, K.hs_exp_of.argtypes = C.c_double, [C.c_double]
         # the masks the kernel's ballot loop would build: copied from the evaluation harness's staging buffer
-        ks = np.ctypeslib.as_array(K.hs_kernel_smem(), shape=(1 << 18,))
         for k in range(self.lib.hs_n_bern()):
             n, m0 = self.lib.hs_bern_n(k), self.lib.hs_bern_mask(k)
             nb = 4 * ((n + 31) // 32 + 1)
-            ks[m0:m0 + nb] = self.smem[m0:m0 + nb]
+            K.hs_preset(m0, self.smem[m0:m0 + nb].ctypes.data, nb)
         self.init = np.array([m.init[c] for c in range(self.D)], dtype=np.float64)
         self.n_params = int(m.n_params)
 
@@ -301,8 +471,7 @@ class HostKernel(HostProgram):
         self.curr = np.full(Cn, lp0)
         self.perm = np.full(Cn, sum(p << (4 * p) for p in range(self.n_params)) if self.n_params <= 16 else 0, dtype=np.uint64)
         self.rng_n = np.zeros(Cn, dtype=np.uint64)
-        self.cols = [np.ascontiguousarray(np.asarray(c, dtype=np.float64)) for c in self.prog.columns]
-        self.colp = (C.POINTER(C.c_double) * max(len(self.cols), 1))(*[c.ctypes.data_as(C.POINTER(C.c_double)) for c in self.cols])
+        self.cols, self.colp = self._upload(self.prog.columns)
         self.adapting = np.ones(D, dtype=np.uint8)
         m = self.s._model_keepalive[-1]
         max_dim0 = max([m.params[p].dim0 for p in range(self.n_params) if m.params[p].n_comp > 1] + [1])
@@ -325,6 +494,7 @@ class HostKernel(HostProgram):
                         p(self.rng_n, C.c_uint64), C.c_uint64(self.chains), C.c_uint64(self.first_chain), C.c_uint64(self.seed), C.c_longlong(n),
                         C.c_longlong(0), C.c_longlong(thin), 1 if record else 0, int(mon.size), p(mon, C.c_int), p(out, C.c_double), self.colp,
                         len(self.cols), p(self.adapting, C.c_ubyte), *self._ext())
+        self._contract(self.cols)
         return out[:rows]
 
     def run(self, chains, first_chain, seed, sweeps):
@@ -370,6 +540,7 @@ class HostKernel(HostProgram):
                             p(self.rng_n, C.c_uint64), C.c_uint64(1), C.c_uint64(self.first_chain), C.c_uint64(self.seed), C.c_longlong(L),
                             C.c_longlong(i0), C.c_longlong(thin), 1 if record else 0, int(mon.size), p(mon, C.c_int), p(out, C.c_double), self.colp,
                             len(self.cols), p(self.adapting, C.c_ubyte), *self._ext())
+            self._contract(self.cols)
             for c in range(self.D):
                 if not self.is_adapting[c]:
                     continue
@@ -423,13 +594,12 @@ static inline int atomicAdd(int* p, int v) { const int o = *p; *p = o + v; retur
 static inline int min(int a, int b) { return a < b ? a : b; }
 static inline int max(int a, int b) { return a > b ? a : b; }
 namespace amwg {
-static inline double2 lds_f64x2(unsigned a) { double2 v; std::memcpy(&v, g_smem_base + a, 16); return v; }
+static inline double2 lds_f64x2(unsigned a) { double2 v{0.0, 0.0}; if (lds_ok(a, 16)) std::memcpy(&v, g_smem_base + a, 16); return v; }
 }
 '''
 
-STAT_EXPORTS = r'''
+STAT_EXPORTS = CONTRACT_EXPORTS + r'''
 extern "C" {
-unsigned char* hs_kernel_smem() { return amwg::smem; }
 double hs_exp_of(double x) { return amwg::js_exp(x); }
 int hs_nt() { return JNT; }
 void hs_sweep(double* state, double* psd, int* acc, double* work /* [2 JNT + 2 JD][C] */, unsigned short* vseq, unsigned long long* perm,
@@ -444,9 +614,7 @@ void hs_sweep(double* state, double* psd, int* acc, double* work /* [2 JNT + 2 J
   A.sa.n_sweeps = n_sweeps; A.sa.sample_i0 = 0; A.sa.thin = thin; A.sa.record = 1; A.sa.n_monitor = n_monitor; A.sa.monitor = monitor; A.sa.out = out;
   for (int k = 0; k < n_cols; ++k) A.col[k] = cols[k];
   A.adapting = adapting;
-  g_smem_base = amwg::smem;
-  blockDim.x = 1; threadIdx.x = 0;
-  for (unsigned long long c = 0; c < C; ++c) { blockIdx.x = (unsigned)c; amwg::amwg_jit_sweep(A); }
+  for (unsigned long long c = 0; c < C && !g_fault[0]; ++c) { hs_cta_begin((unsigned)c); amwg::amwg_jit_sweep(A); }
 }
 }
 '''
@@ -461,21 +629,25 @@ def _sum_sq_text():
 
 def _stat_kernel_text(generated):
     text = open(os.path.join(CSRC, "amwg_jit_kernel.cuh")).read()
-    lines, n_asm = [], 0
+    lines, n_asm, n_smem = [], 0, 0
     for ln in text.splitlines():
         if "asm volatile(" in ln:
             assert "fence.mbarrier_init" in ln, ln
             n_asm += 1
             continue
+        if "extern __shared__" in ln:
+            assert ln.strip() == "extern __shared__ __align__(16) unsigned char smem[];", ln
+            n_smem += 1
+            continue
         lines.append(ln)
-    assert n_asm == 1
+    assert n_asm == 1 and n_smem == 1
     text = "\n".join(lines)
     inc = '#include "amwg_jit_generated.inc"'
     assert text.count(inc) == 1
     return text.replace(inc, generated).replace("#pragma once", "")
 
 
-class HostStatKernel:
+class HostStatKernel(StrictShim):
     """`edit`: applied to the kernel's text before it is compiled (the self-checks of tests/stat_check.py plant a defect with it).
     After run(), `work` holds the working set ([tval | tcand | bprop | bcoin][chain]; work[:NT] is the term cache) and `state` the
     chains' components."""
@@ -499,11 +671,8 @@ class HostStatKernel:
             assert edited != kernel, "the edit did not change the kernel"
             kernel = edited
         cpp.write_text(src[:cut] + HOST_PRELUDE + STAT_SHIM + _tma_structs() + _sum_sq_text() + kernel + STAT_EXPORTS)
-        so = tmp_path / "stat_kernel.so"
-        r = subprocess.run(["g++", "-std=c++17", "-O1", "-ffp-contract=off", "-fPIC", "-shared", "-w", "-I" + os.path.join(ROOT, "tests", "host_shim"),
-                            "-I" + CSRC, str(cpp), "-o", str(so)], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        self.K = K = C.CDLL(str(so))
+        K = _compile(cpp, tmp_path / "stat_kernel.so")
+        self._shim_setup(K, src, msg)
         K.hs_exp_of.restype, K.hs_exp_of.argtypes = C.c_double, [C.c_double]
         self.D, self.NT, self.n_params = int(m.n_comp), K.hs_nt(), int(m.n_params)
         assert self.NT == self.prog.n_terms
@@ -525,8 +694,7 @@ class HostStatKernel:
         rng_n = np.zeros(Cn, dtype=np.uint64)
         mon = np.arange(D + len(self.s._derived_names), dtype=np.int32)
         out = np.full(((sweeps + thin - 1) // thin, mon.size, Cn), np.nan)
-        cols = [np.ascontiguousarray(np.asarray(c, dtype=np.float64)) for c in self.prog.columns]
-        colp = (C.POINTER(C.c_double) * max(len(cols), 1))(*[c.ctypes.data_as(C.POINTER(C.c_double)) for c in cols])
+        cols, colp = self._upload(self.prog.columns)
         adapting = np.ones(D, dtype=np.uint8) if adapting is None else np.asarray(adapting, dtype=np.uint8)
         self.acc, self.work, self.state = acc, work, state
         p = lambda a, t: a.ctypes.data_as(C.POINTER(t))
@@ -534,6 +702,7 @@ class HostStatKernel:
                         p(rng_n, C.c_uint64), C.c_uint64(Cn), C.c_uint64(first_chain), C.c_uint64(seed), C.c_longlong(sweeps), int(mon.size), p(mon, C.c_int),
                         p(out, C.c_double), colp, len(cols), p(adapting, C.c_ubyte),
                         perm_ext.ctypes.data_as(C.POINTER(C.c_ubyte)) if perm_ext is not None else None, None, C.c_longlong(thin))
+        self._contract(cols)
         return out, rng_n
 
 
@@ -701,3 +870,74 @@ def test_the_specialised_kernel_on_the_host_follows_the_golden_scripts(pkg, orc,
     for k in hk.s.params:
         assert gu.same(hk.state[e:e + width[k], 0], np.asarray(st[k], dtype=np.float64).reshape(-1)), k
         e += width[k]
+
+
+# ---- the strict shim itself: each rule of the bulk copy and the mbarrier refuses a bad call, with a message that says why -------------
+@pytest.fixture(scope="module")
+def shim(tmp_path_factory):
+    d = tmp_path_factory.mktemp("shim")
+    cpp = d / "shim.cpp"
+    cpp.write_text(HOST_PRELUDE + KERNEL_SHIM + CONTRACT_EXPORTS)
+    K = _compile(cpp, d / "shim.so")
+    K.hs_register_alloc.argtypes = [C.c_void_p, C.c_ulonglong]
+    K.hs_kernel_smem.restype = C.POINTER(C.c_ubyte)
+    K.hs_tma_bulk_g2s.argtypes = [C.c_ulonglong, C.c_void_p, C.c_uint, C.c_void_p]
+    K.hs_mbar_init.argtypes = K.hs_mbar_expect_tx.argtypes = K.hs_mbar_wait.argtypes = [C.c_void_p, C.c_uint]
+    return K
+
+
+def _stage(K, col, dst_off, bytes_, expect=None, parity=0, smem=1024, register=None):
+    """one staging as the kernels do it: init, expect_tx, one bulk copy of `bytes_` from `col`, wait -> the shim's first fault"""
+    K.hs_clear_fault()
+    K.hs_set_dyn_smem(smem)
+    K.hs_clear_allocs()
+    base, n = register if register is not None else (col.ctypes.data, col.nbytes)
+    K.hs_register_alloc(base, n)
+    bar = np.zeros(1, dtype=np.uint64)
+    K.hs_mbar_init(bar.ctypes.data, 1)
+    K.hs_mbar_expect_tx(bar.ctypes.data, bytes_ if expect is None else expect)
+    K.hs_tma_bulk_g2s(dst_off, col.ctypes.data, bytes_, bar.ctypes.data)
+    K.hs_mbar_wait(bar.ctypes.data, parity)
+    return K.hs_fault_msg().decode()
+
+
+def test_the_strict_shim_accepts_a_staging_that_follows_the_rules(shim):
+    (col,) = device_columns([np.arange(71.0)])                   # 568 bytes of data, 576 on the device
+    assert col.nbytes == 576 and col.ctypes.data % 16 == 0 and col[71] == 0.0
+    assert _stage(shim, col, 64, 576) == ""
+    got = np.ctypeslib.as_array(shim.hs_kernel_smem(), shape=(1024,))[64:64 + 576].copy().view(np.float64)
+    assert np.array_equal(got, col)
+
+
+def test_the_strict_shim_refuses_a_misaligned_source(shim):
+    (col,) = device_columns([np.arange(72.0)])
+    raw = np.ctypeslib.as_array((C.c_double * 72).from_address(col.ctypes.data + 8), shape=(71,))
+    msg = _stage(shim, raw, 0, 560, register=(col.ctypes.data, col.nbytes))
+    assert "16-byte aligned" in msg, msg
+
+
+def test_the_strict_shim_refuses_the_unpadded_column_copies(shim):
+    col = np.arange(71.0)                                         # a 568-byte column as numpy holds it
+    msg = _stage(shim, col, 0, 568, register=(col.ctypes.data, 568))
+    assert "positive multiple of 16" in msg, msg
+    msg = _stage(shim, col, 0, 576, register=(col.ctypes.data, 568))           # the padded size from an unpadded allocation
+    assert "runs past its end" in msg, msg
+
+
+def test_the_strict_shim_refuses_a_copy_past_the_declared_shared_memory(shim):
+    (col,) = device_columns([np.arange(71.0)])
+    msg = _stage(shim, col, 512, 576, smem=1024)
+    assert "outside the 1024 bytes of dynamic shared memory" in msg, msg
+
+
+def test_the_strict_shim_reports_an_expect_tx_that_differs_as_a_hang(shim):
+    (col,) = device_columns([np.arange(71.0)])
+    for expect in (576 + 16, 576 - 16):
+        msg = _stage(shim, col, 0, 576, expect=expect)
+        assert "would hang on the device" in msg and f"{expect} transaction bytes expected, 576 delivered" in msg, msg
+
+
+def test_the_strict_shim_refuses_a_wait_on_the_wrong_phase(shim):
+    (col,) = device_columns([np.arange(71.0)])
+    msg = _stage(shim, col, 0, 576, parity=1)
+    assert "parity 1 while the mbarrier is in phase 0" in msg, msg
