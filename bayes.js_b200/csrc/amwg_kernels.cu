@@ -557,14 +557,15 @@ __device__ __noinline__ double cold_op(int op, double x, double y, double z, dou
   }
 }
 
+// `loop_i0`: the point index DATA_I / COMP_I read outside a LOOP (a pointwise log-likelihood body, amwg_loo_pointwise).
 template <bool CACHE>
 __device__ __noinline__ double run_program_t(unsigned code_sa, unsigned consts_sa, const Ctx& ctx, const EvalStateT<CACHE>& es, int pc,
-                                             double* der, bool want_top) {
+                                             double* der, bool want_top, int loop_i0 = 0) {
   double stk[kStack];
   double tos = 0.0;
   int sp = 0;
   double lp = 0.0;
-  int loop_i = 0, loop_n = 0;
+  int loop_i = loop_i0, loop_n = 0;
 #define AMWG_NEXT() ((int)lds_u32(code_sa + 4u * (unsigned)(pc++)))
 #define AMWG_POP(dst) do { dst = tos; --sp; tos = stk[sp]; } while (0)
 #define AMWG_OPND(dst, mode)                                                               \
@@ -1325,6 +1326,7 @@ struct amwg_sampler {
   int jit_threads = 0;
   std::string jit_note = "not attempted";
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool;
+  std::vector<int64_t> col_n;      // values per data column (amwg_loo_pointwise checks its program's reads against them)
 };
 
 template <typename T>
@@ -1682,6 +1684,7 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
     double* d_col = nullptr;
     if (dev_upload(s, md->columns[k].values, (size_t)md->columns[k].n, &d_col)) return bail(-1);
     m.col_global[k] = d_col;
+    s->col_n.push_back(md->columns[k].n);
     m.col_bytes[k] = pad16(std::max<size_t>(sizeof(double) * (size_t)md->columns[k].n, 16));
     if (smem_used + m.col_bytes[k] <= resident_budget) { m.col_smem_off[k] = (int)smem_used; smem_used += m.col_bytes[k]; }
     else m.col_smem_off[k] = -1;       // too large for shared memory: served from L2 (streamed tiles: DESIGN.md "next")
@@ -2196,4 +2199,5 @@ extern "C" int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uin
 }
 
 #include "amwg_summary.cuh"
+#include "amwg_summary_loo.cuh"
 #include "amwg_peak.cuh"

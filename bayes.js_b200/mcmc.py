@@ -700,7 +700,7 @@ class AmwgSampler(Sampler):
         return buf
 
     def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None,
-                       nested=None):
+                       nested=None, loo=None):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -761,10 +761,24 @@ class AmwgSampler(Sampler):
         summarised (this handle's, or all of them with options.distributed) must be whole superchains. The device scratch
         (summary.nested_scratch_bytes) is counted in the memory check. Every other key keeps its bits. A refused nested (True
         without options.superchain_size, anything but None / False / True / an int >= 1, or chains that are not whole
-        superchains) raises ValueError before the chains move (summary.resolve_nested); see summary.finalize_nested."""
+        superchains) raises ValueError before the chains move (summary.resolve_nested); see summary.finalize_nested.
+        loo={"log_lik": f, "points": N} (optional "r_eff": a finite float > 0, default 1.0) adds the top-level key "loo": PSIS-LOO
+        and WAIC (Vehtari, Gelman & Gabry 2017; Vehtari et al. 2024) in ArviZ's conventions, from the pointwise log-likelihood
+        ll[s, i] = f(state, data, i) at every kept draw s (S = kept rows x chains, on all GPUs with options.distributed) and point
+        i < N, formed on the device and never moved to the host. f is traced once with a symbolic point index i, as a body under
+        mcmc.points(n) is (data.y[i], mu[data.g[i]], ld.*, Math.*), and evaluated with the model's arithmetic; components it reads
+        that are not monitored are sampled alongside and not returned. The dict holds "elpd_loo", "se_elpd_loo", "p_loo", "looic",
+        "elpd_waic", "se_elpd_waic", "p_waic", "waic", "pointwise" ({"elpd_loo", "lppd", "p_loo", "elpd_waic", "p_waic",
+        "pareto_k"}, each [N]), "pareto_k_threshold" (min(1 - 1/log10 S, 0.7)), "n_high_k", "r_eff", "n_draws" and "points"; see
+        summary.loo_block for the estimator. A point with a non-finite ll is NaN throughout, and so are the totals. r_eff = 1 is exact
+        for one row of independent chains; pass the relative efficiency for long chains. The points run in chunks sized to the
+        free device memory. Every other key keeps its bits. A refused loo (not a dict, unknown keys, points not an int >= 1, r_eff
+        not finite and > 0, a log_lik that branches on a parameter or indexes past a data array for some i < N, fewer than 2
+        draws, or a monitored name "loo") raises ValueError before the chains move (summary.resolve_loo, tracer.trace_log_lik)."""
         import torch
-        from .summary import (CudaBlockReducer, check_diagnostics, comoments_scratch_bytes, covariance_block, histogram_block, nested_block,
-                              nested_scratch_bytes, resolve_covariance, resolve_histogram, resolve_nested, summarise_block)
+        from .summary import (CudaBlockReducer, CudaPointwise, check_diagnostics, check_loo_size, comoments_scratch_bytes, covariance_block,
+                              histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block, nested_scratch_bytes, resolve_covariance,
+                              resolve_histogram, resolve_loo, resolve_nested, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
@@ -779,14 +793,30 @@ class AmwgSampler(Sampler):
         cov_plan = resolve_covariance(covariance, named, dims)
         first, held = (0, self.n_chains) if self.distributed else (self.first_chain, self.local_chains)
         superchain = resolve_nested(nested, self.superchain_size, first, held)
+        loo_plan = resolve_loo(loo, named)
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
         if rows == 0 or not entries:
             raise JsThrow("sample_summary needs at least one kept iteration and one monitored entry")
+        sampled = list(entries)                                 # the block's entries: the monitored ones, then what log_lik reads besides
+        if loo_plan is not None:
+            from .tracer import trace_log_lik
+            loo_m = check_loo_size(rows * self.n_chains, loo_plan.r_eff)
+            lik = trace_log_lik(loo_plan.log_lik, self.params, self._offsets, self.data, loo_plan.points)
+            start = {}
+            for name in lik.reads:
+                if name in spans and spans[name][1] > 0:
+                    start[name] = spans[name][0]
+                else:
+                    start[name] = len(sampled)
+                    sampled.extend(self._entries(name))
+            loo_prog = lik.lower(start)
         L = _ffi.lib()
         dev = torch.device("cuda", self.device)
-        need = rows * len(entries) * self.local_chains * 8
+        need = rows * len(sampled) * self.local_chains * 8
+        if len(sampled) > len(entries):
+            need += rows * len(entries) * self.local_chains * 8         # the monitored entries' block, copied out after the loo pass
         if plan is not None:
             # edges and counts of the histograms, and the extremes (8 B each)
             nb, pb = plan.bins or 0, plan.pair_bins
@@ -807,12 +837,30 @@ class AmwgSampler(Sampler):
             if need + 2 * len(entries) * self.local_chains * 8 + scratch > 0.9 * free:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
                               "device memory; raise thin() or lower n" % (need / 1e9, scratch / 1e9))
-        block = torch.empty((rows, len(entries), self.local_chains), dtype=torch.float64, device=dev)
-        mon = np.asarray(entries, dtype=np.int32)
+        if loo_plan is not None:
+            world = torch.distributed.get_world_size() if self.distributed else 1
+            per_point = loo_point_bytes(rows, self.local_chains, loo_tail_cap(loo_m), world)
+            chunk_points = int((0.9 * free - need - 2 * len(entries) * self.local_chains * 8) // per_point)
+            if chunk_points < 1:
+                raise JsThrow("sample_summary: the sample block (%.1f GB) and one point of the pointwise log-likelihood (%.1f GB) do not fit "
+                              "in device memory; raise thin() or lower n" % (need / 1e9, per_point / 1e9))
+            chunk_points = min(chunk_points, loo_plan.points, 65535)
+            if self.distributed:                                  # every rank takes the same chunks: the collectives pair up
+                t = torch.tensor([chunk_points], dtype=torch.int64, device=dev)
+                torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MIN)
+                chunk_points = int(t.item())
+        block = torch.empty((rows, len(sampled), self.local_chains), dtype=torch.float64, device=dev)
+        mon = np.asarray(sampled, dtype=np.int32)
         torch.cuda.current_stream(dev).synchronize()   # the library writes `block` on its own stream: torch's queued work goes first
-        rc = L.amwg_sample_device(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(entries), block.data_ptr())
+        rc = L.amwg_sample_device(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(sampled), block.data_ptr())
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
+        loo_out = None
+        if loo_plan is not None:
+            loo_out = loo_block(CudaBlockReducer(self.device), CudaPointwise(self._handle, loo_prog, block, self.device), rows, self.n_chains,
+                                loo_plan.points, loo_plan.r_eff, chunk_points, self.distributed)
+            if len(sampled) > len(entries):
+                block = block[:, :len(entries)].contiguous()
         res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
         hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
@@ -843,6 +891,8 @@ class AmwgSampler(Sampler):
             out.update(hist["pairs"])
         if cov is not None:
             out["covariance"] = cov
+        if loo_out is not None:
+            out["loo"] = loo_out
         return out
 
     def start_adaptation(self):

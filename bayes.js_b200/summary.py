@@ -261,6 +261,33 @@ class CudaBlockReducer:
                                                    out.ctypes.data))
         return out
 
+    def loo_reduce(self, ll, llmin, llmax, cut, cap: int):
+        """-> (sums [P, 3], tails float64 tensor [P, cap], counts int32 tensor [P]) of this shard; see amwg_loo_reduce in include/amwg.h."""
+        import torch
+        rows, P, chains = ll.shape
+        tails = torch.empty((P, cap), dtype=torch.float64, device=ll.device)
+        counts = torch.zeros(P, dtype=torch.int32, device=ll.device)
+        sums = np.empty((P, 3), dtype=np.float64)
+        f = lambda a: np.ascontiguousarray(a, dtype=np.float64)
+        mn, mx, ct = f(llmin), f(llmax), f(cut)
+        torch.cuda.current_stream(ll.device).synchronize()
+        self._ffi.check(self.L.amwg_loo_reduce(self.device, ll.data_ptr(), rows, P, chains, mn.ctypes.data, mx.ctypes.data, ct.ctypes.data, cap,
+                                               tails.data_ptr(), counts.data_ptr(), sums.ctypes.data))
+        return sums, tails, counts
+
+
+    def loo_fit(self, tails, counts, llmin, cut, skip) -> np.ndarray:
+        """tails [shards, P, cap], counts int32 [shards, P] (device) -> [P, 4]; see amwg_loo_fit in include/amwg.h."""
+        import torch
+        shards, P, cap = tails.shape
+        out = np.empty((P, 4), dtype=np.float64)
+        mn, ct = np.ascontiguousarray(llmin, dtype=np.float64), np.ascontiguousarray(cut, dtype=np.float64)
+        sk = np.ascontiguousarray(skip, dtype=np.int32)
+        torch.cuda.current_stream(tails.device).synchronize()
+        self._ffi.check(self.L.amwg_loo_fit(self.device, tails.data_ptr(), counts.data_ptr(), shards, P, cap, mn.ctypes.data, ct.ctypes.data,
+                                            sk.ctypes.data, out.ctypes.data))
+        return out
+
 
 # ---------------------------------------------------------------------------------------------------------------------
 # split-chain effective sample size (Vehtari et al. 2021, §3; Stan's `ess` on split chains, ArviZ's method="mean"/"tail")
@@ -1051,3 +1078,205 @@ def nested_block(reducer, block, rows: int, first_chain: int, M: int, distribute
     else:
         recs = [rec]
     return finalize_nested(merge_nested_records(recs, M, rows))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# PSIS-LOO and WAIC (Vehtari, Gelman & Gabry 2017; Vehtari et al., JMLR 2024), in ArviZ's conventions: DESIGN.md §4.7
+LOO_KEYS = ("log_lik", "points", "r_eff")
+MAX_LOO_TAIL = 1 << 20                 # include/amwg.h: amwg_loo_fit, tail_cap <= 2^20
+LOG_TINY = float(np.log(np.finfo(float).tiny))
+
+
+class LooPlan(NamedTuple):
+    """A checked `loo=` argument."""
+    log_lik: object
+    points: int
+    r_eff: float
+
+
+def resolve_loo(spec, names: Sequence[str]) -> Optional[LooPlan]:
+    """Checks the `loo=` argument of sample_summary: None, or {"log_lik": callable (state, data, i), "points": int >= 1,
+    "r_eff": finite float > 0 (default 1.0)}, with no monitored name "loo" (the key the result uses). Pure: raises ValueError
+    before any device work (tracing log_lik is the caller's next check)."""
+    if spec is None:
+        return None
+    if not isinstance(spec, dict):
+        raise ValueError("loo must be None or a dict {\"log_lik\": ..., \"points\": ...}, not %r" % (spec,))
+    unknown = [k for k in spec if k not in LOO_KEYS]
+    if unknown:
+        raise ValueError("loo has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(LOO_KEYS)))
+    if not callable(spec.get("log_lik")):
+        raise ValueError("loo needs \"log_lik\": a function (state, data, i) -> the log-likelihood of point i")
+    points = spec.get("points")
+    if not (_is_int(points) and points >= 1):
+        raise ValueError("loo points must be an int >= 1, not %r" % (points,))
+    r_eff = spec.get("r_eff", 1.0)
+    if not (isinstance(r_eff, numbers.Real) and not isinstance(r_eff, bool) and np.isfinite(r_eff) and r_eff > 0):
+        raise ValueError("loo r_eff must be a finite number > 0, not %r" % (r_eff,))
+    if "loo" in names:
+        raise ValueError("loo: a monitored parameter or derived quantity is named 'loo', the key the result would use")
+    return LooPlan(spec["log_lik"], int(points), float(r_eff))
+
+
+def loo_tail_length(S: int, r_eff: float) -> int:
+    """M = ceil(min(0.2 S, 3 sqrt(S / r_eff))): the Pareto tail holds the draws above the (M + 1)-th largest log weight."""
+    return int(np.ceil(min(0.2 * S, 3 * np.sqrt(S / r_eff))))
+
+
+def loo_tail_cap(M: int) -> int:
+    """The tail buffers' length per point: the power of two >= max(M, 8) (the fit kernel's bitonic sort)."""
+    cap = 8
+    while cap < M:
+        cap *= 2
+    return cap
+
+
+def loo_point_bytes(rows: int, chains: int, cap: int, world: int) -> int:
+    """Device bytes one point of a chunk takes, from the sizes the calls allocate (include/amwg.h): its ll column of the chunk; its
+    tail buffer and count (this rank's, and with world > 1 every rank's gathered); the fit's sort and value scratch (16 cap) and its
+    llmin / cut / skip / out (56); the per-CTA records of amwg_summary_moments (32 G + 32) and the sums of amwg_loo_reduce
+    (24 G + 48), G = min(ceil(chains / 256), 1184) CTAs; the select's prefix and digit counts (8 + 8 x 256); the finite range and
+    non-finite counts (16 + 24 + 16 + 24: the device keys and the returned tensors)."""
+    G = min(-(-chains // 256), 1184)
+    tails = (8 * cap + 4) * (1 + (world if world > 1 else 0))
+    return 8 * rows * chains + tails + 16 * cap + 56 + (32 * G + 32) + (24 * G + 48) + (8 + 8 * 256) + 80
+
+
+def check_loo_size(S: int, r_eff: float) -> int:
+    """-> M, or ValueError when S < 2 or the tail exceeds what the fit kernel holds."""
+    if S < 2:
+        raise ValueError("loo needs at least 2 draws (kept rows x chains), not %d" % S)
+    M = loo_tail_length(S, r_eff)
+    if M > MAX_LOO_TAIL:
+        raise ValueError("loo: a Pareto tail of %d draws per point (S = %d, r_eff = %g) exceeds %d" % (M, S, r_eff, MAX_LOO_TAIL))
+    return M
+
+
+class CudaPointwise:
+    """The pointwise log-likelihood chunks of one sample block: amwg_loo_pointwise over the handle's data columns."""
+
+    def __init__(self, handle, prog, block, device: int):
+        from . import _ffi
+        self.L, self._ffi = _ffi.lib(), _ffi
+        self.h, self.block, self.device = handle, block, device
+        self.code = np.ascontiguousarray(prog.code, dtype=np.int32)
+        self.consts = np.ascontiguousarray(prog.consts if prog.consts else [0.0], dtype=np.float64)
+        self.fold_prog = np.ascontiguousarray(prog.fold_prog if prog.fold_prog else [0], dtype=np.int32)
+        self.fold_dst = np.ascontiguousarray(prog.fold_dst if prog.fold_dst else [0], dtype=np.int32)
+        self.n_fold = len(prog.fold_prog)
+        self.body = prog.logpost_prog
+
+    def chunk(self, p0: int, P: int):
+        """-> float64 CUDA tensor [rows, P, chains]: ll of points p0 .. p0 + P - 1 at every kept draw of the block."""
+        import torch
+        rows, entries, chains = self.block.shape
+        out = torch.empty((rows, P, chains), dtype=torch.float64, device=self.block.device)
+        torch.cuda.current_stream(self.block.device).synchronize()
+        i32p = C.POINTER(C.c_int32)
+        self._ffi.check(self.L.amwg_loo_pointwise(self.h, self.code.ctypes.data_as(i32p), self.code.size,
+                                                  self.consts.ctypes.data_as(C.POINTER(C.c_double)), self.consts.size, self.body,
+                                                  self.fold_prog.ctypes.data_as(i32p), self.fold_dst.ctypes.data_as(i32p), self.n_fold,
+                                                  self.block.data_ptr(), rows, entries, p0, P, out.data_ptr()))
+        return out
+
+
+
+
+def _merged_range(reducer, ll, distributed: bool):
+    """-> (llmin, llmax, any non-finite) per point over all shards: the finite extremes and the non-finite counts."""
+    import torch
+    rng, nonfinite = reducer.finite_range(ll)
+    if distributed:
+        import torch.distributed as dist
+        P = ll.shape[1]
+        r = rng.cpu().numpy()
+        keys = torch.from_numpy(np.concatenate([-_sortable(r[:, 0]), _sortable(r[:, 1])]))
+        if ll.is_cuda:
+            keys = keys.to(ll.device)
+        dist.all_reduce(keys, op=dist.ReduceOp.MAX)
+        keys = keys.cpu().numpy()
+        rng = np.stack([_unsortable(-keys[:P]), _unsortable(keys[P:])], axis=1)
+        dist.all_reduce(nonfinite)
+    else:
+        rng = rng.cpu().numpy()
+    nf = nonfinite.cpu().numpy().sum(axis=1) > 0
+    return rng[:, 0].copy(), rng[:, 1].copy(), nf
+
+
+def _gather_tensor(t, distributed: bool):
+    """this rank's tensor -> [world, *shape] in rank order ([1, *shape] when not distributed)."""
+    if not distributed:
+        return t[None]
+    import torch
+    import torch.distributed as dist
+    ws = dist.get_world_size()
+    out = torch.empty((ws * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out, t.contiguous())
+    return out.reshape((ws,) + tuple(t.shape))
+
+
+def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff: float, chunk_points: int, distributed: bool) -> dict:
+    """-> the "loo" dict of sample_summary over all shards: PSIS-LOO and WAIC from the pointwise log-likelihood ll[s, i] of the
+    S = rows x total_chains kept draws. `source.chunk(p0, P)` gives ll of points p0 .. p0 + P - 1 as a [rows, P, chains] block
+    (this shard's chains); the points go in chunks of at most `chunk_points`. Per chunk, on the device: the finite range and
+    non-finite counts (amwg_summary_finite_range), the moments (amwg_summary_moments: var_s ll = (sum of within-chain M2 +
+    rows x M2 of the chain means) / S), the M-th smallest ll (0-based; the radix select of the quantiles), M =
+    ceil(min(0.2 S, 3 sqrt(S / r_eff))), so the (M + 1)-th largest lw = llmin - ll is c = llmin - that value and
+    cut = max(c, log(DBL_MIN)); then one pass for the sums and the tail (reducer.loo_reduce) and the Pareto fit over the tail
+    (reducer.loo_fit). Per point i, with lw = llmin - ll:
+      lppd_i      = llmax + log(sum exp(ll - llmax)) - log S
+      p_waic_i    = var_s ll (ddof 0),  elpd_waic_i = lppd_i - p_waic_i
+      elpd_loo_i  = llmin + log(sum exp(lw' + ll - llmin)) - log(sum exp(lw')), lw' the smoothed log weights
+                    (logsumexp(lw' - logsumexp(lw') + ll)),  p_loo_i = lppd_i - elpd_loo_i
+      pareto_k_i  the fitted k (+inf for a tail of <= 4 draws)
+    A point with any non-finite ll gets NaN in every value. Totals: sums of the pointwise values, se_* = sqrt(points var_i(elpd_*_i))
+    (ddof 0), looic = -2 elpd_loo, waic = -2 elpd_waic, pareto_k_threshold = min(1 - 1 / log10 S, 0.7), n_high_k = #{k > threshold}.
+    Distributed: extremes and counts all-reduce, moment records all-gather and merge in rank order, the select's counts
+    all-reduce, sums all-gather and add in rank order, tails all-gather (at most M values per point in all); the fit runs on the
+    merged tail, so every rank returns the same numbers."""
+    import torch
+    S = rows * total_chains
+    M = check_loo_size(S, r_eff)
+    cap = loo_tail_cap(M)
+    cols = {k: np.full(points, np.nan) for k in ("elpd_loo", "lppd", "p_loo", "elpd_waic", "p_waic", "pareto_k")}
+    for p0 in range(0, points, chunk_points):
+        P = min(chunk_points, points - p0)
+        ll = source.chunk(p0, P)
+        llmin, llmax, skip = _merged_range(reducer, ll, distributed)
+        rec = reducer.moments(ll)
+        if distributed:
+            rec = merge_moment_records(list(_gather_tensor(torch.from_numpy(rec).to(ll.device), True).cpu().numpy()))
+        var = (rec[:, 3] + rows * rec[:, 2]) / S
+        llM = _select(reducer, ll, np.array([M], dtype=np.int64), distributed).values()[:, 0]
+        with np.errstate(invalid="ignore"):
+            cut = np.maximum(llmin - llM, LOG_TINY)
+        # a point with a non-finite ll is NaN throughout: keep its draws out of the tail
+        mn, mx, ct = np.where(skip, 0.0, llmin), np.where(skip, 0.0, llmax), np.where(skip, np.inf, cut)
+        sums, tails, counts = reducer.loo_reduce(ll, mn, mx, ct, cap)
+        del ll
+        if distributed:
+            parts = _gather_tensor(torch.from_numpy(np.ascontiguousarray(sums)).to(tails.device), True).cpu().numpy()
+            sums = parts[0].copy()
+            for q in parts[1:]:
+                sums = sums + q
+        fit = reducer.loo_fit(_gather_tensor(tails, distributed), _gather_tensor(counts, distributed), mn, ct, skip.astype(np.int32))
+        del tails, counts
+        if np.any(fit[~skip, 3] > M):
+            raise RuntimeError("loo: a point's tail holds more than M = %d draws (inconsistent select)" % M)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            lppd = llmax + np.log(sums[:, 0]) - np.log(float(S))
+            elpd = llmin + np.log(sums[:, 2] + fit[:, 2]) - np.log(sums[:, 1] + fit[:, 1])
+        sl = slice(p0, p0 + P)
+        cols["lppd"][sl], cols["p_waic"][sl], cols["elpd_waic"][sl] = lppd, var, lppd - var
+        cols["elpd_loo"][sl], cols["p_loo"][sl], cols["pareto_k"][sl] = elpd, lppd - elpd, fit[:, 0]
+        for key in cols:
+            cols[key][sl][skip] = np.nan
+    thr = min(1.0 - 1.0 / np.log10(S), 0.7)
+    with np.errstate(invalid="ignore"):
+        n_high = int(np.sum(cols["pareto_k"] > thr))
+        out = {"elpd_loo": float(np.sum(cols["elpd_loo"])), "se_elpd_loo": float(np.sqrt(points * np.var(cols["elpd_loo"]))),
+               "p_loo": float(np.sum(cols["p_loo"])), "elpd_waic": float(np.sum(cols["elpd_waic"])),
+               "se_elpd_waic": float(np.sqrt(points * np.var(cols["elpd_waic"]))), "p_waic": float(np.sum(cols["p_waic"]))}
+    out["looic"], out["waic"] = -2.0 * out["elpd_loo"], -2.0 * out["elpd_waic"]
+    out.update(pointwise=cols, pareto_k_threshold=float(thr), n_high_k=n_high, r_eff=float(r_eff), n_draws=int(S), points=int(points))
+    return out

@@ -1214,6 +1214,82 @@ def trace(log_post, params: Dict[str, dict], offsets: Dict[str, int], n_comp: in
     return prog, list(derived.keys())
 
 
+class LogLik:
+    """A traced pointwise log-likelihood (sample_summary(..., loo=...)): the recorded expression of ``log_lik(state, data, i)``
+    at a symbolic point index i of `points` points, and the parameters it reads (in the parameters' order)."""
+
+    def __init__(self, tracer: Tracer, expr: Sym, reads: List[str], ranges: List[Tuple[str, int, int]]):
+        self.tracer, self.expr, self.reads, self._ranges = tracer, expr, reads, ranges
+
+    def lower(self, entry_start: Dict[str, int]) -> Program:
+        """The body as an expression program addressing the sample block's ENTRIES: component c of parameter `name` (first
+        component `off`) becomes entry entry_start[name] + c - off, for COMP and for the base of COMP_I alike (a parameter's
+        entries are contiguous in the block). The body is at word 0 and leaves its value on the stack; its constant
+        sub-expressions become fold programs (evaluated on the device, amwg_loo_pointwise) with their own constant bank."""
+        def entry(c: int) -> int:
+            for name, off, n in self._ranges:
+                if off <= c < off + n:
+                    return entry_start[name] + c - off
+            raise JsThrow("log_lik reads component %d, which belongs to no parameter" % c)
+        memo: Dict[int, Sym] = {}
+
+        def remap(n: Sym) -> Sym:
+            got = memo.get(id(n))
+            if got is not None:
+                return got
+            if n.op == "COMP":
+                out = Sym("COMP", (), entry(n.val))
+            elif n.op == "COMP_I":
+                col, off, stride, base, pid = n.val
+                out = Sym("COMP_I", (), (col, off, stride, entry(base), pid))
+            elif n.args:
+                out = Sym(n.op, tuple(remap(a) for a in n.args), n.val)
+            else:
+                out = n
+            memo[id(n)] = out
+            return out
+        low = Lowering(self.tracer, 0)
+        low.emit_expr(remap(self.expr))
+        low.prog.emit("END")
+        low.prog.logpost_prog = 0
+        return low.finish()
+
+
+def trace_log_lik(log_lik, params: Dict[str, dict], offsets: Dict[str, int], data, points: int) -> LogLik:
+    """Run ``log_lik(state, data, i)`` once with symbolic parameters, proxied data and a symbolic point index i over `points`
+    points (``data.y[i]`` -> DATA_I, ``mu[data.g[i]]`` -> COMP_I, as under mcmc.points), with the ld.* / Math rules of log_post.
+    Raises ValueError when the closure cannot be traced for the device: it branches on a parameter, reads a data array past its
+    end at some i < points, indexes a parameter with data values outside it, or returns something that is not a number."""
+    tr = Tracer()
+    wrapped = tr.wrap_data(data)
+    i = tr.new_plate_index(points)
+    state = tr.make_state(params, offsets)
+    _ACTIVE.append(tr)
+    try:
+        result = log_lik(state, wrapped, i)
+        if result is None:
+            raise JsThrow("log_lik returned undefined")
+        expr = lift(result)
+    except JsThrow as exc:
+        raise ValueError("loo: log_lik cannot be evaluated on the device: " + exc.message) from None
+    finally:
+        _ACTIVE.pop()
+    ranges = [(name, offsets[name], int(np.prod(p["dim"]))) for name, p in params.items()]
+    comps, stack, seen = set(), [expr], set()
+    while stack:
+        n = stack.pop()
+        if id(n) in seen:
+            continue
+        seen.add(id(n))
+        if n.op == "COMP":
+            comps.add(n.val)
+        elif n.op == "COMP_I":
+            comps.add(n.val[3])
+        stack.extend(n.args)
+    reads = [name for name, off, n in ranges if any(off <= c < off + n for c in comps)]
+    return LogLik(tr, expr, reads, ranges)
+
+
 _ACTIVE: List[Tracer] = []
 
 

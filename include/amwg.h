@@ -402,6 +402,39 @@ AMWG_API int amwg_summary_comoments(int device, const double* dev_samples, int64
 AMWG_API int amwg_summary_nested(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int64_t first_chain,
                                  int64_t superchain_size, double* host_out);
 
+/* ---- PSIS-LOO and WAIC (sample_summary(..., loo=...), DESIGN.md §4.7) ------------------------------------------------------
+ * amwg_loo_pointwise: dev_out[row][p][chain] = the pointwise log-likelihood at point p0 + p (p < n_points) of the kept draw (row,
+ *   chain) of dev_samples, a block in amwg_sample_device's layout [rows][entries][chains] with chains = the handle's chains. The
+ *   program (host_code[n_code], constants host_consts[n_consts]) is an expression program: body_prog leaves the value and ends
+ *   with END; COMP and COMP_I address block ENTRIES (the host maps every component the body reads to its entry); DATA_I / COMP_I
+ *   read the handle's data columns at the point index. Before the body runs, each fold program host_fold_prog[k] (in order) is
+ *   evaluated on the device into constant host_fold_dst[k], as amwg_create folds the model's constants. One thread per (row,
+ *   chain) runs the model's interpreter over the points; the output is the sample-block layout with points as entries, so the
+ *   amwg_summary_* reductions read it unchanged. Errors (nothing runs): a malformed program, one that is not an expression (sums,
+ *   plates, loops, stores, cache words), a constant, entry or fold index out of range, a data read outside its column at some point
+ *   of the range, a COMP_I data value that is not an entry, program and constants over 200 KB.
+ * amwg_loo_reduce: over a chunk dev_ll[rows][points][chains] and per point the host's llmin, llmax (smallest / largest finite ll)
+ *   and cut: host_sums[point][3] = { sum exp(ll - llmax) over all draws, sum exp(lw) and sum exp((lw + ll) - llmin) over the draws
+ *   with lw = llmin - ll <= cut }, each formed in a fixed order (deterministic); every draw with lw > cut has its ll appended to
+ *   dev_tail[point][tail_cap] at slot dev_count[point]++ (int32, zeroed by the caller; slots past tail_cap are counted, not
+ *   written). Errors: an empty block, points > 65535, tail_cap outside 1..2^20, null pointers.
+ * amwg_loo_fit: one CTA per point gathers the tails dev_tails[shard][point][tail_cap] (dev_counts[shard][point] values each),
+ *   sorts them and fits a generalised Pareto to the ascending exp(lw) - exp(cut), lw = llmin - ll (Zhang & Stephens 2009 with
+ *   the prior on k; csrc/amwg_loo.cuh). host_out[point][4] = { k, sum exp(lw), sum exp((lw + ll) - llmin) over the tail with lw
+ *   replaced by the smoothed weights when k is finite, the tail draws over all shards }; a tail of <= 4 draws gives k = +inf and
+ *   raw weights; host_skip[point] != 0 gives NaN. Deterministic. Errors: tail_cap not a power of two in 8..2^20, shards or points
+ *   < 1, null pointers.
+ * Device scratch of the three calls, from one per-device pool grown on demand: the program (pointwise), 3 x 8 points + 24 points
+ *   G (G = min(ceil(chains / 256), 1184)) bytes (reduce), 3 x 8 points + 16 points tail_cap + 32 points bytes (fit). */
+AMWG_API int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
+                                int32_t body_prog, const int32_t* host_fold_prog, const int32_t* host_fold_dst, int32_t n_fold,
+                                const double* dev_samples, int64_t rows, int32_t entries, int64_t p0, int32_t n_points, double* dev_out);
+AMWG_API int amwg_loo_reduce(int device, const double* dev_ll, int64_t rows, int32_t points, int64_t chains, const double* host_llmin,
+                             const double* host_llmax, const double* host_cut, int32_t tail_cap, double* dev_tail, int32_t* dev_count,
+                             double* host_sums);
+AMWG_API int amwg_loo_fit(int device, const double* dev_tails, const int32_t* dev_counts, int32_t shards, int32_t points, int32_t tail_cap,
+                          const double* host_llmin, const double* host_cut, const int32_t* host_skip, double* host_out);
+
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it
  * for sm_90a with NVRTC and steps with that kernel instead of the bytecode interpreter (csrc/amwg_jit.cuh; AMWG_JIT=0 in the

@@ -529,6 +529,48 @@ BINDING(summary_nested)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// loo_pointwise(handle, code [n], consts [k], body_prog, fold_prog [f], fold_dst [f], samples ptr, rows, entries, p0, n_points, out ptr)
+//                                                                                                          amwg_loo_pointwise
+BINDING(loo_pointwise)
+  Handle* h = handle_of(env, a.at(0));
+  const std::vector<int32_t> code = ints(env, a.at(1)), fp = ints(env, a.at(4)), fd = ints(env, a.at(5));
+  const std::vector<double> consts = doubles(env, a.at(2));
+  if (fp.size() != fd.size()) throw Throw{"loo_pointwise: fold_prog and fold_dst must have the same length"};
+  if (amwg_loo_pointwise(h->s, code.data(), (int32_t)code.size(), consts.data(), (int32_t)consts.size(), (int32_t)to_double(env, a.at(3)),
+                         fp.data(), fd.data(), (int32_t)fp.size(), (const double*)(uintptr_t)to_u64(env, a.at(6)), (int64_t)to_double(env, a.at(7)),
+                         (int32_t)to_double(env, a.at(8)), (int64_t)to_double(env, a.at(9)), (int32_t)to_double(env, a.at(10)),
+                         (double*)(uintptr_t)to_u64(env, a.at(11))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// loo_reduce(device, ll ptr, rows, points, chains, llmin [points], llmax [points], cut [points], tail_cap, tail ptr, count ptr)
+//   -> Float64Array [points][3]                                                                                  amwg_loo_reduce
+BINDING(loo_reduce)
+  const int32_t points = (int32_t)to_double(env, a.at(3));
+  const std::vector<double> mn = doubles(env, a.at(5)), mx = doubles(env, a.at(6)), ct = doubles(env, a.at(7));
+  if (points < 0 || mn.size() != (size_t)points || mx.size() != (size_t)points || ct.size() != (size_t)points)
+    throw Throw{"loo_reduce: llmin, llmax and cut must hold one number per point"};
+  std::vector<double> out((size_t)points * 3);
+  if (amwg_loo_reduce((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)), points,
+                      (int64_t)to_double(env, a.at(4)), mn.data(), mx.data(), ct.data(), (int32_t)to_double(env, a.at(8)),
+                      (double*)(uintptr_t)to_u64(env, a.at(9)), (int32_t*)(uintptr_t)to_u64(env, a.at(10)), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
+// loo_fit(device, tails ptr, counts ptr, shards, points, tail_cap, llmin [points], cut [points], skip [points]) -> Float64Array [points][4]
+//                                                                                                               amwg_loo_fit
+BINDING(loo_fit)
+  const int32_t points = (int32_t)to_double(env, a.at(4));
+  const std::vector<double> mn = doubles(env, a.at(6)), ct = doubles(env, a.at(7));
+  const std::vector<int32_t> skip = ints(env, a.at(8));
+  if (points < 0 || mn.size() != (size_t)points || ct.size() != (size_t)points || skip.size() != (size_t)points)
+    throw Throw{"loo_fit: llmin, cut and skip must hold one value per point"};
+  std::vector<double> out((size_t)points * 4);
+  if (amwg_loo_fit((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (const int32_t*)(uintptr_t)to_u64(env, a.at(2)),
+                   (int32_t)to_double(env, a.at(3)), points, (int32_t)to_double(env, a.at(5)), mn.data(), ct.data(), skip.data(), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
 // term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
 BINDING(term_cache)
   Handle* h = handle_of(env, a.at(0));
@@ -563,6 +605,7 @@ NAPI_MODULE_INIT() {
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
       {"summary_comoments", summary_comoments}, {"summary_nested", summary_nested},
+      {"loo_pointwise", loo_pointwise}, {"loo_reduce", loo_reduce}, {"loo_fit", loo_fit},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
