@@ -2200,4 +2200,5 @@ extern "C" int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uin
 
 #include "amwg_summary.cuh"
 #include "amwg_summary_loo.cuh"
+#include "amwg_summary_ppc.cuh"
 #include "amwg_peak.cuh"

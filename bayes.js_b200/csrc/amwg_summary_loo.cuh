@@ -198,28 +198,23 @@ inline int loo_scratch(int device, size_t need, void** out, const char* who) {
 
 static std::mutex g_loo_mu;               // the calls below share one scratch pool per device
 
-extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
-                                  int32_t body_prog, const int32_t* host_fold_prog, const int32_t* host_fold_dst, int32_t n_fold,
-                                  const double* dev_samples, int64_t rows, int32_t entries, int64_t p0, int32_t n_points, double* dev_out) {
-  const char* who = "amwg_loo_pointwise";
-  if (!s) return fail("amwg_loo_pointwise: NULL handle");
-  if (!host_code || !host_consts || !dev_samples || !dev_out || (n_fold > 0 && (!host_fold_prog || !host_fold_dst)))
-    return fail("amwg_loo_pointwise: null pointer");
-  if (rows <= 0 || entries <= 0 || n_points <= 0 || n_code <= 0 || n_consts <= 0 || n_fold < 0) return fail("amwg_loo_pointwise: empty program or block");
-  if (p0 < 0 || p0 + n_points > ((int64_t)1 << 31) - 1) return fail("amwg_loo_pointwise: point range out of bounds");
-  const size_t smem = (((size_t)n_code * 4 + 7) & ~(size_t)7) + (size_t)n_consts * 8;
-  if (smem > kSmemBudget) return fail("amwg_loo_pointwise: the program and its constants exceed the shared memory budget");
-  // every program: well formed, an expression (no sum, plate, loop, store or cache word), each index inside its table and, for
-  // the body, each data read inside its column at every point of the range; the body leaves one value
+// The checks of amwg_loo_pointwise and amwg_ppc_pointwise, before anything runs: every program well formed and an expression (no
+// sum, plate, loop, store or cache word), each index inside its table and, for the body programs `bodies`, each data read inside
+// its column at every point of p0 .. p0 + n_points - 1; each program leaves one value.
+static int check_pointwise_programs(amwg_sampler* s, const char* who, const int32_t* host_code, int32_t n_code, int32_t n_consts,
+                                    const std::vector<int>& bodies, const int32_t* host_fold_prog, const int32_t* host_fold_dst,
+                                    int32_t n_fold, int32_t entries, int64_t p0, int32_t n_points) {
   amwg_model md{};
   md.code = host_code; md.n_code = n_code;
-  std::vector<int> progs{body_prog};
+  std::vector<int> progs(bodies);
+  const size_t n_bodies = bodies.size();
   for (int k = 0; k < n_fold; ++k) {
-    if (host_fold_dst[k] < 0 || host_fold_dst[k] >= n_consts) return fail("amwg_loo_pointwise: constant-folding table out of range");
+    if (host_fold_dst[k] < 0 || host_fold_dst[k] >= n_consts) return fail(std::string(who) + ": constant-folding table out of range");
     progs.push_back(host_fold_prog[k]);
   }
   const int64_t p1 = p0 + n_points - 1;
   for (size_t q = 0; q < progs.size(); ++q) {
+    const bool fold = q >= n_bodies;
     std::vector<jit::Insn> ins;
     std::string err;
     int depth = 0;
@@ -231,17 +226,17 @@ extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int
       if (in.acc || in.store) return fail(std::string(who) + ": the program must be an expression");
       for (int k = 0; k < 4; ++k) {
         if (in.mode[k] == AMWG_MODE_CONST && (in.inl[k] < 0 || in.inl[k] >= n_consts)) return fail(std::string(who) + ": constant index out of range");
-        if (in.mode[k] == AMWG_MODE_COMP && (q > 0 || in.inl[k] < 0 || in.inl[k] >= entries)) return fail(std::string(who) + ": entry index out of range");
+        if (in.mode[k] == AMWG_MODE_COMP && (fold || in.inl[k] < 0 || in.inl[k] >= entries)) return fail(std::string(who) + ": entry index out of range");
       }
       switch (in.op) {
         case AMWG_OP_END: break;
         case AMWG_OP_CONST: if (in.a >= n_consts) return fail(std::string(who) + ": constant index out of range"); break;
-        case AMWG_OP_COMP: if (q > 0 || in.a >= entries) return fail(std::string(who) + ": entry index out of range"); break;
+        case AMWG_OP_COMP: if (fold || in.a >= entries) return fail(std::string(who) + ": entry index out of range"); break;
         case AMWG_OP_DATA:
           if (in.a >= (int)s->col_n.size() || in.extra[0] < 0 || in.extra[0] >= s->col_n[in.a]) return fail(std::string(who) + ": data index out of range");
           break;
         case AMWG_OP_DATA_I: case AMWG_OP_COMP_I: {
-          if (q > 0 || in.a >= (int)s->col_n.size()) return fail(std::string(who) + ": data column out of range");
+          if (fold || in.a >= (int)s->col_n.size()) return fail(std::string(who) + ": data column out of range");
           const int64_t off = in.extra[0], stride = in.extra[1], lo = off + stride * p0, hi = off + stride * p1, n = s->col_n[in.a];
           if (lo < 0 || lo >= n || hi < 0 || hi >= n) return fail(std::string(who) + ": a point index runs past the end of a data column");
           if (in.op == AMWG_OP_COMP_I) {                     // entries[base + data[i]] must stay inside the block's entries
@@ -264,9 +259,16 @@ extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int
     }
     if (left != 1) return fail(std::string(who) + ": the program must leave exactly one value");
   }
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(s->device));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));               // the sampler's stream wrote the block
+  return 0;
+}
+
+// Copies the checked program, its constants, the fold table and the handle's data column pointers into the per-device pool and
+// folds the constants on the device (K_l0), for a pointwise kernel with `smem` bytes of dynamic shared memory. The caller holds
+// g_loo_mu and has selected the handle's device.
+static int stage_pointwise_program(amwg_sampler* s, const char* who, const void* kernel, size_t smem, const int32_t* host_code,
+                                   int32_t n_code, const double* host_consts, int32_t n_consts, const int32_t* host_fold_prog,
+                                   const int32_t* host_fold_dst, int32_t n_fold, int** d_code_out, double** d_consts_out,
+                                   summary::LooColumns** d_cols_out) {
   const size_t b_code = ((size_t)n_code * 4 + 15) & ~(size_t)15, b_consts = ((size_t)n_consts * 8 + 15) & ~(size_t)15;
   const size_t b_fold = (((size_t)std::max(n_fold, 1) * 4) + 15) & ~(size_t)15;
   void* base = nullptr;
@@ -289,9 +291,35 @@ extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int
   CUDA_TRY(cudaMemcpy(d_cols, &cols, sizeof cols, cudaMemcpyHostToDevice));
   if (smem > 48 * 1024) {
     CUDA_TRY(cudaFuncSetAttribute(summary::amwg_loo_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CUDA_TRY(cudaFuncSetAttribute(summary::amwg_loo_pointwise_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
   if (n_fold > 0) summary::amwg_loo_fold_kernel<<<1, 1, smem>>>(d_code, n_code, d_consts, n_consts, d_fp, d_fd, n_fold, d_cols);
+  *d_code_out = d_code; *d_consts_out = d_consts; *d_cols_out = d_cols;
+  return 0;
+}
+
+extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
+                                  int32_t body_prog, const int32_t* host_fold_prog, const int32_t* host_fold_dst, int32_t n_fold,
+                                  const double* dev_samples, int64_t rows, int32_t entries, int64_t p0, int32_t n_points, double* dev_out) {
+  const char* who = "amwg_loo_pointwise";
+  if (!s) return fail("amwg_loo_pointwise: NULL handle");
+  if (!host_code || !host_consts || !dev_samples || !dev_out || (n_fold > 0 && (!host_fold_prog || !host_fold_dst)))
+    return fail("amwg_loo_pointwise: null pointer");
+  if (rows <= 0 || entries <= 0 || n_points <= 0 || n_code <= 0 || n_consts <= 0 || n_fold < 0) return fail("amwg_loo_pointwise: empty program or block");
+  if (p0 < 0 || p0 + n_points > ((int64_t)1 << 31) - 1) return fail("amwg_loo_pointwise: point range out of bounds");
+  const size_t smem = (((size_t)n_code * 4 + 7) & ~(size_t)7) + (size_t)n_consts * 8;
+  if (smem > kSmemBudget) return fail("amwg_loo_pointwise: the program and its constants exceed the shared memory budget");
+  if (check_pointwise_programs(s, who, host_code, n_code, n_consts, {body_prog}, host_fold_prog, host_fold_dst, n_fold, entries, p0, n_points))
+    return -1;
+  std::lock_guard<std::mutex> lock(g_loo_mu);
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));               // the sampler's stream wrote the block
+  int* d_code = nullptr;
+  double* d_consts = nullptr;
+  summary::LooColumns* d_cols = nullptr;
+  if (stage_pointwise_program(s, who, (const void*)summary::amwg_loo_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
+                              host_fold_prog, host_fold_dst, n_fold, &d_code, &d_consts, &d_cols))
+    return -1;
   const long long C = (long long)s->a.C;
   const dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)std::min<int64_t>(rows, 65535), (unsigned)((rows + 65534) / 65535));
   summary::amwg_loo_pointwise_kernel<<<grid, kThreads, smem>>>(d_code, n_code, d_consts, n_consts, body_prog, d_cols, dev_samples, entries, rows,

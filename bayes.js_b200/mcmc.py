@@ -700,7 +700,7 @@ class AmwgSampler(Sampler):
         return buf
 
     def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None,
-                       nested=None, loo=None):
+                       nested=None, loo=None, ppc=None):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -774,11 +774,29 @@ class AmwgSampler(Sampler):
         for one row of independent chains; pass the relative efficiency for long chains. The points run in chunks sized to the
         free device memory. Every other key keeps its bits. A refused loo (not a dict, unknown keys, points not an int >= 1, r_eff
         not finite and > 0, a log_lik that branches on a parameter or indexes past a data array for some i < N, fewer than 2
-        draws, or a monitored name "loo") raises ValueError before the chains move (summary.resolve_loo, tracer.trace_log_lik)."""
+        draws, or a monitored name "loo") raises ValueError before the chains move (summary.resolve_loo, tracer.trace_log_lik).
+        ppc={"log_lik": f, "points": N} adds the top-level key "ppc": posterior predictive checks (BDA3 ch. 6; ArviZ's plot_ppc /
+        plot_bpv). f is the kind of function loo= takes (often the same one), traced the same way; its value must be one ld.* call
+        whose first argument is a data value at the point index, e.g. ld.norm(data.y[i], mu[data.g[i]], sigma): that names the
+        observation y_i and the family, and the other arguments are the family's parameters at point i. At every kept draw (S =
+        kept rows x chains, all GPUs with options.distributed) the device draws a replicated dataset y_rep_0 .. y_rep_{N-1} from
+        that family (csrc/amwg_ppc.cuh: every family but hyper, with the samplers and domains listed there; parameters outside the
+        domain give NaN), from the chain's own Math.random() stream at positions reserved for (kept row, point) (DESIGN.md §4.8:
+        repeated calls reuse those positions for new posterior draws), and nothing of it moves to the host. The dict holds
+        "family" (the ld name), "points", "n_draws", "pointwise" ({"mean", "sd" (pooled, ddof 1), "n_below", "n_equal", "n_nan"
+        (int64: y_rep_i < y_i, == y_i, NaN), "pit" = (n_below + n_equal) / S}, each [N]) and "stats": for each T in "mean", "sd",
+        "min", "max" of a dataset (points in index order; sequential Welford, sd ddof 1, NaN-propagating min / max) {"observed"
+        T(y), "mean", "sd", "quantiles" (probs) of T(y_rep), "n_greater", "n_equal", "n_nan", "p_value" = (n_greater + n_equal)
+        / S: Pr(T(y_rep) >= T(y)), a NaN draw counting as not >=}; see summary.ppc_block. With loo= it shares the sample block.
+        The points run in chunks sized to the free device memory. Every other key keeps its bits. A refused ppc (not a dict,
+        unknown keys, points not an int >= 1, anything loo refuses in f, a value that is not one ld.* call with data[i] first, a
+        family without a sampler, kept rows x points >= 2^46, or a monitored name "ppc") raises ValueError before the chains move
+        (summary.resolve_ppc, summary.check_ppc_call, tracer.LogLik.observed_call)."""
         import torch
-        from .summary import (CudaBlockReducer, CudaPointwise, check_diagnostics, check_loo_size, comoments_scratch_bytes, covariance_block,
-                              histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block, nested_scratch_bytes, resolve_covariance,
-                              resolve_histogram, resolve_loo, resolve_nested, summarise_block)
+        from .summary import (CudaBlockReducer, CudaPointwise, CudaPpc, check_diagnostics, check_loo_size, check_ppc_call, comoments_scratch_bytes,
+                              covariance_block, histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block, nested_scratch_bytes,
+                              ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance, resolve_histogram, resolve_loo, resolve_nested,
+                              resolve_ppc, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries: List[int] = []
@@ -794,29 +812,46 @@ class AmwgSampler(Sampler):
         first, held = (0, self.n_chains) if self.distributed else (self.first_chain, self.local_chains)
         superchain = resolve_nested(nested, self.superchain_size, first, held)
         loo_plan = resolve_loo(loo, named)
+        ppc_plan = resolve_ppc(ppc, named)
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
         if rows == 0 or not entries:
             raise JsThrow("sample_summary needs at least one kept iteration and one monitored entry")
         sampled = list(entries)                                 # the block's entries: the monitored ones, then what log_lik reads besides
-        if loo_plan is not None:
-            from .tracer import trace_log_lik
-            loo_m = check_loo_size(rows * self.n_chains, loo_plan.r_eff)
-            lik = trace_log_lik(loo_plan.log_lik, self.params, self._offsets, self.data, loo_plan.points)
-            start = {}
-            for name in lik.reads:
+        start = {}
+
+        def block_entries(reads):
+            for name in reads:
+                if name in start:
+                    continue
                 if name in spans and spans[name][1] > 0:
                     start[name] = spans[name][0]
                 else:
                     start[name] = len(sampled)
                     sampled.extend(self._entries(name))
+        if loo_plan is not None:
+            from .tracer import trace_log_lik
+            loo_m = check_loo_size(rows * self.n_chains, loo_plan.r_eff)
+            lik = trace_log_lik(loo_plan.log_lik, self.params, self._offsets, self.data, loo_plan.points)
+        if ppc_plan is not None:
+            from .tracer import trace_log_lik
+            ppc_lik = trace_log_lik(ppc_plan.log_lik, self.params, self._offsets, self.data, ppc_plan.points, what="ppc")
+            ppc_family, ppc_y, ppc_args = ppc_lik.observed_call(ppc_plan.points)
+            ppc_code = check_ppc_call(ppc_family, rows, ppc_plan.points)
+        if loo_plan is not None:
+            block_entries(lik.reads)
             loo_prog = lik.lower(start)
+        if ppc_plan is not None:
+            block_entries(ppc_lik.reads)
+            ppc_prog, ppc_offs = ppc_lik.lower_exprs(ppc_args, start)
         L = _ffi.lib()
         dev = torch.device("cuda", self.device)
         need = rows * len(sampled) * self.local_chains * 8
         if len(sampled) > len(entries):
-            need += rows * len(entries) * self.local_chains * 8         # the monitored entries' block, copied out after the loo pass
+            need += rows * len(entries) * self.local_chains * 8         # the monitored entries' block, copied out after the loo / ppc pass
+        if ppc_plan is not None:
+            need += ppc_fixed_bytes(rows, self.local_chains)
         if plan is not None:
             # edges and counts of the histograms, and the extremes (8 B each)
             nb, pb = plan.bins or 0, plan.pair_bins
@@ -837,18 +872,23 @@ class AmwgSampler(Sampler):
             if need + 2 * len(entries) * self.local_chains * 8 + scratch > 0.9 * free:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
                               "device memory; raise thin() or lower n" % (need / 1e9, scratch / 1e9))
-        if loo_plan is not None:
-            world = torch.distributed.get_world_size() if self.distributed else 1
-            per_point = loo_point_bytes(rows, self.local_chains, loo_tail_cap(loo_m), world)
+        def chunk_size(per_point, points, what):
             chunk_points = int((0.9 * free - need - 2 * len(entries) * self.local_chains * 8) // per_point)
             if chunk_points < 1:
-                raise JsThrow("sample_summary: the sample block (%.1f GB) and one point of the pointwise log-likelihood (%.1f GB) do not fit "
-                              "in device memory; raise thin() or lower n" % (need / 1e9, per_point / 1e9))
-            chunk_points = min(chunk_points, loo_plan.points, 65535)
+                raise JsThrow("sample_summary: the sample block (%.1f GB) and one point of the %s (%.1f GB) do not fit "
+                              "in device memory; raise thin() or lower n" % (need / 1e9, what, per_point / 1e9))
+            chunk_points = min(chunk_points, points, 65535)
             if self.distributed:                                  # every rank takes the same chunks: the collectives pair up
                 t = torch.tensor([chunk_points], dtype=torch.int64, device=dev)
                 torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MIN)
                 chunk_points = int(t.item())
+            return chunk_points
+        if loo_plan is not None:
+            world = torch.distributed.get_world_size() if self.distributed else 1
+            chunk_points = chunk_size(loo_point_bytes(rows, self.local_chains, loo_tail_cap(loo_m), world), loo_plan.points,
+                                      "pointwise log-likelihood")
+        if ppc_plan is not None:
+            ppc_chunk = chunk_size(ppc_point_bytes(rows, self.local_chains), ppc_plan.points, "replicated data")
         block = torch.empty((rows, len(sampled), self.local_chains), dtype=torch.float64, device=dev)
         mon = np.asarray(sampled, dtype=np.int32)
         torch.cuda.current_stream(dev).synchronize()   # the library writes `block` on its own stream: torch's queued work goes first
@@ -859,8 +899,12 @@ class AmwgSampler(Sampler):
         if loo_plan is not None:
             loo_out = loo_block(CudaBlockReducer(self.device), CudaPointwise(self._handle, loo_prog, block, self.device), rows, self.n_chains,
                                 loo_plan.points, loo_plan.r_eff, chunk_points, self.distributed)
-            if len(sampled) > len(entries):
-                block = block[:, :len(entries)].contiguous()
+        ppc_out = None
+        if ppc_plan is not None:
+            ppc_out = ppc_block(CudaBlockReducer(self.device), CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points),
+                                rows, self.n_chains, ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed)
+        if len(sampled) > len(entries):
+            block = block[:, :len(entries)].contiguous()
         res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
         hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
@@ -893,6 +937,8 @@ class AmwgSampler(Sampler):
             out["covariance"] = cov
         if loo_out is not None:
             out["loo"] = loo_out
+        if ppc_out is not None:
+            out["ppc"] = ppc_out
         return out
 
     def start_adaptation(self):

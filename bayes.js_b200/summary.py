@@ -261,6 +261,17 @@ class CudaBlockReducer:
                                                    out.ctypes.data))
         return out
 
+    def threshold_counts(self, block, thresholds):
+        """-> torch int64 CUDA tensor [entries, 4]: this shard's draws <, ==, > thresholds[entry] and NaN (amwg_summary_threshold_counts)"""
+        import torch
+        rows, entries, chains = block.shape
+        out = torch.empty((entries, 4), dtype=torch.int64, device=block.device)
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64)
+        torch.cuda.current_stream(block.device).synchronize()
+        self._ffi.check(self.L.amwg_summary_threshold_counts(self.device, block.data_ptr(), rows, entries, chains, thr.ctypes.data,
+                                                             out.data_ptr()))
+        return out
+
     def loo_reduce(self, ll, llmin, llmax, cut, cap: int):
         """-> (sums [P, 3], tails float64 tensor [P, cap], counts int32 tensor [P]) of this shard; see amwg_loo_reduce in include/amwg.h."""
         import torch
@@ -1280,3 +1291,175 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
     out["looic"], out["waic"] = -2.0 * out["elpd_loo"], -2.0 * out["elpd_waic"]
     out.update(pointwise=cols, pareto_k_threshold=float(thr), n_high_k=n_high, r_eff=float(r_eff), n_draws=int(S), points=int(points))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# posterior predictive checks (BDA3 ch. 6; ArviZ's plot_ppc / plot_bpv): DESIGN.md §4.8
+PPC_KEYS = ("log_lik", "points")
+# the families with a sampler, in the order of the family codes of csrc/amwg_ppc.cuh (amwg_ppc_pointwise)
+PPC_FAMILIES = ("norm", "lnorm", "cauchy", "laplace", "logis", "exp", "weibull", "pareto", "unif", "gamma", "invgamma", "beta", "t",
+                "bern", "pois", "binom", "nbinom")
+PPC_STATS = ("mean", "sd", "min", "max")
+MAX_PPC_DRAWS = 1 << 46                # rows x points: the stream region of amwg_ppc_pointwise (2^16 uniforms each below 2^63)
+
+
+class PpcPlan(NamedTuple):
+    """A checked `ppc=` argument."""
+    log_lik: object
+    points: int
+
+
+def resolve_ppc(spec, names: Sequence[str]) -> Optional[PpcPlan]:
+    """Checks the `ppc=` argument of sample_summary: None, or {"log_lik": callable (state, data, i), "points": int >= 1}, with no
+    monitored name "ppc" (the key the result uses). Pure: raises ValueError before any device work (tracing log_lik and
+    check_ppc_call are the caller's next checks)."""
+    if spec is None:
+        return None
+    if not isinstance(spec, dict):
+        raise ValueError("ppc must be None or a dict {\"log_lik\": ..., \"points\": ...}, not %r" % (spec,))
+    unknown = [k for k in spec if k not in PPC_KEYS]
+    if unknown:
+        raise ValueError("ppc has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(PPC_KEYS)))
+    if not callable(spec.get("log_lik")):
+        raise ValueError("ppc needs \"log_lik\": a function (state, data, i) -> one ld.* call at data point i")
+    points = spec.get("points")
+    if not (_is_int(points) and points >= 1):
+        raise ValueError("ppc points must be an int >= 1, not %r" % (points,))
+    if "ppc" in names:
+        raise ValueError("ppc: a monitored parameter or derived quantity is named 'ppc', the key the result would use")
+    return PpcPlan(spec["log_lik"], int(points))
+
+
+def check_ppc_call(family: str, rows: int, points: int) -> int:
+    """-> the family code of amwg_ppc_pointwise, or ValueError for a family without a sampler or rows x points >= 2^46."""
+    if family not in PPC_FAMILIES:
+        raise ValueError("ppc: ld.%s has no sampler; the families are %s" % (family, ", ".join(PPC_FAMILIES)))
+    if rows * points >= MAX_PPC_DRAWS:
+        raise ValueError("ppc: kept rows x points = %d must stay below 2^46" % (rows * points))
+    return PPC_FAMILIES.index(family)
+
+
+def dataset_stats(y) -> np.ndarray:
+    """T(y) = (mean, sd, min, max) of one dataset, the points in index order, with the device's operations: sequential Welford
+    (d = y - m; m += d / j; M2 += d (y - m)), sd = sqrt(M2 / (N - 1)) (NaN for N = 1), min and max propagating NaN."""
+    m = M2 = 0.0
+    mn = mx = float("nan")
+    for j, v in enumerate(np.asarray(y, dtype=np.float64).tolist(), 1):
+        d = v - m
+        m += d / j
+        M2 += d * (v - m)
+        if j == 1:
+            mn = mx = v
+        elif mn != mn or v != v:
+            mn = mx = float("nan")
+        else:
+            mn, mx = (v if v < mn else mn), (v if v > mx else mx)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        sd = float(np.sqrt(np.float64(M2) / np.float64(len(y) - 1)))
+    return np.array([m, sd, mn, mx])
+
+
+def ppc_point_bytes(rows: int, chains: int) -> int:
+    """Device bytes one point of a chunk takes, from the sizes the calls allocate (include/amwg.h): its y_rep column of the chunk,
+    the per-CTA records of amwg_summary_moments (32 G + 32, G = min(ceil(chains / 256), 1184)) and the threshold and counts of
+    amwg_summary_threshold_counts (8 + 32)."""
+    G = min(-(-chains // 256), 1184)
+    return 8 * rows * chains + (32 * G + 32) + 40
+
+
+def ppc_fixed_bytes(rows: int, chains: int) -> int:
+    """Device bytes of the whole call: the statistics records T [rows][4][chains] (32 rows chains) and the scratch of summarising
+    them as a 4-entry block (two entries' worth of chain records, as the base summary's check counts)."""
+    return 32 * rows * chains + 2 * 4 * chains * 8
+
+
+class CudaPpc:
+    """The replicated data of one sample block, in chunks of points: amwg_ppc_pointwise over the handle's data columns. The
+    statistics records live on the device from the first chunk to the last; `stats()` returns them once the last chunk ran."""
+
+    def __init__(self, handle, prog, offsets, family: int, block, points: int):
+        import torch
+        from . import _ffi
+        self.L, self._ffi = _ffi.lib(), _ffi
+        self.h, self.block, self.family, self.points = handle, block, family, points
+        self.code = np.ascontiguousarray(prog.code, dtype=np.int32)
+        self.consts = np.ascontiguousarray(prog.consts if prog.consts else [0.0], dtype=np.float64)
+        self.fold_prog = np.ascontiguousarray(prog.fold_prog if prog.fold_prog else [0], dtype=np.int32)
+        self.fold_dst = np.ascontiguousarray(prog.fold_dst if prog.fold_dst else [0], dtype=np.int32)
+        self.n_fold = len(prog.fold_prog)
+        self.args = np.ascontiguousarray(offsets, dtype=np.int32)
+        rows, _, chains = block.shape
+        self.T = torch.empty((rows, 4, chains), dtype=torch.float64, device=block.device)
+
+    def chunk(self, p0: int, P: int):
+        """-> float64 CUDA tensor [rows, P, chains]: y_rep of points p0 .. p0 + P - 1 at every kept draw of the block (chunks in order)."""
+        import torch
+        rows, entries, chains = self.block.shape
+        out = torch.empty((rows, P, chains), dtype=torch.float64, device=self.block.device)
+        torch.cuda.current_stream(self.block.device).synchronize()
+        i32p = C.POINTER(C.c_int32)
+        self._ffi.check(self.L.amwg_ppc_pointwise(self.h, self.code.ctypes.data_as(i32p), self.code.size,
+                                                  self.consts.ctypes.data_as(C.POINTER(C.c_double)), self.consts.size, self.family,
+                                                  self.args.ctypes.data_as(i32p), self.args.size, self.fold_prog.ctypes.data_as(i32p),
+                                                  self.fold_dst.ctypes.data_as(i32p), self.n_fold, self.block.data_ptr(), rows, entries,
+                                                  self.points, p0, P, out.data_ptr(), self.T.data_ptr()))
+        return out
+
+    def stats(self):
+        """-> the [rows, 4, chains] block of every draw's (mean, sd, min, max), after the last chunk"""
+        return self.T
+
+
+def _pooled_moments(reducer, block, rows: int, distributed: bool):
+    """(mean, sd) per entry over all shards, as summarise_block forms them (finalize_moments of the merged records)"""
+    import torch
+    rec = reducer.moments(block)
+    if distributed:
+        rec = merge_moment_records(list(_gather_tensor(torch.from_numpy(rec).to(block.device), True).cpu().numpy()))
+    mean, sd, _ = finalize_moments(rec, rows)
+    return mean, sd
+
+
+def _counts(reducer, block, thresholds, distributed: bool) -> np.ndarray:
+    """-> int64 [entries, 4] (<, ==, >, NaN) over all shards: integer sums, exact on any number of GPUs"""
+    c = reducer.threshold_counts(block, np.ascontiguousarray(thresholds, dtype=np.float64))
+    if distributed:
+        import torch.distributed as dist
+        dist.all_reduce(c)
+    return c.cpu().numpy().astype(np.int64)
+
+
+def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family: str, y, probs: Sequence[float], chunk_points: int,
+              distributed: bool) -> dict:
+    """-> the "ppc" dict of sample_summary over all shards, for the S = rows x total_chains kept draws. `source.chunk(p0, P)` gives
+    y_rep of points p0 .. p0 + P - 1 as a [rows, P, chains] block (this shard's chains; chunks of at most `chunk_points`, in
+    order), and `source.stats()` after the last chunk the [rows, 4, chains] block of each draw's T(y_rep) = (mean, sd, min,
+    max) (amwg_ppc_pointwise). y: the observed y_0 .. y_{N-1}.
+    pointwise: "mean" and "sd" of y_rep_i over the S draws as the base summary forms them (finalize_moments: pooled, ddof 1),
+    "n_below" / "n_equal" / "n_nan" (int64: y_rep_i < y_i, == y_i, NaN), "pit" = (n_below + n_equal) / S (ArviZ's u-value).
+    stats: per T, "observed" T(y) (dataset_stats), "mean", "sd" and "quantiles" (`probs`) of T(y_rep) from summarise_block,
+    "n_greater", "n_equal", "n_nan" and "p_value" = (n_greater + n_equal) / S, Pr(T(y_rep) >= T(y)) with a NaN draw counted as
+    not >= (and with T(y) NaN, no draw is). Distributed: moment records all-gather and merge in rank order, counts all-reduce,
+    summarise_block takes its distributed path; every rank returns the same numbers."""
+    S = rows * total_chains
+    y = np.ascontiguousarray(y, dtype=np.float64)
+    pw = {"mean": np.empty(points), "sd": np.empty(points)}
+    cnt = np.empty((points, 4), dtype=np.int64)
+    for p0 in range(0, points, chunk_points):
+        P = min(chunk_points, points - p0)
+        yrep = source.chunk(p0, P)
+        sl = slice(p0, p0 + P)
+        pw["mean"][sl], pw["sd"][sl] = _pooled_moments(reducer, yrep, rows, distributed)
+        cnt[sl] = _counts(reducer, yrep, y[sl], distributed)
+        del yrep
+    pw.update(n_below=cnt[:, 0], n_equal=cnt[:, 1], pit=(cnt[:, 0] + cnt[:, 1]) / S, n_nan=cnt[:, 3])
+    T = source.stats()
+    obs = dataset_stats(y)
+    mean, sd, _rhat, q = summarise_block(reducer, T, rows, total_chains, probs, distributed)
+    tc = _counts(reducer, T, obs, distributed)
+    stats = {}
+    for k, name in enumerate(PPC_STATS):
+        stats[name] = {"observed": float(obs[k]), "mean": float(mean[k]), "sd": float(sd[k]), "quantiles": q[:, k].copy(),
+                       "n_greater": int(tc[k, 2]), "n_equal": int(tc[k, 1]), "n_nan": int(tc[k, 3]),
+                       "p_value": float((tc[k, 2] + tc[k, 1]) / S)}
+    return {"family": family, "points": int(points), "n_draws": int(S), "pointwise": pw, "stats": stats}

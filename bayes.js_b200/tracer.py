@@ -1226,6 +1226,13 @@ class LogLik:
         component `off`) becomes entry entry_start[name] + c - off, for COMP and for the base of COMP_I alike (a parameter's
         entries are contiguous in the block). The body is at word 0 and leaves its value on the stack; its constant
         sub-expressions become fold programs (evaluated on the device, amwg_loo_pointwise) with their own constant bank."""
+        prog, _ = self.lower_exprs([self.expr], entry_start)
+        return prog
+
+    def lower_exprs(self, exprs: Sequence[Sym], entry_start: Dict[str, int]) -> Tuple[Program, List[int]]:
+        """Sub-expressions of the body (the parameters of its ld.* call, amwg_ppc_pointwise) lowered as `lower` lowers the body:
+        one END-terminated program each, in order, sharing one constant bank and one set of fold programs. -> (program, the
+        programs' offsets)."""
         def entry(c: int) -> int:
             for name, off, n in self._ranges:
                 if off <= c < off + n:
@@ -1249,17 +1256,37 @@ class LogLik:
             memo[id(n)] = out
             return out
         low = Lowering(self.tracer, 0)
-        low.emit_expr(remap(self.expr))
-        low.prog.emit("END")
+        offs = []
+        for e in exprs:
+            offs.append(len(low.prog.code))
+            low.emit_expr(remap(e))
+            low.prog.emit("END")
         low.prog.logpost_prog = 0
-        return low.finish()
+        return low.finish(), offs
+
+    def observed_call(self, points: int):
+        """The body as a posterior predictive check reads it (sample_summary(..., ppc=...)): one ld.* call whose first argument
+        is a data value at the point index. -> (ld name, the observed values y_0 .. y_{points-1}, the call's other arguments).
+        Raises ValueError for anything else: an expression around the call, or a first argument that is not data[i]."""
+        e = self.expr
+        if not e.op.startswith("LD_"):
+            raise ValueError("ppc: log_lik must return one ld.* call (e.g. ld.norm(data.y[i], mu, sigma)), not %r" % (e,))
+        family = e.op[3:].lower()
+        obs = e.args[0]
+        if obs.op != "DATA_I":
+            raise ValueError("ppc: the first argument of ld.%s must be a data value at the point index (data.y[i]), not %r" % (family, obs))
+        col, off, stride, _pid = obs.val
+        column = np.asarray(self.tracer.columns[col], dtype=np.float64)
+        y = column[off: off + stride * (points - 1) + 1: stride].copy()
+        return family, y, list(e.args[1:])
 
 
-def trace_log_lik(log_lik, params: Dict[str, dict], offsets: Dict[str, int], data, points: int) -> LogLik:
+def trace_log_lik(log_lik, params: Dict[str, dict], offsets: Dict[str, int], data, points: int, what: str = "loo") -> LogLik:
     """Run ``log_lik(state, data, i)`` once with symbolic parameters, proxied data and a symbolic point index i over `points`
     points (``data.y[i]`` -> DATA_I, ``mu[data.g[i]]`` -> COMP_I, as under mcmc.points), with the ld.* / Math rules of log_post.
     Raises ValueError when the closure cannot be traced for the device: it branches on a parameter, reads a data array past its
-    end at some i < points, indexes a parameter with data values outside it, or returns something that is not a number."""
+    end at some i < points, indexes a parameter with data values outside it, or returns something that is not a number. `what`
+    names the argument in the message ("loo", "ppc")."""
     tr = Tracer()
     wrapped = tr.wrap_data(data)
     i = tr.new_plate_index(points)
@@ -1271,7 +1298,7 @@ def trace_log_lik(log_lik, params: Dict[str, dict], offsets: Dict[str, int], dat
             raise JsThrow("log_lik returned undefined")
         expr = lift(result)
     except JsThrow as exc:
-        raise ValueError("loo: log_lik cannot be evaluated on the device: " + exc.message) from None
+        raise ValueError(what + ": log_lik cannot be evaluated on the device: " + exc.message) from None
     finally:
         _ACTIVE.pop()
     ranges = [(name, offsets[name], int(np.prod(p["dim"]))) for name, p in params.items()]

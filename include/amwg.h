@@ -435,6 +435,29 @@ AMWG_API int amwg_loo_reduce(int device, const double* dev_ll, int64_t rows, int
 AMWG_API int amwg_loo_fit(int device, const double* dev_tails, const int32_t* dev_counts, int32_t shards, int32_t points, int32_t tail_cap,
                           const double* host_llmin, const double* host_cut, const int32_t* host_skip, double* host_out);
 
+/* ---- posterior predictive checks (sample_summary(..., ppc=...), DESIGN.md §4.8) -----------------------------------------------
+ * amwg_ppc_pointwise: dev_out[row][p][chain] = a replicated observation y_rep of point p0 + p (p < n_points, of `points` points in
+ *   all) at the kept draw (row, chain) of dev_samples ([rows][entries][chains], chains = the handle's chains), drawn from family
+ *   `family` (csrc/amwg_ppc.cuh: 0 norm, 1 lnorm, 2 cauchy, 3 laplace, 4 logis, 5 exp, 6 weibull, 7 pareto, 8 unif, 9 gamma,
+ *   10 invgamma, 11 beta, 12 t, 13 bern, 14 pois, 15 binom, 16 nbinom) whose n_args parameters are the values of the expression
+ *   programs host_arg_progs[k] at the point (programs, constants and fold programs as amwg_loo_pointwise's, each program leaving
+ *   one value). The draw of (row, point i) for global chain g takes the uniforms #(2^62 + (row points + i) 2^16 + k) of chain g's
+ *   Math.random() stream, keyed by the handle's seed; one needing k >= 2^16, or parameters outside the family's domain, give NaN.
+ *   dev_stats[row][4][chain] carries each draw's running statistics of its replicated dataset over the points in index order
+ *   (Welford mean, M2, min, max; min and max propagate NaN): the call with p0 = 0 starts them, and the call whose chunk ends at
+ *   `points` replaces M2 by sd = sqrt(M2 / (points - 1)), leaving the sample block (mean, sd, min, max). Errors (nothing runs): as
+ *   amwg_loo_pointwise, an unknown family, n_args not the family's parameter count, p0 + n_points > points, rows x points >= 2^46.
+ * amwg_summary_threshold_counts: dev_counts[entry][4] (int64, overwritten) = the draws of each entry of a sample block
+ *   [rows][entries][chains] that are < host_thresholds[entry], ==, >, and NaN; exact and independent of order. Errors: an empty
+ *   block, entries > 65535, null pointers.
+ * Device scratch, from the pool of the LOO calls: the programs (pointwise), 8 entries bytes (counts). */
+AMWG_API int amwg_ppc_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
+                                int32_t family, const int32_t* host_arg_progs, int32_t n_args, const int32_t* host_fold_prog,
+                                const int32_t* host_fold_dst, int32_t n_fold, const double* dev_samples, int64_t rows, int32_t entries,
+                                int64_t points, int64_t p0, int32_t n_points, double* dev_out, double* dev_stats);
+AMWG_API int amwg_summary_threshold_counts(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                           const double* host_thresholds, int64_t* dev_counts);
+
 /* ---- run-time specialisation ----------------------------------------------------------------------------------------------
  * For models that run the statistics sweep (stat_prog) amwg_create generates CUDA source from the model's programs, compiles it
  * for sm_90a with NVRTC and steps with that kernel instead of the bytecode interpreter (csrc/amwg_jit.cuh; AMWG_JIT=0 in the

@@ -571,6 +571,32 @@ BINDING(loo_fit)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// ppc_pointwise(handle, code [n], consts [k], family, arg_progs [K], fold_prog [f], fold_dst [f], samples ptr, rows, entries, points,
+//               p0, n_points, out ptr, stats ptr)                                                           amwg_ppc_pointwise
+BINDING(ppc_pointwise)
+  Handle* h = handle_of(env, a.at(0));
+  const std::vector<int32_t> code = ints(env, a.at(1)), ap = ints(env, a.at(4)), fp = ints(env, a.at(5)), fd = ints(env, a.at(6));
+  const std::vector<double> consts = doubles(env, a.at(2));
+  if (fp.size() != fd.size()) throw Throw{"ppc_pointwise: fold_prog and fold_dst must have the same length"};
+  if (amwg_ppc_pointwise(h->s, code.data(), (int32_t)code.size(), consts.data(), (int32_t)consts.size(), (int32_t)to_double(env, a.at(3)),
+                         ap.data(), (int32_t)ap.size(), fp.data(), fd.data(), (int32_t)fp.size(), (const double*)(uintptr_t)to_u64(env, a.at(7)),
+                         (int64_t)to_double(env, a.at(8)), (int32_t)to_double(env, a.at(9)), (int64_t)to_double(env, a.at(10)),
+                         (int64_t)to_double(env, a.at(11)), (int32_t)to_double(env, a.at(12)), (double*)(uintptr_t)to_u64(env, a.at(13)),
+                         (double*)(uintptr_t)to_u64(env, a.at(14))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
+// summary_threshold_counts(device, samples ptr, rows, entries, chains, thresholds [entries], counts ptr)
+//                                                                                              amwg_summary_threshold_counts
+BINDING(summary_threshold_counts)
+  const int32_t entries = (int32_t)to_double(env, a.at(3));
+  const std::vector<double> thr = doubles(env, a.at(5));
+  if (entries < 0 || thr.size() != (size_t)entries) throw Throw{"summary_threshold_counts: thresholds must hold one number per entry"};
+  if (amwg_summary_threshold_counts((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                                    entries, (int64_t)to_double(env, a.at(4)), thr.data(), (int64_t*)(uintptr_t)to_u64(env, a.at(6))) != 0)
+    fail_from_library();
+  return js_undefined(env);
+END_BINDING
 // term_cache(handle, n_terms) -> Float64Array [n_terms][chains] (empty without a cache) amwg_get_term_cache
 BINDING(term_cache)
   Handle* h = handle_of(env, a.at(0));
@@ -606,6 +632,7 @@ NAPI_MODULE_INIT() {
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
       {"summary_comoments", summary_comoments}, {"summary_nested", summary_nested},
       {"loo_pointwise", loo_pointwise}, {"loo_reduce", loo_reduce}, {"loo_fit", loo_fit},
+      {"ppc_pointwise", ppc_pointwise}, {"summary_threshold_counts", summary_threshold_counts},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
   for (const auto& e : table) {
