@@ -49,25 +49,32 @@ __host__ __device__ inline double smoothed(int j, int n, double k, double sigma,
   return v > 0.0 ? 0.0 : v;
 }
 
-// weight of candidate j from the m profile values L: 1 / sum_l exp(L_l - L_j), or 0 when below 10 eps (dropped)
+// weight of candidate j from the m profile values L: 1 / sum_l exp(L_l - L_j) over the candidates whose L is finite, or 0 when
+// L_j is not finite or the weight is below 10 eps (dropped). A candidate b of exactly 0 (a tied tail, where 1 - sqrt(m / (j - 0.5))
+// = -3 meets x_q = x_max) has k(b) = 0 and L = NaN; x_q = 0 makes every b infinite and every L NaN. ArviZ lets such an L poison
+// every weight; leaving it out keeps the fit of the other candidates (DESIGN.md §4.7).
 __host__ __device__ inline double fit_weight(const double* L, int m, int j) {
+  if (!(L[j] - L[j] == 0.0)) return 0.0;                       // NaN or infinite
   double s = 0.0;
-  for (int l = 0; l < m; ++l) s += exp(L[l] - L[j]);
+  for (int l = 0; l < m; ++l)
+    if (L[l] - L[l] == 0.0) s += exp(L[l] - L[j]);
   const double w = 1.0 / s;
   return w >= 10.0 * kEps ? w : 0.0;
 }
 
-// the weighted mean of the candidates b with the kept weights w normalised to sum 1
+// the weighted mean of the candidates b with the kept weights w normalised to sum 1; NaN when no candidate is kept (every L
+// non-finite), which the fit reports as k = +inf: the tail keeps its raw weights, as a tail of at most 4 draws does
 __host__ __device__ inline double fit_b_post(const double* b, const double* w, int m) {
   double tot = 0.0;
   for (int j = 0; j < m; ++j) tot += w[j];
+  if (!(tot > 0.0)) return NAN;
   double bp = 0.0;
   for (int j = 0; j < m; ++j) bp += b[j] * (w[j] / tot);
   return bp;
 }
 
 // The whole fit over the n ascending values x (n >= 5), sequential sums; b, L, w: scratch of fit_m(n) doubles each.
-// -> k (with the prior) and sigma.
+// -> k (with the prior; +inf when no candidate has a finite profile value) and sigma (NaN then).
 __host__ __device__ inline void loo_fit_seq(const double* x, int n, double* b, double* L, double* w, double* k_out, double* sigma_out) {
   const int m = fit_m(n);
   const double xq = x[fit_quartile(n)], xmax = x[n - 1];
@@ -79,6 +86,7 @@ __host__ __device__ inline void loo_fit_seq(const double* x, int n, double* b, d
   }
   for (int j = 0; j < m; ++j) w[j] = fit_weight(L, m, j);
   const double bp = fit_b_post(b, w, m);
+  if (bp != bp) { *k_out = INFINITY; *sigma_out = NAN; return; }
   double s = 0.0;
   for (int i = 0; i < n; ++i) s += fit_term(bp, x[i]);
   const double k = s / (double)n;

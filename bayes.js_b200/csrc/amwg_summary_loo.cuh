@@ -101,7 +101,8 @@ __global__ void __launch_bounds__(256) amwg_loo_reduce_kernel(const double* __re
 }
 
 // K_l3. One CTA per point. tails[shard][point][cap] with counts[shard][point]; work and xs: [point][cap] scratch, cap a power of two.
-// out[point][4] = { k (+inf for a tail of <= 4 draws, NaN for a skipped point), sum exp(lw), sum exp(lw + ll - llmin) over the
+// out[point][4] = { k (+inf for a tail of <= 4 draws or one where no candidate of the fit has a finite profile value, NaN for a
+// skipped point), sum exp(lw), sum exp(lw + ll - llmin) over the
 // tail with lw smoothed when k is finite, the number of tail draws over all shards }.
 __global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double* __restrict__ tails, const int* __restrict__ counts, int shards,
                                                                    int P, int cap, const double* __restrict__ llmin, const double* __restrict__ cut,
@@ -161,11 +162,13 @@ __global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double*
     if (t == 0) s_bp = loo::fit_b_post(sb, sw, m);
     __syncthreads();
     const double bp = s_bp;
-    double s = 0.0;
-    for (int i = t; i < n; i += T) s += loo::fit_term(bp, xp[i]);
-    const double kh = cta_sum<kFitThreads>(sh, s) / (double)n;
-    sigma = -kh / bp;
-    k = loo::fit_prior_k(kh, n);
+    if (bp == bp) {                                           // NaN: no candidate with a finite profile value, k stays +inf
+      double s = 0.0;
+      for (int i = t; i < n; i += T) s += loo::fit_term(bp, xp[i]);
+      const double kh = cta_sum<kFitThreads>(sh, s) / (double)n;
+      sigma = -kh / bp;
+      k = loo::fit_prior_k(kh, n);
+    }
   }
   const bool smooth = isfinite(k);
   double s_w = 0.0, s_wl = 0.0;

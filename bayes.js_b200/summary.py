@@ -1239,7 +1239,7 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
       p_waic_i    = var_s ll (ddof 0),  elpd_waic_i = lppd_i - p_waic_i
       elpd_loo_i  = llmin + log(sum exp(lw' + ll - llmin)) - log(sum exp(lw')), lw' the smoothed log weights
                     (logsumexp(lw' - logsumexp(lw') + ll)),  p_loo_i = lppd_i - elpd_loo_i
-      pareto_k_i  the fitted k (+inf for a tail of <= 4 draws)
+      pareto_k_i  the fitted k (+inf for a tail of <= 4 draws, or when no candidate of the fit has a finite profile value)
     A point with any non-finite ll gets NaN in every value. Totals: sums of the pointwise values, se_* = sqrt(points var_i(elpd_*_i))
     (ddof 0), looic = -2 elpd_loo, waic = -2 elpd_waic, pareto_k_threshold = min(1 - 1 / log10 S, 0.7), n_high_k = #{k > threshold}.
     Distributed: extremes and counts all-reduce, moment records all-gather and merge in rank order, the select's counts

@@ -421,8 +421,8 @@ AMWG_API int amwg_summary_nested(int device, const double* dev_samples, int64_t 
  * amwg_loo_fit: one CTA per point gathers the tails dev_tails[shard][point][tail_cap] (dev_counts[shard][point] values each),
  *   sorts them and fits a generalised Pareto to the ascending exp(lw) - exp(cut), lw = llmin - ll (Zhang & Stephens 2009 with
  *   the prior on k; csrc/amwg_loo.cuh). host_out[point][4] = { k, sum exp(lw), sum exp((lw + ll) - llmin) over the tail with lw
- *   replaced by the smoothed weights when k is finite, the tail draws over all shards }; a tail of <= 4 draws gives k = +inf and
- *   raw weights; host_skip[point] != 0 gives NaN. Deterministic. Errors: tail_cap not a power of two in 8..2^20, shards or points
+ *   replaced by the smoothed weights when k is finite, the tail draws over all shards }; a tail of <= 4 draws, or one where no
+ *   candidate of the fit has a finite profile value, gives k = +inf and raw weights; host_skip[point] != 0 gives NaN. Deterministic. Errors: tail_cap not a power of two in 8..2^20, shards or points
  *   < 1, null pointers.
  * Device scratch of the three calls, from one per-device pool grown on demand: the program (pointwise), 3 x 8 points + 24 points
  *   G (G = min(ceil(chains / 256), 1184)) bytes (reduce), 3 x 8 points + 16 points tail_cap + 32 points bytes (fit). */

@@ -15,6 +15,11 @@ void hs_loo_fit(const double* x, int n, double* out) {
   loo::loo_fit_seq(x, n, b.data(), L.data(), w.data(), &out[0], &out[1]);
 }
 
+// the candidate count of a tail of n, and the limits the fit kernel's arrays are sized by
+int hs_loo_fit_m(int n) { return loo::fit_m(n); }
+int hs_loo_max_tail() { return loo::kMaxTail; }
+int hs_loo_max_m() { return loo::kMaxM; }
+
 // out[j] = the smoothed log weight of the j-th smallest of n tail draws, j < n
 void hs_loo_smoothed(int n, double k, double sigma, double expcut, double* out) {
   for (int j = 0; j < n; ++j) out[j] = loo::smoothed(j, n, k, sigma, expcut);

@@ -10,15 +10,28 @@ EPS = np.finfo(float).eps
 LOG_TINY = np.log(np.finfo(float).tiny)
 
 
-def gpdfit(x):
-    """Zhang & Stephens (2009) with the weakly informative prior on k (prior_bs = 3, prior_k = 10); x ascending. -> (k, sigma)."""
+BLOCK_ELEMENTS = 1 << 24              # gpdfit's candidate matrix is formed in row blocks of at most this many elements
+
+
+def gpdfit(x, block=None):
+    """Zhang & Stephens (2009) with the weakly informative prior on k (prior_bs = 3, prior_k = 10); x ascending. -> (k, sigma).
+    Candidates whose profile value L is not finite are left out (a b of exactly 0 in a tied tail, or every b infinite when a
+    quarter of x is 0); ArviZ keeps them and gets NaN weights. With none left: (inf, nan), the tail is not smoothed.
+    k(b) is the mean of log1p(-b x) over a [rows, n] block of candidates at a time: `block` rows (default: as many as keep the
+    block within BLOCK_ELEMENTS), so n = 2^20 does not need the m x n matrix (8.8 GB)."""
     n = len(x)
     m = 30 + int(n ** 0.5)
     b = 1 - np.sqrt(m / (np.arange(1, m + 1, dtype=float) - 0.5))
     b /= 3 * x[int(n / 4 + 0.5) - 1]
     b += 1 / x[-1]
-    k = np.log1p(-b[:, None] * x).mean(axis=1)
-    L = n * (np.log(-(b / k)) - k - 1)
+    rows = block or max(1, BLOCK_ELEMENTS // n)
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        k = np.concatenate([np.log1p(-b[j:j + rows, None] * x).mean(axis=1) for j in range(0, m, rows)])
+        L = n * (np.log(-(b / k)) - k - 1)
+    fin = np.isfinite(L)
+    if not fin.any():
+        return np.inf, np.nan
+    b, L = b[fin], L[fin]
     w = 1 / np.exp(L - L[:, None]).sum(axis=1)
     keep = w >= 10 * EPS
     w, b = w[keep], b[keep]

@@ -2,7 +2,8 @@
 restatement of tests/ppc_ref.py at every kept draw, bit for bit, for every family; the config-2 model's whole "ppc" dict against the
 restatement on an identically seeded twin's draws; every other key and the chains' state unchanged by the option, alone and with
 loo=; the dict independent of where the block holds the parameters; calibration on a conjugate Normal model; a misfit detected;
-and 10^6 device draws per family against scipy.stats."""
+10^6 device draws per sampler regime against scipy.stats and 2000 of them bit for bit; an out-of-domain body, NaN throughout; the
+dict byte-equal over chunks of points; and the threshold counts on an adversarial block against numpy."""
 import ctypes as C
 
 import numpy as np
@@ -18,21 +19,32 @@ from test_summary_ppc_host import REGIMES, distribution_p
 pytestmark = pytest.mark.gpu
 
 
-def _replicated(s, log_lik, points, n):
-    """-> (block [rows, entries, chains] of every component's draws, y_rep [rows, points, chains], T [rows, 4, chains]) of the next
-    n sweeps, formed by the library's kernel on the sampled block (entries = the components in order)."""
+def _sample_block(s, n):
+    """-> the device block [n, entries, chains] of every component's draws over the next n sweeps (entries = the components in order)"""
     from bayes_js_b200 import _ffi
-    from bayes_js_b200.summary import PPC_FAMILIES, CudaPpc
-    from bayes_js_b200.tracer import trace_log_lik
     entries = list(range(s.n_comp))
     block = torch.empty((n, len(entries), s.local_chains), dtype=torch.float64, device="cuda:%d" % s.device)
     mon = np.asarray(entries, dtype=np.int32)
     torch.cuda.synchronize()
     _ffi.check(_ffi.lib().amwg_sample_device(s._handle, n, 1, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(entries), block.data_ptr()))
+    return block
+
+
+def _ppc_source(s, log_lik, points, block):
+    """-> (family, observed y, a function giving a fresh CudaPpc over `block`): the library's replicated data of the traced body"""
+    from bayes_js_b200.summary import PPC_FAMILIES, CudaPpc
+    from bayes_js_b200.tracer import trace_log_lik
     lik = trace_log_lik(log_lik, s.params, s._offsets, s.data, points, what="ppc")
     fam, y, args = lik.observed_call(points)
     prog, offs = lik.lower_exprs(args, {name: s._offsets[name] for name in lik.reads})
-    src = CudaPpc(s._handle, prog, offs, PPC_FAMILIES.index(fam), block, points)
+    return fam, y, lambda: CudaPpc(s._handle, prog, offs, PPC_FAMILIES.index(fam), block, points)
+
+
+def _replicated(s, log_lik, points, n):
+    """-> (block [rows, entries, chains] of every component's draws, y_rep [rows, points, chains], T [rows, 4, chains]) of the next
+    n sweeps, formed by the library's kernel on the sampled block (entries = the components in order)."""
+    block = _sample_block(s, n)
+    src = _ppc_source(s, log_lik, points, block)[2]()
     yrep = src.chunk(0, points).cpu().numpy()
     return block.cpu().numpy(), yrep, src.stats().cpu().numpy()
 
@@ -189,16 +201,88 @@ def test_a_normal_fitted_to_heavy_tailed_data_fails_the_max_check(gpu_pkg):
     assert out["stats"]["max"]["p_value"] < 0.01, out["stats"]["max"]
 
 
-def test_device_draws_follow_the_distribution(gpu_pkg):
+def test_device_draws_follow_the_distribution(gpu_pkg, orc):
+    """10^6 device draws per regime against scipy, and 2000 of them bit for bit against the restatement"""
     mcmc, ld = gpu_pkg.mcmc, gpu_pkg.ld
+    O = orc.lib()
     N = 1000
     s = mcmc.AmwgSampler({"mu": {"type": "real"}}, lambda t, d: ld.norm(t.mu, 0, 1), {"y": [0.0] * N}, {"chains": 1000, "seed": 2})
     s.burn(10)
     fn = {"dexp": "laplace"}
+    rng = np.random.default_rng(3)
     for fam, p in REGIMES:
         call = getattr(ld, fam)
         f = (lambda call, p: lambda t, d, i: call(d.y[i], *p))(call, p)
         _, yrep, _ = _replicated(s, f, N, 1)
+        for _ in range(2000):
+            c, i = int(rng.integers(1000)), int(rng.integers(N))
+            want, _ = ppc_ref.draw_at(O, fn.get(fam, fam), tuple(float(v) for v in p), 2, c, 0, N, i)
+            assert np.float64(yrep[0, i, c]).tobytes() == np.float64(want).tobytes(), (fam, p, c, i, yrep[0, i, c], want)
         x = yrep.ravel()
         assert x.size == 10 ** 6 and np.all(np.isfinite(x)), fam
         assert distribution_p(x, fn.get(fam, fam), p) > 1e-3, (fam, p)
+
+
+def test_out_of_domain_parameters_give_nan_everywhere(gpu_pkg):
+    """ld.norm with sd = -1: every y_rep is NaN, so no draw is below, equal to or above y_i (pit 0), every dataset statistic of a
+    draw is NaN, no draw counts as >= T(y) (p-values 0) and the summaries of T(y_rep) are NaN"""
+    mcmc, ld = gpu_pkg.mcmc, gpu_pkg.ld
+    y = [0.5, -1.0, 2.0, 3.25, 0.0]
+    mk = lambda: mcmc.AmwgSampler({"mu": {"type": "real"}}, lambda t, d: ld.norm(t.mu, 0, 1), {"y": y}, {"chains": 300, "seed": 6})
+    a, b = mk(), mk()
+    a.burn(20); b.burn(20)
+    f = lambda t, d, i: ld.norm(d.y[i], 0, -1)
+    out = a.sample_summary(4, probs=(0.1, 0.5), ppc={"log_lik": f, "points": len(y)})["ppc"]
+    _, yrep, T = _replicated(b, f, len(y), 4)
+    assert np.all(np.isnan(yrep)) and np.all(np.isnan(T))
+    S = 4 * 300
+    pw = out["pointwise"]
+    assert out["n_draws"] == S and np.all(pw["n_nan"] == S) and np.all(pw["n_below"] == 0) and np.all(pw["n_equal"] == 0)
+    assert np.all(pw["pit"] == 0) and np.all(np.isnan(pw["mean"])) and np.all(np.isnan(pw["sd"]))
+    obs = ppc_ref.dataset_stats(y)
+    for k, name in enumerate(ppc_ref.STATS):
+        st_ = out["stats"][name]
+        assert st_["observed"] == obs[k] and st_["n_nan"] == S and st_["n_greater"] == 0 and st_["n_equal"] == 0, name
+        assert st_["p_value"] == 0 and np.isnan(st_["mean"]) and np.isnan(st_["sd"]) and np.all(np.isnan(st_["quantiles"])), name
+
+
+def test_chunks_of_points_give_the_same_bytes(gpu_pkg):
+    """ppc_block over chunks of 1, 7 and all N points: the draws' Welford records carry across chunks on the device, so the whole
+    dict keeps its bytes"""
+    from bayes_js_b200.summary import CudaBlockReducer, ppc_block
+    mcmc, ld = gpu_pkg.mcmc, gpu_pkg.ld
+    params = {"mu": {"type": "real"}, "sigma": {"type": "real", "lower": 0}}
+    data = config2_data()[:60]
+    s = mcmc.AmwgSampler(params, models.norm_post_readme(ld), data.tolist(), {"chains": 3000, "seed": 19})
+    s.burn(300)
+    rows, N = 5, len(data)
+    block = _sample_block(s, rows)
+    fam, y, fresh = _ppc_source(s, lambda t, d, i: ld.norm(d[i], t.mu, t.sigma), N, block)
+    outs = [ppc_block(CudaBlockReducer(0), fresh(), rows, 3000, N, fam, y, (0.05, 0.5, 0.95), chunk, False) for chunk in (N, 1, 7)]
+    assert np.isfinite(outs[0]["stats"]["sd"]["mean"])
+    for other in outs[1:]:
+        assert _same(outs[0], other)
+
+
+def test_threshold_counts_on_an_adversarial_block(gpu_pkg):
+    """amwg_summary_threshold_counts over draws and thresholds from both zeros, subnormals, infinities and NaN of both signs, at
+    (rows, chains) of (1, 1), (7, 255) and (3, 1184 x 256 + 77), and at 65535 entries: numpy's <, ==, > and isnan, count for count"""
+    from bayes_js_b200.summary import CudaBlockReducer
+    from test_gpu_summary_hist import _pool
+    red = CudaBlockReducer(0)
+    rng = np.random.default_rng(73)
+    pool = np.concatenate([_pool(-1.0, 1.0, (7, 64), rng), [-np.nan, np.copysign(np.nan, -1.0)]])
+    assert np.signbit(pool[np.isnan(pool)]).any() and not np.signbit(pool[np.isnan(pool)]).all()
+
+    def check(x, thr):
+        got = red.threshold_counts(torch.from_numpy(x).to("cuda:0"), thr).cpu().numpy()
+        t = thr[None, :, None]
+        want = np.stack([(x < t).sum(axis=(0, 2)), (x == t).sum(axis=(0, 2)), (x > t).sum(axis=(0, 2)), np.isnan(x).sum(axis=(0, 2))], axis=1)
+        assert got.dtype == np.int64 and np.array_equal(got, want), (x.shape, np.flatnonzero((got != want).any(axis=1))[:5])
+
+    special = np.array([np.nan, np.inf, -np.inf, -0.0, 0.0, 5e-324, -1e-310])
+    for rows, chains in ((1, 1), (7, 255), (3, 1184 * 256 + 77)):
+        thr = np.concatenate([special, rng.choice(pool, 9)])
+        check(rng.choice(pool, size=(rows, len(thr), chains)), thr)
+    thr = rng.choice(np.concatenate([pool, special]), 65535)
+    check(rng.choice(pool, size=(1, 65535, 3)), thr)

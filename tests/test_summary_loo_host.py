@@ -35,6 +35,10 @@ def _load(path):
     lib.hs_loo_fit.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     lib.hs_loo_smoothed.restype = None
     lib.hs_loo_smoothed.argtypes = [C.c_int, C.c_double, C.c_double, C.c_double, C.c_void_p]
+    lib.hs_loo_fit_m.restype = C.c_int
+    lib.hs_loo_fit_m.argtypes = [C.c_int]
+    lib.hs_loo_max_tail.restype = C.c_int
+    lib.hs_loo_max_m.restype = C.c_int
     return lib
 
 
@@ -173,91 +177,177 @@ def _normal_ll(rows, chains, y, seed, df=None):
     return -0.5 * np.log(2 * np.pi) - np.log(sd) - (yy - mu) ** 2 / (2 * sd * sd)
 
 
-def test_well_behaved_model(H):
-    y = np.random.default_rng(1).normal(3.0, 2.0, 30)
-    ll3 = _normal_ll(4, 500, y, 2)
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
-    assert np.all(np.isfinite(out["pointwise"]["pareto_k"]))
+# ---- the ll matrices of the cases: one list, which tests/test_gpu_summary_loo_reduce.py runs through the device reductions ----
+def case_well_behaved():
+    return _normal_ll(4, 500, np.random.default_rng(1).normal(3.0, 2.0, 30), 2)
 
 
-def test_heavy_tailed_point(H):
+def case_heavy_tailed():
     y = np.random.default_rng(3).normal(0.0, 1.0, 12)
     y[5] = 9.0                                                     # an outlier: its leave-one-out weights have a heavy tail
-    ll3 = _normal_ll(2, 2000, y, 4)
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
-    assert out["pointwise"]["pareto_k"][5] > 0.7 and out["n_high_k"] >= 1
+    return _normal_ll(2, 2000, y, 4)
 
 
-def test_small_sample_where_the_tail_is_a_fifth(H):
-    ll3 = _normal_ll(2, 60, np.random.default_rng(5).normal(0, 1, 7), 6)         # S = 120: 0.2 S = 24 < 3 sqrt(S) = 32.9
-    assert 0.2 * 120 < 3 * math.sqrt(120)
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
+def case_small_sample():
+    return _normal_ll(2, 60, np.random.default_rng(5).normal(0, 1, 7), 6)        # S = 120: 0.2 S = 24 < 3 sqrt(S) = 32.9
 
 
-def test_tied_ll_of_discrete_data(H):
+def case_tied_discrete():
     rng = np.random.default_rng(7)
     theta = rng.choice([0.2, 0.35, 0.5, 0.65], size=(3, 1, 400))               # few distinct draws: ll ties everywhere
     y = rng.integers(0, 2, 15).astype(float)[None, :, None]
-    ll3 = np.log(y * theta + (1 - y) * (1 - theta))
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
+    return np.log(y * theta + (1 - y) * (1 - theta))
 
 
-def test_tail_of_at_most_four_draws(H):
-    ll3 = _normal_ll(1, 20, np.random.default_rng(8).normal(0, 1, 5), 9)         # S = 20: M = 4
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
-    assert np.all(np.isinf(out["pointwise"]["pareto_k"]))
+def case_tail_of_four():
+    return _normal_ll(1, 20, np.random.default_rng(8).normal(0, 1, 5), 9)        # S = 20: M = 4
 
 
-def test_log_dbl_min_floor(H):
+def case_dbl_min_floor():
     rng = np.random.default_rng(10)
     S, N = 1000, 3
     ll = rng.normal(0.0, 1.0, size=(S, N))
     ll[:50] -= 1000.0                                              # 50 draws far below: the 96th largest lw is under log(DBL_MIN)
-    ll3 = ll.reshape(1, S, N).transpose(0, 2, 1).copy()
-    ref = loo_ref.loo(ll)
-    assert all(loo_ref.psis_point(ll[:, i])["cut"] == loo_ref.LOG_TINY for i in range(N))
-    out, red = run_loo(H, ll3)
-    assert_matches(out, ref, red, ll)
+    return ll.reshape(1, S, N).transpose(0, 2, 1).copy()
 
 
-def test_non_finite_point(H):
+def case_non_finite():
     ll3 = _normal_ll(2, 100, np.random.default_rng(11).normal(0, 1, 6), 12)
     ll3[1, 2, 17] = -np.inf
     ll3[0, 4, 3] = np.nan
-    out, red = run_loo(H, ll3)
-    ref = loo_ref.loo(_flat(ll3))
+    return ll3
+
+
+def case_forced_chunks():
+    return _normal_ll(3, 150, np.random.default_rng(13).normal(1, 2, 11), 14)
+
+
+def case_r_eff():
+    return _normal_ll(2, 300, np.random.default_rng(15).normal(0, 1, 4), 16)
+
+
+def case_two_valued(rows, chains, c, seed):
+    """the ll of a binary observation: log 0.2 at c draws (the rarer state) and log 0.8 at the others, and the mirror point.
+    With c <= M the first point's tail is exactly the c tied draws."""
+    S = rows * chains
+    low = np.zeros(S, dtype=bool)
+    low[np.random.default_rng(seed).choice(S, c, replace=False)] = True
+    ll = np.stack([np.where(low, np.log(0.2), np.log(0.8)), np.where(low, np.log(0.8), np.log(0.2))], axis=1)
+    return ll.reshape(rows, chains, 2).transpose(0, 2, 1).copy()
+
+
+def case_zero_x_quarter():
+    """a tail of M = 269 (S = 8000) whose 100 smallest lw sit within 1e-19 of the cut: exp(lw) - exp(cut) rounds to 0 for them,
+    so the fit's first quartile x_q is 0 and every candidate b is infinite"""
+    rng = np.random.default_rng(21)
+    S, M = 8000, 269
+    ll = np.full(S, -1e-5)                                         # the bulk: lw = cut exactly (llmin - ll, exact by Sterbenz)
+    ll[:100] = -1e-5 - np.arange(1, 101) * 2e-21                   # a hair below the bulk: lw a hair above the cut
+    ll[100:M - 1] = rng.uniform(-2e-5, -1.1e-5, M - 101)
+    ll[M - 1] = -2e-5                                              # llmin
+    ll = ll[rng.permutation(S)]
+    return np.stack([ll, ll[::-1]], axis=1).reshape(2, 4000, 2).transpose(0, 2, 1).copy()
+
+
+# name -> (builder of ll3 [rows, points, chains], r_eff)
+CASES = {
+    "well_behaved": (case_well_behaved, 1.0),
+    "heavy_tailed": (case_heavy_tailed, 1.0),
+    "small_sample": (case_small_sample, 1.0),
+    "tied_discrete": (case_tied_discrete, 1.0),
+    "tail_of_four": (case_tail_of_four, 1.0),
+    "dbl_min_floor": (case_dbl_min_floor, 1.0),
+    "non_finite": (case_non_finite, 1.0),
+    "forced_chunks": (case_forced_chunks, 1.0),
+    "r_eff": (case_r_eff, 0.3),
+    "two_valued_c60": (lambda: case_two_valued(2, 4000, 60, 22), 1.0),      # S = 8000, M = 269: a tail of 60 tied draws
+    "two_valued_c110": (lambda: case_two_valued(2, 4000, 110, 23), 1.0),    # a tail of 110: candidate 3 of m = 40 has b = 0
+    "two_valued_c700": (lambda: case_two_valued(3, 20000, 700, 24), 1.0),   # S = 60000, M = 735: a tail of 700, b_4 of 56 = 0
+    "zero_x_quarter": (case_zero_x_quarter, 1.0),
+}
+
+
+def run_case(H, name, chunk=None):
+    build, r_eff = CASES[name]
+    ll3 = build()
+    out, red = run_loo(H, ll3, r_eff, chunk)
+    ref = loo_ref.loo(_flat(ll3), r_eff)
     assert_matches(out, ref, red, _flat(ll3))
+    return out, ref, ll3
+
+
+def test_well_behaved_model(H):
+    out, _, _ = run_case(H, "well_behaved")
+    assert np.all(np.isfinite(out["pointwise"]["pareto_k"]))
+
+
+def test_heavy_tailed_point(H):
+    out, _, _ = run_case(H, "heavy_tailed")
+    assert out["pointwise"]["pareto_k"][5] > 0.7 and out["n_high_k"] >= 1
+
+
+def test_small_sample_where_the_tail_is_a_fifth(H):
+    assert 0.2 * 120 < 3 * math.sqrt(120)
+    run_case(H, "small_sample")
+
+
+def test_tied_ll_of_discrete_data(H):
+    run_case(H, "tied_discrete")
+
+
+def test_tail_of_at_most_four_draws(H):
+    out, _, _ = run_case(H, "tail_of_four")
+    assert np.all(np.isinf(out["pointwise"]["pareto_k"]))
+
+
+def test_log_dbl_min_floor(H):
+    ll = _flat(case_dbl_min_floor())
+    assert all(loo_ref.psis_point(ll[:, i])["cut"] == loo_ref.LOG_TINY for i in range(ll.shape[1]))
+    run_case(H, "dbl_min_floor")
+
+
+def test_non_finite_point(H):
+    out, _, _ = run_case(H, "non_finite")
     for key, v in out["pointwise"].items():
         assert np.isnan(v[2]) and np.isnan(v[4]) and not np.isnan(v[0]), key
     assert np.isnan(out["elpd_loo"]) and np.isnan(out["waic"])
 
 
 def test_several_forced_chunks(H):
-    ll3 = _normal_ll(3, 150, np.random.default_rng(13).normal(1, 2, 11), 14)
+    ll3 = case_forced_chunks()
     one, _ = run_loo(H, ll3)
-    out, red = run_loo(H, ll3, chunk=3)
-    ref = loo_ref.loo(_flat(ll3))
-    assert_matches(out, ref, red, _flat(ll3))
+    out, _, _ = run_case(H, "forced_chunks", chunk=3)
     for key in one["pointwise"]:
         assert np.array_equal(one["pointwise"][key], out["pointwise"][key]), key
 
 
 def test_r_eff_moves_the_tail(H):
-    ll3 = _normal_ll(2, 300, np.random.default_rng(15).normal(0, 1, 4), 16)
-    out, red = run_loo(H, ll3, r_eff=0.3)
-    ref = loo_ref.loo(_flat(ll3), r_eff=0.3)
-    assert_matches(out, ref, red, _flat(ll3))
+    out, _, _ = run_case(H, "r_eff")
     assert out["r_eff"] == 0.3
+
+
+@pytest.mark.parametrize("name, c", [("two_valued_c60", 60), ("two_valued_c110", 110), ("two_valued_c700", 700)])
+def test_tied_tail_of_a_binary_observation(H, name, c):
+    """the rarer state's c <= M draws are the whole tail, all tied. At c = 110 and 700 one candidate b is 0 and its profile value
+    NaN; left out, the fit stays finite, continuous with the tails around it, and so does every value of the point"""
+    out, ref, ll3 = run_case(H, name)
+    assert len(ref["tails"][0]) == c and ref["tails"][1].size == 0
+    k = out["pointwise"]["pareto_k"][0]
+    assert np.isfinite(k) and k < -5, k
+    assert all(np.isfinite(v[0]) for v in out["pointwise"].values()) and np.isfinite(out["elpd_loo"])
+    assert np.isinf(out["pointwise"]["pareto_k"][1])                  # the mirror point: an empty tail
+
+
+def test_tail_whose_first_quartile_rounds_to_zero(H):
+    """x = exp(lw) - exp(cut) is 0 for more than a quarter of the tail: every candidate is infinite, no profile value is finite,
+    and the point keeps its raw weights with k = +inf (counted as high k), its other values finite"""
+    out, ref, ll3 = run_case(H, "zero_x_quarter")
+    ll = _flat(ll3)
+    r = loo_ref.psis_point(ll[:, 0])
+    x = np.exp(np.sort((ll[:, 0].min() - ll[:, 0])[r["tail"]])) - np.exp(r["cut"])
+    assert len(x) == 269 and np.sum(x == 0) >= len(x) / 4 and x[int(len(x) / 4 + 0.5) - 1] == 0
+    assert np.all(np.isinf(out["pointwise"]["pareto_k"])) and out["n_high_k"] == 2
+    assert np.isfinite(out["elpd_loo"])
 
 
 # ---- the header's fit and smoothing ----------------------------------------------------------------------------------------------
@@ -273,6 +363,42 @@ def test_fit_and_smoothing_equal_the_restatement(H, n, k, seed):
     ref = np.log(loo_ref.gpinv(np.arange(0.5, n) / n, want[0], want[1]) + expcut)
     ref[ref > 0] = 0
     assert np.allclose(sm, ref, rtol=1e-12, atol=1e-14)
+
+
+def test_fit_of_all_equal_tails_equals_the_restatement(H):
+    """every n in 5..4000, an all-equal tail: for n with m = 16 j - 8 (100..120, 676..728, 1764..1848, 3364..3480) candidate j
+    is b = 0 with a NaN profile value. Header and restatement leave it out alike and the fit stays finite for every n"""
+    ks = []
+    for v in (0.37, 1e-3):
+        for n in range(5, 4001):
+            x = np.full(n, v)
+            got, want = host_fit(H, x), loo_ref.gpdfit(x)
+            assert np.isfinite(got[0]) and np.isfinite(got[1]), (v, n, got)
+            assert abs(got[0] - want[0]) <= 1e-9 * max(1.0, abs(want[0])) and abs(got[1] - want[1]) <= 1e-9 * abs(want[1]), (v, n, got, want)
+            if v == 0.37:
+                ks.append(got[0])
+    d = np.diff(ks)                                                 # k falls with n, in small steps also where a candidate drops out
+    assert np.all(d < 0) and np.max(np.abs(d[45:])) < 0.04, (np.argmax(d) + 5, np.max(np.abs(d[45:])))
+
+
+def test_fit_kernel_arrays_hold_the_largest_tail(H):
+    """the fit kernel's candidate arrays (kMaxM) hold the candidates of the largest tail the API accepts (kMaxTail)"""
+    assert H.hs_loo_max_tail() == 1 << 20
+    assert H.hs_loo_fit_m(H.hs_loo_max_tail()) <= H.hs_loo_max_m()
+    assert H.hs_loo_fit_m(H.hs_loo_max_tail()) == 30 + 1024 == 30 + int((1 << 20) ** 0.5)
+    from bayes_js_b200.summary import MAX_LOO_TAIL
+    assert MAX_LOO_TAIL == H.hs_loo_max_tail()
+
+
+@pytest.mark.parametrize("n, k, seed", [(5, 0.2, 1), (17, -0.3, 2), (100, 0.5, 3), (1000, 0.9, 4), (3000, 0.0, 5), (20000, 0.7, 6)])
+def test_blocked_restatement_equals_the_whole_matrix(n, k, seed):
+    """loo_ref.gpdfit forms k(b) over blocks of candidates (for n = 2^20 the whole m x n matrix would be 8.8 GB): the same fit"""
+    x = np.sort(loo_ref.gpinv(np.random.default_rng(seed).uniform(size=n), k, 1.7))
+    m = 30 + int(n ** 0.5)
+    whole = loo_ref.gpdfit(x, block=m)
+    for rows in (1, 7, None):
+        got = loo_ref.gpdfit(x, block=rows)
+        assert abs(got[0] - whole[0]) <= 1e-15 * max(1.0, abs(whole[0])) and abs(got[1] - whole[1]) <= 1e-15 * abs(whole[1]), (rows, got, whole)
 
 
 @pytest.mark.parametrize("k", [-0.2, 0.3, 0.7])
