@@ -8,10 +8,47 @@
 // four k (four chains of one row). Per the PTX m8n8k4 f64 layouts, lane l holds A[l >> 2][l & 3] (row-major A, 8 x 4),
 // B[l & 3][l >> 2] (column-major B, 4 x 8) and C[l >> 2][2 (l & 3) + i], i < 2. With A = d of block bi and B = d^T of block bj,
 // a lane's A and B fragments are both the centred value of entry 8b + (l >> 2), chain c0 + (l & 3): one staged value serves as
-// the A fragment of tiles (b, .) and the B fragment of tiles (., b).
+// the A fragment of tiles (b, .) and the B fragment of tiles (., b). The arithmetic of the centres the Gram kernel subtracts (K_c1's
+// chain means, K_c2's shard mean) is here too.
 #pragma once
 
+#include "amwg_nested.cuh"      // run_bits, run_mean
+
 namespace summary {
+
+// K_c1: the mean over rows of one chain's column p[r * stride], r < rows >= 1: a sequential sum, eight loads in flight; a constant
+// run of finite values has that value as its mean (run_mean)
+__host__ __device__ __forceinline__ double co_chain_mean(const double* __restrict__ p, long long rows, size_t stride) {
+  const unsigned long long b0 = run_bits(p[0]);
+  unsigned long long diff = 0;
+  double sum = 0.0;
+  long long r = 0;
+  for (; r + 8 <= rows; r += 8) {
+    double v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) { sum += v[u]; diff |= run_bits(v[u]) ^ b0; }
+  }
+  for (; r < rows; ++r) { const double v = p[r * stride]; sum += v; diff |= run_bits(v) ^ b0; }
+  return run_mean(sum, rows, p[0], diff);
+}
+
+// K_c2, thread t of `threads`: the sequential sum of the chain means xbar[c], c = t, t + threads, .. < C, and run_mean's diff of
+// their bits against xbar[0]. The CTA adds the sums in a fixed tree and ORs the diffs; m = run_mean(total, C, xbar[0], diff), so
+// that m is the chain means' common value when they all have the same bits.
+struct CoMeanPart { double sum; unsigned long long diff; };
+__host__ __device__ __forceinline__ CoMeanPart co_mean_part(const double* __restrict__ xbar, long long C, int t, int threads) {
+  const unsigned long long b0 = run_bits(xbar[0]);
+  CoMeanPart p{0.0, 0};
+#pragma unroll 8
+  for (long long c = t; c < C; c += threads) {              // unrolled: eight loads in flight
+    const double v = xbar[c];
+    p.sum += v;
+    p.diff |= run_bits(v) ^ b0;
+  }
+  return p;
+}
 
 constexpr int kMaxSel = 128;                        // entries per call: 16 blocks, 136 tiles
 constexpr int kCoWarps = 16;                        // warps per CTA of the Gram kernel

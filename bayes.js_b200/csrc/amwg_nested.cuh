@@ -24,8 +24,32 @@ __host__ __device__ __forceinline__ Moments merge(const Moments& a, const Moment
   return r;
 }
 
-// the record (1, mean, 0, M2) of one chain's column p[r * stride], r < rows: two sequential passes, eight loads in flight per thread
+// The bits of x, for the constant-run test of run_mean: equal bits, not equal values, so that a mix of -0 and +0 is not a run.
+__host__ __device__ __forceinline__ unsigned long long run_bits(double x) {
+#ifdef __CUDA_ARCH__
+  return (unsigned long long)__double_as_longlong(x);
+#else
+  unsigned long long u;
+  memcpy(&u, &x, sizeof u);
+  return u;
+#endif
+}
+
+// The mean of a run of n values summed to s, whose first value is x0; `diff` is the OR over the run of run_bits(v) ^ run_bits(x0),
+// 0 exactly when every value has x0's bits. A constant run of finite values has x0 as its mean, so that the values centred on it
+// are exactly 0: fl(fl(n x0) / n) is x0 only for some x0 (7.25, but not 0.1 or 184.3), and a mean one ulp off would give a constant
+// entry a within-chain variance of ~1e-33 where it has none. Every other run (a mix of -0 and +0, a NaN, an infinity, any two
+// values that differ) keeps fl(s / n).
+__host__ __device__ __forceinline__ double run_mean(double s, long long n, double x0, unsigned long long diff) {
+  const bool finite = (run_bits(x0) & 0x7ff0000000000000ull) != 0x7ff0000000000000ull;     // exponent not all ones
+  return diff == 0 && finite ? x0 : s / (double)n;
+}
+
+// the record (1, mean, 0, M2) of one chain's column p[r * stride], r < rows >= 1: two sequential passes, eight loads in flight per
+// thread; the mean is run_mean's
 __host__ __device__ __forceinline__ Moments chain_record(const double* __restrict__ p, long long rows, size_t stride) {
+  const unsigned long long b0 = run_bits(p[0]);
+  unsigned long long diff = 0;
   double s = 0.0;
   long long r = 0;
   for (; r + 8 <= rows; r += 8) {                            // the sum stays sequential
@@ -33,10 +57,10 @@ __host__ __device__ __forceinline__ Moments chain_record(const double* __restric
 #pragma unroll
     for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) s += v[u];
+    for (int u = 0; u < 8; ++u) { s += v[u]; diff |= run_bits(v[u]) ^ b0; }
   }
-  for (; r < rows; ++r) s += p[r * stride];
-  const double m = s / (double)rows;
+  for (; r < rows; ++r) { const double v = p[r * stride]; s += v; diff |= run_bits(v) ^ b0; }
+  const double m = run_mean(s, rows, p[0], diff);
   double m2 = 0.0;
   r = 0;
   for (; r + 8 <= rows; r += 8) {

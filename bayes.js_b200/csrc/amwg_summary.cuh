@@ -366,6 +366,9 @@ __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restr
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
     for (int half = 0; half < 2; ++half) {
       const double* p = x + (size_t)e * C + c + (size_t)(half ? rows - h : 0) * stride;
+      const double x0 = p[0];
+      const unsigned long long x0_bits = run_bits(x0);
+      unsigned long long diff = 0;
       double s0 = 0.0;
       long long n0 = 0, n1 = 0;
       long long r = 0;
@@ -374,11 +377,20 @@ __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restr
 #pragma unroll
         for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
 #pragma unroll
-        for (int u = 0; u < 8; ++u) { s0 += v[u]; if constexpr (NS == 3) { n0 += v[u] <= q0; n1 += v[u] <= q1; } }
+        for (int u = 0; u < 8; ++u) {
+          s0 += v[u];
+          diff |= run_bits(v[u]) ^ x0_bits;
+          if constexpr (NS == 3) { n0 += v[u] <= q0; n1 += v[u] <= q1; }
+        }
       }
-      for (; r < h; ++r) { const double v = p[r * stride]; s0 += v; if constexpr (NS == 3) { n0 += v <= q0; n1 += v <= q1; } }
+      for (; r < h; ++r) {
+        const double v = p[r * stride];
+        s0 += v;
+        diff |= run_bits(v) ^ x0_bits;
+        if constexpr (NS == 3) { n0 += v <= q0; n1 += v <= q1; }
+      }
       double m[NS];
-      m[0] = s0 / (double)h;
+      m[0] = run_mean(s0, h, x0, diff);                      // a constant half-chain is centred on its value (amwg_nested.cuh)
       if constexpr (NS == 3) { m[1] = (double)n0 / (double)h; m[2] = (double)n1 / (double)h; }
 
       double ring[kLagSlots];
@@ -718,36 +730,23 @@ __global__ void __launch_bounds__(256) amwg_rank_z_kernel(const long long* __res
 // the same kernel's Gram matrix of the [1][sel][C] block of chain means centred by m.
 struct SelList { int e[kMaxSel]; };      // block entry of each selected slot, passed by value (512 B of kernel parameters)
 
-// K_c1: xbar[s][c] = the mean over rows of chain c of entry sel[s], summed sequentially as in K_m1
+// K_c1: xbar[s][c] = the mean over rows of chain c of entry sel[s] (co_chain_mean, amwg_comoments.cuh)
 __global__ void __launch_bounds__(256) amwg_chain_means_kernel(const double* __restrict__ x, long long rows, int entries, long long C, SelList sel,
                                                                double* __restrict__ xbar) {
   const int s = blockIdx.y;
   const size_t stride = (size_t)entries * C;
-  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
-    const double* p = x + (size_t)sel.e[s] * C + c;
-    double sum = 0.0;
-    long long r = 0;
-    for (; r + 8 <= rows; r += 8) {                          // eight loads in flight per thread, the sum stays sequential
-      double v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) sum += v[u];
-    }
-    for (; r < rows; ++r) sum += p[r * stride];
-    xbar[(size_t)s * C + c] = sum / (double)rows;
-  }
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x)
+    xbar[(size_t)s * C + c] = co_chain_mean(x + (size_t)sel.e[s] * C + c, rows, stride);
 }
 
-// K_c2: m[s] = (sum over chains of xbar[s][c], in a fixed order) / C
+// K_c2: m[s] = (sum over chains of xbar[s][c], in a fixed order) / C, or the chain means' common value (co_mean_part)
 __global__ void __launch_bounds__(256) amwg_shard_mean_kernel(const double* __restrict__ xbar, long long C, double* __restrict__ m) {
   __shared__ double sh[256];
   const int s = blockIdx.x;
-  double acc = 0.0;
-#pragma unroll 8
-  for (long long c = threadIdx.x; c < C; c += 256) acc += xbar[(size_t)s * C + c];     // unrolled: eight loads in flight
-  const double tot = cta_sum<256>(sh, acc);
-  if (threadIdx.x == 0) m[s] = tot / (double)C;
+  const CoMeanPart part = co_mean_part(xbar + (size_t)s * C, C, threadIdx.x, 256);
+  const double tot = cta_sum<256>(sh, part.sum);
+  const bool differ = __syncthreads_or(part.diff != 0);
+  if (threadIdx.x == 0) m[s] = run_mean(tot, C, xbar[(size_t)s * C], differ ? 1 : 0);
 }
 
 __device__ __forceinline__ void dmma_8x8x4(double (&c)[2], double a, double b) {

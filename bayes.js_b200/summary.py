@@ -46,7 +46,9 @@ def merge_moment_records(records: Sequence[np.ndarray]) -> np.ndarray:
 def finalize_moments(rec: np.ndarray, rows: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """(mean, sd, rhat) per entry from the merged record. sd: pooled over all rows*chains draws, ddof=1. rhat: Gelman-Rubin
     potential scale reduction sqrt(((n-1)/n W + B/n) / W) with n = rows, W the mean within-chain variance, B/n the variance of
-    the chain means (NaN with fewer than 2 rows or chains, or when W = 0)."""
+    the chain means. NaN with fewer than 2 rows or chains, or when W = 0 and B = 0: an entry whose draws all equal one value,
+    whose chain means are that value exactly (run_mean, csrc/amwg_nested.cuh), so its sd is 0. +inf when W = 0 < B: every chain
+    stuck at a value of its own."""
     G, mean, b2, sw = rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3]
     M = G * rows
     with np.errstate(invalid="ignore", divide="ignore"):
@@ -389,7 +391,9 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
       ess_tail   min of the ESS of 1[x <= q05] and of 1[x <= q95] (lo, hi: the pooled exact quantiles; ties count as <=)
       mcse_mean  sd / sqrt(ess_mean), sd the pooled sd
       rhat_split sqrt(var+ / W) of the draws (not rank-normalised)
-    Edge cases: fewer than 10 rows (h < 5): all NaN. A constant entry (vmin == vmax) has ESS = M h and MCSE 0, and an indicator
+    Edge cases: fewer than 10 rows (h < 5): all NaN. A constant entry (vmin == vmax) has ESS = M h, MCSE 0 and rhat_split NaN
+    (its half-chains are centred on their value, so W = 0 and B = 0); half-chains each constant at a value of their own give
+    rhat_split +inf. An indicator
     that is constant (all 1 when the quantile equals the maximum) has ESS = M h. A non-finite minimum or maximum (an infinite or
     NaN draw) makes all four values NaN.
     Lag windows of at most `max_lags` lags are asked for only while some series' Geyer loop still needs a lag it has not got,
@@ -943,7 +947,9 @@ def finalize_comoments(rec: np.ndarray, rows: int) -> dict:
     in numpy.corrcoef's operations (clipped to [-1, 1]), within = W / (C (rows - 1)), between = B / (C - 1) and Brooks & Gelman's
     (1998) multivariate potential scale reduction (n - 1)/n + (C + 1)/C lambda_max(within^-1 between), n = rows, from a Cholesky
     factor of within and eigvalsh. The R-hat is NaN when rows < 2, C < 2, any entry is non-finite, or within is not positive
-    definite (a constant entry, or one that is linear in others)."""
+    definite (a constant entry, or one that is linear in others). An entry whose draws all equal one value is centred on that
+    value exactly on the device, so its rows and columns of cov, within and between are 0 and its correlations NaN, as
+    numpy.corrcoef gives for a row of zero variance."""
     G, m, B, W = split_comoment_record(rec)
     M = G * rows
     with np.errstate(invalid="ignore", divide="ignore"):
@@ -1059,7 +1065,8 @@ def merge_nested_records(records: Sequence[np.ndarray], M: int, rows: int) -> np
 def finalize_nested(rec: np.ndarray) -> np.ndarray:
     """rhat_nested per entry from the merged [entries, 4] superchain-to-total record (K, mean of the superchain means, M2 of the
     superchain means, sum over superchains of B~_k + W-_k): with B^ = M2 / (K - 1) and W^ = sum / K,
-    rhat_nested = sqrt(1 + B^ / W^). NaN when K < 2, when W^ = 0, or when any value of the record is not finite (a NaN or +-inf
+    rhat_nested = sqrt(1 + B^ / W^). NaN when K < 2, when W^ = 0 (an entry whose draws all equal one value, whose chain records
+    then hold that mean and M2 = 0 exactly; or M = 1 with N = 1), or when any value of the record is not finite (a NaN or +-inf
     draw of the entry)."""
     rec = np.asarray(rec, dtype=np.float64)
     K, mean, m2, sw = rec[:, 0], rec[:, 1], rec[:, 2], rec[:, 3]

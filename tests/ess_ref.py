@@ -6,7 +6,7 @@
 Never imported by the product."""
 import numpy as np
 
-from summary_ref import NumpyBlockReducer
+from summary_ref import NumpyBlockReducer, run_means
 
 
 def halves(x):
@@ -105,9 +105,9 @@ def autocov_records(x, thresholds, lag0, n_lags):
             series += [(x[:, e, :] <= thresholds[e][0]).astype(float), (x[:, e, :] <= thresholds[e][1]).astype(float)]
         for s, ys in enumerate(series):
             y = halves(ys)
-            m = y.sum(axis=1) / h
+            m = run_means(y.T)                                 # a constant half-chain of draws is centred on its value
             d = y - m[:, None]
-            mean = m.mean()
+            mean = run_means(m)                                # equal means: that value, as the Chan merge gives
             out[e, s, :4] = (y.shape[0], mean, ((m - mean) ** 2).sum(), (d * d).sum())
             for k in range(n_lags):
                 t = lag0 + k

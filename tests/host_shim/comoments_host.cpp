@@ -2,7 +2,10 @@
 // (csrc/amwg_comoments.cuh, the text the Gram kernel indexes with) and a scalar emulation of mma.sync.m8n8k4.f64 over 32
 // emulated lanes in the PTX fragment layouts, for tests/test_summary_covariance_host.py. Every global, shared and partial index
 // the schedule forms is checked against its buffer, and every fragment read against what was staged; hs_comoments returns the
-// number of violations. Build with -ffp-contract=off, as the library is built with --fmad=false.
+// number of violations, which include a (row, selected entry, chain) of the block loaded other than once over a Gram pass's whole
+// grid walk and a (tile, staged row, quad) step issued other than once across a tile's reps. The centres are K_c1's and K_c2's
+// arithmetic from the same header, K_c2's with its 256-thread CTA tree. Build with -ffp-contract=off, as the library is built with
+// --fmad=false.
 #include "cuda_runtime.h"
 #include "amwg_comoments.cuh"
 
@@ -39,6 +42,8 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
   std::vector<int> writes(partial.size(), 0);
   std::vector<double> st(kCoSmem);
   std::vector<char> staged(kCoSmem);
+  std::vector<int> loads((size_t)rows * n_sel * C, 0);          // loads of (row, selected entry, chain) over the whole walk
+  std::vector<int> steps;                                       // issues of (tile, staged row * nq + quad) in one stage
   for (long long cta = 0; cta < gx; ++cta) {
     std::vector<double> acc((size_t)kCoWarps * kCoSlots * 32 * 2, 0.0);
     for (long long g = cta; g * kCoChains < C; g += gx) {
@@ -58,6 +63,7 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
               const long long xi = co_x_index(r, sel[el.s], c, entries, C), ci = co_cen_index(el.s, c, cen_se, cen_sc);
               check(xi >= 0 && xi < x_len);
               check(ci >= 0 && ci < cen_len);
+              if (r < rows && c < C) ++loads[((size_t)r * n_sel + el.s) * C + c];
               if (xi >= 0 && xi < x_len && ci >= 0 && ci < cen_len) v = x[xi] - cen[ci];
             }
             const int si = co_smem_index(el.rr, el.s, el.cc, nb);
@@ -65,6 +71,7 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
             if (si >= 0 && si < kCoSmem) { check(!staged[si]); st[si] = v; staged[si] = 1; }
           }
         const int nr = (int)(rows - r0 < srows ? rows - r0 : srows);
+        steps.assign((size_t)n_tiles * nr * nq, 0);
         for (int w = 0; w < kCoWarps; ++w)
           for (int k = co_warp_rep(w, nb); k < nr * nq; k += reps) {
             const int base = co_frag_base(k % nq, k / nq, nb);
@@ -74,6 +81,7 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
               int bi = 0, bj = 0;
               co_tile(t, nb, bi, bj);
               check(bi <= bj && bj < nb);
+              ++steps[(size_t)t * nr * nq + k];
               double a[32], b[32];
               for (int l = 0; l < 32; ++l) {
                 const int ia = base + co_frag_lane(l, bi), ib = base + co_frag_lane(l, bj);
@@ -86,6 +94,7 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
               mma_m8n8k4(reinterpret_cast<double(*)[2]>(&acc[(((size_t)w * kCoSlots + s) * 32) * 2]), a, b);
             }
           }
+        for (int n : steps) check(n == 1);                        // every tile takes every (row, quad) step of the stage once
       }
     }
     for (int w = 0; w < kCoWarps; ++w)
@@ -101,6 +110,7 @@ void gram(const double* x, long long x_len, long long rows, int entries, long lo
       }
   }
   for (int wcount : writes) check(wcount == 1);                  // every partial element written exactly once
+  for (int n : loads) check(n == 1);                             // every value of the block loaded exactly once
   const int n_vals = n_tiles * 64;
   out.assign(n_vals, 0.0);
   for (int v = 0; v < n_vals; ++v) {
@@ -118,16 +128,19 @@ long long hs_comoments(const double* x, long long rows, int entries, long long C
   g_bad = 0;
   const long long x_len = rows * entries * C;
   std::vector<double> xbar((size_t)n_sel * C), m(n_sel);
-  for (int s = 0; s < n_sel; ++s)
-    for (long long c = 0; c < C; ++c) {
-      double sum = 0.0;
-      for (long long r = 0; r < rows; ++r) sum += x[co_x_index(r, sel[s], c, entries, C)];
-      xbar[(size_t)s * C + c] = sum / (double)rows;
+  for (int s = 0; s < n_sel; ++s)                                // K_c1
+    for (long long c = 0; c < C; ++c) xbar[(size_t)s * C + c] = co_chain_mean(x + (size_t)sel[s] * C + c, rows, (size_t)entries * C);
+  for (int s = 0; s < n_sel; ++s) {                              // K_c2: 256 threads' parts, cta_sum's tree, the OR of the diffs
+    std::vector<double> sh(256);
+    unsigned long long diff = 0;
+    for (int t = 0; t < 256; ++t) {
+      const CoMeanPart p = co_mean_part(xbar.data() + (size_t)s * C, C, t, 256);
+      sh[t] = p.sum;
+      diff |= p.diff;
     }
-  for (int s = 0; s < n_sel; ++s) {
-    double sum = 0.0;
-    for (long long c = 0; c < C; ++c) sum += xbar[(size_t)s * C + c];
-    m[s] = sum / (double)C;
+    for (int w = 128; w > 0; w >>= 1)
+      for (int t = 0; t < w; ++t) sh[t] += sh[t + w];
+    m[s] = run_mean(sh[0], C, xbar[(size_t)s * C], diff);
   }
   std::vector<int> ident(n_sel);
   for (int i = 0; i < n_sel; ++i) ident[i] = i;

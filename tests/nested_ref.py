@@ -16,7 +16,12 @@ gamma_k = k u / (1 - k u), Higham 3.1):
             errors, and a sum of the leaves' sum_w by at most gamma_L (sum of |sum_w|) + their errors.
   unit      B~_k + W-_k: two divisions and an addition, gamma_3 relative, on top of the errors of M2 / (M - 1) and sum_w / (M (N - 1)).
 The superchain level merges the M chain records of a superchain; the total level merges the K unit records.
-Test infrastructure only."""
+Values that all have the bits of the first, a finite one, have that value as their exact mean (and M2 = 0), at every level.
+
+record_loop restates the records chain by chain with fsum; record() is the same vectorised over chains and superchains, for blocks
+of 2^20 chains: each chain's sums by a compensated sum along the rows (Sum2, tests/moments_ref.py), a superchain's by Sum2 across
+its M chains, and fsum only across the superchains. Sum2 is off by at most u |sum| + gamma_{n-1}^2 sum |x|, one rounding more
+than fsum and far inside the bound; test_summary_nested_host checks the two forms against each other. Test infrastructure only."""
 import math
 
 import numpy as np
@@ -44,10 +49,23 @@ def _chan_bound(means, e_v, m2_leaf, m2_err, sw_leaf, sw_err, steps=None):
     return E, b_m2, b_sw
 
 
+def _same(v, axis=0):
+    """whether the values along `axis` all have the bits of the first, a finite one: their exact mean is that value"""
+    v = np.asarray(v, dtype=np.float64)
+    first = np.take(v, [0], axis=axis)
+    return np.all(v.view(np.uint64) == first.view(np.uint64), axis=axis) & np.isfinite(np.take(v, 0, axis=axis))
+
+
+def _fmean(v):
+    """mean of v with fsum, exact for values that all have the same bits"""
+    v = np.asarray(v, dtype=np.float64)
+    return float(v[0]) if _same(v) else math.fsum(v) / len(v)
+
+
 def _chain(col):
     """exact (mean, M2) of one chain, and the device's error bounds for both"""
     N = len(col)
-    m = math.fsum(col) / N
+    m = _fmean(col)
     m2 = math.fsum((col - m) ** 2)
     dlt = gamma(N + 1) * float(np.mean(np.abs(col)))
     e_m2 = N * dlt * dlt + gamma(N + 2) * float(np.sum((np.abs(col - m) + dlt) ** 2))
@@ -58,14 +76,72 @@ def _superchain(x, e, c0, c1):
     """chain-level record (n, mean, M2, sum_w) of local chains [c0, c1) of entry e, exact, and its bounds"""
     ch = [_chain(np.asarray(x[:, e, c], dtype=np.float64)) for c in range(c0, c1)]
     means = np.array([c[0] for c in ch])
-    mean = math.fsum(means) / len(ch)
+    mean = _fmean(means)
     m2 = math.fsum((means - mean) ** 2)
     sw = math.fsum([c[1] for c in ch])
     bm, bm2, bsw = _chan_bound(means, [c[2] for c in ch], [0.0], [0.0], [c[1] for c in ch], [c[3] for c in ch])
     return np.array([len(ch), mean, m2, sw]), np.array([0.0, bm, bm2, bsw])
 
 
+def _chan_bound_v(means, e_v, sw_leaf, sw_err):
+    """_chan_bound(means[k], e_v[k], [0.0], [0.0], sw_leaf[k], sw_err[k]) for every row k of the [K, n] arrays at once"""
+    n = means.shape[1]
+    L = n + 20
+    A = np.max(np.abs(means), axis=1)
+    D = np.max(means, axis=1) - np.min(means, axis=1)
+    E = np.max(e_v, axis=1) + 3 * L * gamma(4) * A
+    De = 2 * E + U * D
+    ws = n * (1 + math.log2(n)) if n > 1 else 0.0
+    b_m2 = ws * (2 * D * De + De * De) + gamma(L + 6) * (ws * (D + De) ** 2)
+    b_sw = gamma(L) * np.sum(np.abs(sw_leaf), axis=1) + np.sum(sw_err, axis=1)
+    return E, b_m2, b_sw
+
+
 def record(x: np.ndarray, first_chain: int, M: int):
+    """record_loop vectorised (module docstring): the complete superchains at once, the (at most two) cut ones by _superchain"""
+    from moments_ref import _sum2
+    x = np.asarray(x, dtype=np.float64)
+    rows, entries, C = x.shape
+    k0, k1 = first_chain // M, (first_chain + C - 1) // M
+    kf, kl = -(-first_chain // M), (first_chain + C) // M - 1                    # the complete superchains [kf, kl]
+    exact = np.zeros((entries, 14))
+    bound = np.zeros((entries, 14))
+    exact[:, [4, 9]] = -1.0
+    if kl >= kf:
+        K = kl - kf + 1
+        d = x[:, :, kf * M - first_chain:(kl + 1) * M - first_chain]
+        with np.errstate(invalid="ignore", over="ignore"):
+            m = np.where(_same(d), d[0], _sum2(d) / rows)                       # [entries, chains]
+            dev = d - m[None]
+            m2c = _sum2(dev * dev)
+            dlt = gamma(rows + 1) * np.mean(np.abs(d), axis=0)
+            e_m2 = rows * dlt * dlt + gamma(rows + 2) * np.sum((np.abs(dev) + dlt[None]) ** 2, axis=0)
+            for e in range(entries):
+                cm = m[e].reshape(K, M)
+                sk = np.where(_same(cm, axis=1), cm[:, 0], _sum2(cm.T) / M)       # superchain means
+                m2 = _sum2(((cm - sk[:, None]) ** 2).T)
+                sw = _sum2(m2c[e].reshape(K, M).T)
+                bm, bm2, bsw = _chan_bound_v(cm, dlt[e].reshape(K, M), m2c[e].reshape(K, M), e_m2[e].reshape(K, M))
+                bt = m2 / (M - 1) if M > 1 else np.zeros(K)
+                wt = sw / (M * (rows - 1)) if rows > 1 else np.zeros(K)
+                eb = (bm2 / (M - 1) if M > 1 else 0.0) + (bsw / (M * (rows - 1)) if rows > 1 else 0.0) + gamma(3) * (bt + wt)
+                mean = _fmean(sk)
+                exact[e, :4] = (K, mean, math.fsum((sk - mean) ** 2), math.fsum(bt + wt))
+                tb = _chan_bound(sk, bm, [0.0], [0.0], bt + wt, eb)
+                bound[e, :4] = (0.0, *tb)
+    for k in sorted({k0, k1}):
+        c0, c1 = max(k * M - first_chain, 0), min((k + 1) * M - first_chain, C)
+        if c1 - c0 == M:
+            continue
+        slot = 0 if k == k0 else 1                                   # the first superchain, or the last when it is another one
+        for e in range(entries):
+            rec, b = _superchain(x, e, c0, c1)
+            exact[e, 4 + 5 * slot:9 + 5 * slot] = (k, *rec)
+            bound[e, 5 + 5 * slot:9 + 5 * slot] = b
+    return exact, bound
+
+
+def record_loop(x: np.ndarray, first_chain: int, M: int):
     """x [rows, entries, chains] of the global chains [first_chain, first_chain + chains) -> (exact [entries, 14], bound
     [entries, 14]) in amwg_summary_nested's layout: the complete superchains' (K, mean, M2, sum of B~_k + W-_k), then the cut
     records {id, chains, mean, M2, sum_w} of the first and the last superchain when the range cuts them."""
@@ -90,7 +166,7 @@ def record(x: np.ndarray, first_chain: int, M: int):
         if units:
             means = np.array([v[0] for v in units])
             K = len(units)
-            mean = math.fsum(means) / K
+            mean = _fmean(means)
             exact[e, :4] = (K, mean, math.fsum((means - mean) ** 2), math.fsum([v[1] for v in units]))
             bm, bm2, bsw = _chan_bound(means, [b[0] for b in ubnd], [0.0], [0.0], [v[1] for v in units], [b[1] for b in ubnd])
             bound[e, :4] = (0.0, bm, bm2, bsw)

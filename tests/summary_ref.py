@@ -4,15 +4,25 @@ Never imported by the product."""
 import numpy as np
 
 
+def run_means(x: np.ndarray) -> np.ndarray:
+    """means along axis 0 as the device forms them (run_mean, csrc/amwg_nested.cuh): a run whose values all have the bits of its
+    first value, a finite one, has that value as its mean; every other run has fl(sum) / n"""
+    x = np.asarray(x, dtype=np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        m = x.sum(axis=0) / x.shape[0]
+    same = np.all(x.view(np.uint64) == x[:1].view(np.uint64), axis=0) & np.isfinite(x[0])
+    return np.where(same, x[0], m)
+
+
 class NumpyBlockReducer:
     def moments(self, block):
         x = block.numpy()                                    # [rows, entries, chains]
         rows, entries, chains = x.shape
-        m = x.sum(axis=0) / rows                             # [entries, chains]
+        m = run_means(x)                                     # [entries, chains]
         m2 = ((x - m[None]) ** 2).sum(axis=0)
         out = np.empty((entries, 4))
         for e in range(entries):
-            mean = m[e].mean()
+            mean = run_means(m[e])                          # equal chain means: that value, as the Chan merge gives
             out[e] = (chains, mean, ((m[e] - mean) ** 2).sum(), m2[e].sum())
         return out
 
@@ -43,7 +53,7 @@ class ChanBlockReducer(NumpyBlockReducer):
         from bayes_js_b200.summary import merge_moment_records
         x = block.numpy()
         rows, entries, chains = x.shape
-        m = x.sum(axis=0) / rows
+        m = run_means(x)
         with np.errstate(invalid="ignore"):
             m2 = ((x - m[None]) ** 2).sum(axis=0)
         w = 1

@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 import cov_ref
-from summary_ref import NumpyBlockReducer
+from summary_ref import NumpyBlockReducer, run_means
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -24,8 +24,8 @@ class NumpyCovReducer(NumpyBlockReducer):
     def comoments(self, block, sel):
         x = block.numpy()[:, np.asarray(sel), :]                 # [rows, n, chains]
         rows, n, chains = x.shape
-        xbar = x.sum(axis=0) / rows                             # [n, chains]
-        m = xbar.sum(axis=1) / chains
+        xbar = run_means(x)                                     # [n, chains]
+        m = run_means(xbar.T)
         f = xbar - m[:, None]
         d = (x - xbar[None]).transpose(1, 0, 2).reshape(n, -1)
         return np.concatenate([[chains], m, (f @ f.T).ravel(), (d @ d.T).ravel()])
@@ -248,3 +248,92 @@ def test_tile_schedule_on_the_host(H, E, chains):
     bad = H.hs_comoments(x.ctypes.data, rows, entries, chains, sel.ctypes.data, E, out.ctypes.data)
     assert bad == 0
     cov_ref.check_record(out, x, sel, (E, chains))
+
+
+def _co_stage_rows(nb):
+    return max(16 // nb, 1)                                      # amwg_comoments.cuh: co_stage_rows
+
+
+@pytest.mark.parametrize("nb", range(1, 17))
+@pytest.mark.parametrize("chains", [8449, 2 * 8448 + 37])
+def test_tile_schedule_every_block_count_over_the_grid_walk(H, nb, chains):
+    """every block count nb = 1..16, full (8 nb entries) at 8449 chains and ragged (8 nb - 5) at 2 * 8448 + 37, two staged passes
+    plus a ragged row, where each of the 264 CTAs walks two or three 32-chain groups and the last group is ragged: every value
+    loaded once, every (tile, row, quad) step issued once across the reps, and B and W within the bound of the reference"""
+    rows = 2 * _co_stage_rows(nb) + 1
+    for E in [8 * nb if chains == 8449 else max(8 * nb - 5, 1)]:
+        rng = np.random.default_rng(nb * 7919 + chains + E)
+        entries = E + 1
+        x = 184.5 + rng.normal(size=(rows, entries, chains)) * rng.uniform(0.1, 3, size=(1, entries, 1))
+        x += 0.3 * rng.normal(size=(1, entries, chains))
+        sel = rng.permutation(entries)[:E].astype(np.int32)
+        out = np.empty(1 + E + 2 * E * E)
+        assert H.hs_comoments(x.ctypes.data, rows, entries, chains, sel.ctypes.data, E, out.ctypes.data) == 0
+        cov_ref.check_record(out, x, sel, (nb, E, chains), exact=cov_ref.record(x, sel))
+
+
+@pytest.mark.parametrize("rows, chains, n", [(1, 1, 1), (3, 5, 2), (17, 41, 9), (2, 1001, 3), (20, 300, 65)])
+def test_vectorised_reference_agrees_with_its_loop_form(rows, chains, n):
+    rng = np.random.default_rng(rows * 100 + chains + n)
+    x = 1e6 + rng.normal(size=(rows, n + 1, chains)) + rng.normal(size=(1, n + 1, chains))
+    x[:, 0] = 0.1                                               # a constant entry: exact zeros in both forms
+    sel = list(rng.permutation(n + 1)[:n])
+    C0, m0, B0, W0 = cov_ref.exact_record(x, sel)
+    C1, m1, B1, W1 = cov_ref.record(x, sel)
+    bm, bB, bW = cov_ref.device_bound(x, sel)
+    assert C0 == C1
+    assert np.all(np.abs(m1 - m0) <= 2 * cov_ref.U * np.abs(m0))
+    # far inside the device bound: the two forms differ by less than 1 / 100 of it
+    assert np.all(np.abs(W1 - W0) <= bW / 100) and np.all(np.abs(B1 - B0) <= bB / 100)
+
+
+def _constant_block(value, rows, chains, seed):
+    """[rows, 4, chains]: two correlated normal entries, `value` everywhere in entry 2, entry 3 constant within each chain"""
+    rng = np.random.default_rng(seed)
+    z = rng.normal(size=(rows, chains))
+    x = np.empty((rows, 4, chains))
+    x[:, 0] = 10.0 + z
+    x[:, 1] = -3.0 + 0.6 * z + 0.8 * rng.normal(size=(rows, chains))
+    x[:, 2] = value
+    x[:, 3] = value + (abs(value) + 1.0) * 1e-3 * rng.normal(size=(1, chains))
+    return x
+
+
+@pytest.mark.parametrize("value", [0.1, 184.3, 7.25, -1e150, 5e-324])
+@pytest.mark.parametrize("rows, chains", [(3, 1000), (50, 1001)])
+def test_constant_entry_has_exact_zero_rows_on_the_host_build(H, pkg, value, rows, chains):
+    """The kernels' text: an entry whose draws all equal one value has that value as its mean and exactly zero rows and
+    columns of B and W, so corr is NaN there (as numpy.corrcoef gives) and rhat_multivariate is NaN; an entry constant within
+    each chain has zero rows of W and a between part."""
+    from bayes_js_b200.summary import finalize_comoments
+    x = _constant_block(value, rows, chains, 5)
+    sel = np.arange(4, dtype=np.int32)
+    out = np.empty(1 + 4 + 2 * 16)
+    assert H.hs_comoments(x.ctypes.data, rows, 4, chains, sel.ctypes.data, 4, out.ctypes.data) == 0
+    m, B, W = out[1:5], out[5:21].reshape(4, 4), out[21:].reshape(4, 4)
+    assert m[2] == value
+    assert np.all(B[2] == 0) and np.all(B[:, 2] == 0) and np.all(W[2] == 0) and np.all(W[:, 2] == 0)
+    assert np.all(W[3] == 0) and np.all(W[:, 3] == 0) and B[3, 3] > 0
+    fin = finalize_comoments(out, rows)
+    assert np.all(fin["cov"][2] == 0) and np.all(fin["within"][:, 2] == 0) and np.all(fin["between"][2] == 0)
+    assert np.all(np.isnan(fin["corr"][2])) and np.all(np.isnan(fin["corr"][:, 2]))
+    assert np.isnan(fin["rhat_multivariate"])
+    assert np.all(np.isfinite(fin["corr"][np.ix_([0, 1, 3], [0, 1, 3])]))
+    # the two normal entries alone keep their bound and a finite R-hat
+    keep = np.array([0, 1], dtype=np.int32)
+    out2 = np.empty(1 + 2 + 8)
+    assert H.hs_comoments(x.ctypes.data, rows, 4, chains, keep.ctypes.data, 2, out2.ctypes.data) == 0
+    cov_ref.check_record(out2, x, keep, value)
+    assert np.isfinite(finalize_comoments(out2, rows)["rhat_multivariate"])
+
+
+def test_mixed_signed_zeros_keep_the_summed_mean(H):
+    """a run of -0 and +0 is not bitwise constant: the mean is fl(sum) / n = +0, as before the rule"""
+    x = np.zeros((4, 1, 3))
+    x[0, 0, :] = -0.0
+    x[:, 0, 1] = -0.0                                            # chain 1 all -0: its mean is -0
+    sel = np.zeros(1, dtype=np.int32)
+    out = np.empty(1 + 1 + 2)
+    assert H.hs_comoments(x.ctypes.data, 4, 1, 3, sel.ctypes.data, 1, out.ctypes.data) == 0
+    assert out[1] == 0 and out[2] == 0 and out[3] == 0
+    assert not np.signbit(out[1])                                # the chain means -0, +0, +0 differ in bits: summed, +0

@@ -296,3 +296,57 @@ def test_nested_over_gloo_world2(H):
     assert all(p.exitcode == 0 for p in procs)
     assert all(ok for _, ok, _ in res)
     assert res[0][2] == res[1][2]
+
+
+@pytest.mark.parametrize("M, rows, chains, first", CASES + [(64, 3, 10, 5), (2, 4, 2 * 3000 + 1, 1)])
+def test_vectorised_reference_agrees_with_its_loop_form(M, rows, chains, first):
+    x = _draws(rows, 3, chains, M + rows + chains, 1e6)
+    x[:, 2] = 0.1                                                    # a constant entry
+    a, ba = nested_ref.record(x, first, M)
+    b, bb = nested_ref.record_loop(x, first, M)
+    assert np.array_equal(a[:, [0, 4, 5, 9, 10]], b[:, [0, 4, 5, 9, 10]])
+    assert np.all(np.abs(a - b) <= ba / 100 + 4 * nested_ref.U * np.abs(b))    # far inside the bound
+    assert np.allclose(ba, bb, rtol=1e-6, atol=0)
+    assert np.all(a[2, [2, 3]] == 0) and a[2, 1] == 0.1 or a[2, 0] == 0
+
+
+@pytest.mark.parametrize("value", [0.1, 184.3, 7.25, -1e150])
+@pytest.mark.parametrize("M, rows, chains", [(16, 3, 1024), (64, 50, 4096), (1, 2, 300)])
+def test_constant_entry_on_the_host_build(H, pkg, value, M, rows, chains):
+    """the kernels' text: an entry whose draws all equal one value gives records with that mean and M2 = sum_w = 0 exactly, so
+    rhat_nested is NaN; the normal entries keep the bound; an entry constant within each chain but not between them (chains
+    stuck apart) has W-_k = 0 and B~_k > 0"""
+    from bayes_js_b200.summary import finalize_nested, merge_nested_records
+    x = _draws(rows, 3, chains, M + chains)
+    x[:, 1] = value
+    x[:, 2] = value + (abs(value) + 1.0) * 1e-3 * np.random.default_rng(1).normal(size=(1, chains))
+    got = host_nested(H, x, 0, M)
+    assert got[1, 1] == value and got[1, 2] == 0 and got[1, 3] == 0
+    rh = finalize_nested(merge_nested_records([got], M, rows))
+    assert np.isnan(rh[1]) and np.isfinite(rh[0])
+    assert (M == 1) == np.isnan(rh[2])                               # M = 1: W^ = 0 with B^ > 0 stays NaN
+    exact, bound = nested_ref.record(x, 0, M)
+    ok = np.abs(got[[0, 2]] - exact[[0, 2]]) <= bound[[0, 2]]
+    assert np.all(ok | (np.isnan(got[[0, 2]]) & np.isnan(exact[[0, 2]])))
+
+
+def test_constant_rule_of_the_numpy_stand_ins(pkg):
+    """summary_ref's and ess_ref's stand-ins follow the device's rule: sd 0, rhat and rhat_split NaN for a constant entry; chains
+    stuck at different values (W = 0 < B) have rhat = +inf, as sqrt(var+ / W) gives"""
+    import torch
+    import ess_ref
+    from bayes_js_b200.summary import summarise_block
+    rows, chains = 40, 64
+    rng = np.random.default_rng(3)
+    x = np.empty((rows, 5, chains))
+    x[:, 0] = rng.normal(size=(rows, chains))
+    x[:, 1] = 0.1
+    x[:, 2] = 184.3
+    x[:, 3] = 7.25
+    x[:, 4] = 0.1 * np.arange(chains)[None, :]                      # each chain stuck at its own value
+    red = ess_ref.NumpyAutocovReducer()
+    mean, sd, rhat, q, (diag, _windows) = summarise_block(red, torch.from_numpy(x), rows, chains, (0.05, 0.5, 0.95), False, diagnostics=True)
+    assert np.all(sd[1:4] == 0) and np.all(np.isnan(rhat[1:4])) and np.all(np.isnan(diag["rhat_split"][1:4]))
+    assert np.array_equal(mean[1:4], [0.1, 184.3, 7.25])
+    assert np.isfinite(rhat[0]) and rhat[4] == np.inf and diag["rhat_split"][4] == np.inf
+    assert np.all(diag["ess_mean"][1:4] == 2 * chains * (rows // 2)) and np.all(diag["mcse_mean"][1:4] == 0)
