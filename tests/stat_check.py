@@ -240,6 +240,30 @@ def audit_divergence(prog, consts, steps, before, gpu_after, orc_after, tile, or
     raise AssertionError("the rows differ but every decision agrees: a wrong value, not a tie")
 
 
+def compare_and_audit(prog, consts, same, gpu_rows, gpu_final, orc_rows, orc_final, oracle_trace, burn, tile, oracle_error):
+    """n chains of a statistics sweep against the oracle: `same` [n] says whose recorded entries equal the oracle's bit for bit;
+    gpu_final / orc_final [n, >= D] are the states the chains end in (the oracle's may carry derived quantities after the D
+    components). Every chain that differs in either must pass audit_divergence at its first differing row. gpu_rows / orc_rows
+    [rows, n, D]: every component as recorded at thin 1 (None when the run cannot localise a decision: thin > 1 or a monitored
+    subset). oracle_trace(k) -> the oracle's trace rows (OracleSampler.trace_rows) of chain k over its burn + sample sweeps.
+    -> (indices of the chains that differ, how many were audited as ties)"""
+    D = gpu_final.shape[1]
+    same = same & (gpu_final.view(np.uint64) == orc_final[:, :D].view(np.uint64)).all(axis=1)
+    div = np.flatnonzero(~same)
+    audited = 0
+    for c in div:
+        assert gpu_rows is not None, f"chain {c} differs at thin > 1 or on a monitored subset: its decisions cannot be localised"
+        g = np.vstack([gpu_rows[:, c], gpu_final[c]])
+        o = np.vstack([orc_rows[:, c], orc_final[c, :D]])
+        r = int(np.flatnonzero((g.view(np.uint64) != o.view(np.uint64)).any(axis=1))[0])
+        assert r > 0, f"chain {c} differs already in its first recorded row: the divergence lies in the burn and cannot be localised"
+        tr = oracle_trace(int(c))
+        sweep = burn + r - 1
+        audit_divergence(prog, consts, tr[sweep * D:(sweep + 1) * D], g[r - 1], g[r], o[r], tile, oracle_error)
+        audited += 1
+    return div, audited
+
+
 def oracle_decisions_agree(prog, consts, steps, start, tile, oracle_error):
     """Every traced step of the oracle, from state `start`: its decision is exp(delta*) > u unless |log u - delta*| is within the
     bound -- the audit accepts the oracle's own decisions. -> the smallest |log u - delta*| / bound seen."""

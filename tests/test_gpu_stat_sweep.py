@@ -189,25 +189,17 @@ def test_specialised_statistics_sweep_chain_for_chain_against_the_oracle(gpu_pkg
         assert a.shape == b.shape, (k, a.shape, b.shape)
         same &= (a.view(np.uint64) == b.view(np.uint64)).reshape(a.shape[0], C, -1).all(axis=(0, 2))
     D = final.shape[1]
-    same &= (final.view(np.uint64) == ofinal[:, :D].view(np.uint64)).all(axis=1)
-    div = np.flatnonzero(~same)
-    audited = 0
-    for c in div:
-        assert cs["thin"] == 1 and cs["monitor"] is None, f"chain {c} differs at thin {cs['thin']}: its decisions cannot be localised"
-        g = _components(s, d, names)[:, c]
-        o = np.concatenate([np.asarray(ref[n], np.float64).reshape(cs["sample"], C, -1)[:, c] for n in names], axis=1)
-        g = np.vstack([g, final[c]])
-        o = np.vstack([o, ofinal[c, :D]])
-        r = int(np.flatnonzero((g.view(np.uint64) != o.view(np.uint64)).any(axis=1))[0])
-        assert r > 0, f"chain {c} differs already in its first recorded row: the divergence lies in the burn and cannot be localised"
-        orc_s = orc.OracleSampler(cs["model"], cs["odata"], cs["params"], seed=cs["seed"], chain=cs["first"] + int(c), comp_options=comp_options)
+
+    def trace(c):
+        orc_s = orc.OracleSampler(cs["model"], cs["odata"], cs["params"], seed=cs["seed"], chain=cs["first"] + c, comp_options=comp_options)
         orc_s.trace((cs["burn"] + cs["sample"]) * D)
         orc_s.burn(cs["burn"])
         orc_s.sample(cs["sample"])
-        tr = orc_s.trace_rows()
-        sweep = cs["burn"] + r - 1
-        sc.audit_divergence(s._program, consts, tr[sweep * D:(sweep + 1) * D], g[r - 1], g[r], o[r], tile, cs["err"])
-        audited += 1
+        return orc_s.trace_rows()
+    rows = cs["thin"] == 1 and cs["monitor"] is None
+    g = _components(s, d, names) if rows else None
+    o = np.concatenate([np.asarray(ref[n], np.float64).reshape(cs["sample"], C, -1) for n in names], axis=2) if rows else None
+    div, audited = sc.compare_and_audit(s._program, consts, same, g, final, o, ofinal, trace, cs["burn"], tile, cs["err"])
     _report(f"{name}: {C} chains compared, {div.size} divergent, {audited} audited as ties; worst err/bound specialised: "
             f"stat {worst['stat']:.3g}, term {worst['term']:.3g}; oracle {t_orc:.1f} s on {os.cpu_count()} cores")
 
