@@ -2198,6 +2198,7 @@ extern "C" int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uin
   return 0;
 }
 
+#include "amwg_summary_scratch.h"
 #include "amwg_summary.cuh"
 #include "amwg_summary_loo.cuh"
 #include "amwg_summary_ppc.cuh"

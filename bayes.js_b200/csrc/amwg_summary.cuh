@@ -40,10 +40,14 @@
 namespace summary {
 
 constexpr int kMaxPrefixes = 32;      // distinct prefixes per entry and pass (order statistics being selected at once)
-// CTAs per entry of the chain-wise kernels (fewer when there are fewer 256-chain groups): a fixed number, not the device's SM
-// count, because it sets the merge order of the moments and so their last bits; ~9 CTAs per SM of an H100.
+// CTAs per entry of the chain-wise kernels at most (chain_ctas): a fixed number, not the device's SM count; ~9 CTAs per SM of an
+// H100.
 constexpr long long kChainCtas = 1184;
 static_assert(kNestedCtas == kChainCtas, "amwg_nested.cuh caps the segment kernel's grid like the chain-wise kernels");
+
+// CTAs of a grid-stride kernel over n chains (or draws): min(ceil(n / 256), kChainCtas). It depends on n only, so the order in
+// which the per-CTA records are merged, and with it the last bits of the result, is fixed.
+inline long long chain_ctas(long long n) { return std::min((n + 255) / 256, kChainCtas); }
 
 __device__ __forceinline__ unsigned long long ordered_key(double x) {
   unsigned long long u = (unsigned long long)__double_as_longlong(x);
@@ -141,8 +145,8 @@ __global__ void __launch_bounds__(256) amwg_digit_hist_kernel(const double* __re
 // CTAs per entry of the counting kernels (digit_hist, the histograms): at most kChainCtas, doubled while one CTA would see 2^32
 // values or more, because its shared bins are 32-bit (rows < 2^32 is checked by the callers).
 inline int64_t count_ctas(int64_t chains, int64_t rows) {
-  int64_t bx = std::min<int64_t>((chains + 255) / 256, kChainCtas);
-  while (bx < (chains + 255) / 256 && ((chains + bx - 1) / bx) * rows >= ((int64_t)1 << 32)) bx *= 2;
+  int64_t bx = chain_ctas(chains);
+  while (256 * bx < chains && ((chains + bx - 1) / bx) * rows >= ((int64_t)1 << 32)) bx *= 2;     // bx < ceil(chains / 256)
   return bx;
 }
 
@@ -884,29 +888,13 @@ __global__ void __launch_bounds__(256) amwg_nested_seg_kernel(const double* __re
 extern "C" int amwg_summary_moments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, double* host_stats) {
   if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_moments: empty sample block");
   if (!dev_samples || !host_stats) return fail("amwg_summary_moments: null pointer");
-  CUDA_TRY(cudaSetDevice(device));
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);     // depends on `chains` only: a fixed merge order
-  // scratch that lives as long as the process (per device, grown on demand): no cudaMalloc / cudaFree on the path of a call
-  struct Scratch { void* p = nullptr; size_t bytes = 0; };
-  static Scratch scratch[64];
-  static std::mutex scratch_mu;
-  const size_t need_partial = (size_t)entries * bx * sizeof(summary::Moments), need_out = (size_t)entries * 4 * sizeof(double);
-  const size_t need = ((need_partial + 255) / 256) * 256 + need_out;
-  summary::Moments* partial = nullptr;
-  double* d_out = nullptr;
-  {
-    std::lock_guard<std::mutex> lock(scratch_mu);
-    if (device < 0 || device >= 64) return fail("amwg_summary_moments: device index out of range");
-    Scratch& sc = scratch[device];
-    if (sc.bytes < need) {
-      if (sc.p) cudaFree(sc.p);
-      sc.p = nullptr; sc.bytes = 0;
-      CUDA_TRY(cudaMalloc(&sc.p, need));
-      sc.bytes = need;
-    }
-    partial = reinterpret_cast<summary::Moments*>(sc.p);
-    d_out = reinterpret_cast<double*>(reinterpret_cast<char*>(sc.p) + ((need_partial + 255) / 256) * 256);
-  }
+  if (summary::select_device(device, "amwg_summary_moments")) return -1;
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
+  const size_t need_out = (size_t)entries * 4 * sizeof(double);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_moments", {(size_t)entries * bx * sizeof(summary::Moments), need_out})) return -1;
+  auto* partial = sc.part<summary::Moments>(0);
+  auto* d_out = sc.part<double>(1);
   summary::amwg_chain_moments_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, partial);
   summary::amwg_merge_moments_kernel<<<(unsigned)entries, 1024>>>(partial, (int)bx, d_out);
   cudaError_t e = cudaGetLastError();
@@ -922,10 +910,8 @@ extern "C" int amwg_summary_digit_hist(int device, const double* dev_samples, in
   if (n_prefix < 1 || n_prefix > summary::kMaxPrefixes) return fail("amwg_summary_digit_hist: n_prefix must be 1.." + std::to_string(summary::kMaxPrefixes));
   if (rows >= (int64_t)1 << 32) return fail("amwg_summary_digit_hist: more than 2^32 rows");
   if (!dev_samples || !dev_prefix || !dev_counts) return fail("amwg_summary_digit_hist: null pointer");
-  CUDA_TRY(cudaSetDevice(device));
-  // a CTA's shared bins are 32-bit: bound the values one CTA sees by 2^32 (rows < 2^32 and the grid below keeps chains per CTA small)
-  int64_t bx = std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
-  while (bx < (chains + 255) / 256 && ((chains + bx - 1) / bx) * rows >= ((int64_t)1 << 32)) bx *= 2;
+  if (summary::select_device(device, "amwg_summary_digit_hist")) return -1;
+  const int64_t bx = summary::count_ctas(chains, rows);
   summary::amwg_digit_hist_kernel<<<dim3((unsigned)bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, pass,
                                                                                   reinterpret_cast<const unsigned long long*>(dev_prefix), n_prefix,
                                                                                   reinterpret_cast<unsigned long long*>(dev_counts));
@@ -942,33 +928,19 @@ extern "C" int amwg_summary_autocov(int device, const double* dev_samples, int64
   if (lag0 < 0 || lag0 + n_lags > rows / 2)
     return fail("amwg_summary_autocov: the lag window [lag0, lag0 + n_lags) must lie in [0, rows/2) (rows/2 = " + std::to_string(rows / 2) + ")");
   if (!dev_samples || !host_out) return fail("amwg_summary_autocov: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_autocov: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_autocov")) return -1;
   const int ns = host_thresholds ? 3 : 1;
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);     // depends on `chains` only: a fixed merge order
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
   const size_t rec = (size_t)entries * ns, sums = rec * n_lags;
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_pmom = up(rec * bx * sizeof(summary::Moments)), b_psum = up(sums * bx * sizeof(double));
-  const size_t b_mom = up(rec * 4 * sizeof(double)), b_sum = up(sums * sizeof(double)), b_thr = up((size_t)entries * 2 * sizeof(double));
-  const size_t need = b_pmom + b_psum + b_mom + b_sum + b_thr;
-  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
-  struct Scratch { void* p = nullptr; size_t bytes = 0; };
-  static Scratch scratch[64];
-  static std::mutex scratch_mu;
-  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
-  Scratch& sc = scratch[device];
-  if (sc.bytes < need) {
-    if (sc.p) cudaFree(sc.p);
-    sc.p = nullptr; sc.bytes = 0;
-    CUDA_TRY(cudaMalloc(&sc.p, need));
-    sc.bytes = need;
-  }
-  char* base = reinterpret_cast<char*>(sc.p);
-  auto* pmom = reinterpret_cast<summary::Moments*>(base);
-  auto* psum = reinterpret_cast<double*>(base + b_pmom);
-  auto* d_mom = reinterpret_cast<double*>(base + b_pmom + b_psum);
-  auto* d_sum = reinterpret_cast<double*>(base + b_pmom + b_psum + b_mom);
-  auto* d_thr = reinterpret_cast<double*>(base + b_pmom + b_psum + b_mom + b_sum);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_autocov", {rec * bx * sizeof(summary::Moments), sums * bx * sizeof(double), rec * 4 * sizeof(double),
+                                                  sums * sizeof(double), (size_t)entries * 2 * sizeof(double)}))
+    return -1;
+  auto* pmom = sc.part<summary::Moments>(0);
+  auto* psum = sc.part<double>(1);
+  auto* d_mom = sc.part<double>(2);
+  auto* d_sum = sc.part<double>(3);
+  auto* d_thr = sc.part<double>(4);
   if (host_thresholds) CUDA_TRY(cudaMemcpy(d_thr, host_thresholds, (size_t)entries * 2 * sizeof(double), cudaMemcpyHostToDevice));
   for (int k0 = 0; k0 < n_lags; k0 += summary::kLagSlots) {                 // one pass over the block per kLagSlots lags
     const int nk = std::min(summary::kLagSlots, n_lags - k0);
@@ -1002,35 +974,21 @@ extern "C" int amwg_summary_rank_sort(int device, const double* dev_samples, int
   if (n >= ((int64_t)1 << 32) || chains >= ((int64_t)1 << 32))
     return fail("amwg_summary_rank_sort: 2 * (rows / 2) * chains = " + std::to_string(n) + " draws, the indices hold fewer than 2^32");
   if (!dev_samples || !dev_keys || !dev_index) return fail("amwg_summary_rank_sort: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_rank_sort: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_rank_sort")) return -1;
   const long long tiles = (n + summary::kSortTile - 1) / summary::kSortTile;
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_hist = up(8 * 256 * sizeof(unsigned long long)), b_tab = up((size_t)256 * tiles * sizeof(unsigned));
-  const size_t need = b_hist + 2 * b_tab;
-  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
-  struct Scratch { void* p = nullptr; size_t bytes = 0; };
-  static Scratch scratch[64];
-  static std::mutex scratch_mu;
-  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the last pass
-  Scratch& sc = scratch[device];
-  if (sc.bytes < need) {
-    if (sc.p) cudaFree(sc.p);
-    sc.p = nullptr; sc.bytes = 0;
-    CUDA_TRY(cudaMalloc(&sc.p, need));
-    sc.bytes = need;
-  }
-  char* base = reinterpret_cast<char*>(sc.p);
-  auto* hist = reinterpret_cast<unsigned long long*>(base);
-  auto* counts = reinterpret_cast<unsigned*>(base + b_hist);
-  auto* offsets = reinterpret_cast<unsigned*>(base + b_hist + b_tab);
+  const size_t b_tab = (size_t)256 * tiles * sizeof(unsigned);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_rank_sort", {8 * 256 * sizeof(unsigned long long), b_tab, b_tab})) return -1;
+  auto* hist = sc.part<unsigned long long>(0);
+  auto* counts = sc.part<unsigned>(1);
+  auto* offsets = sc.part<unsigned>(2);
   auto* keys = reinterpret_cast<unsigned long long*>(dev_keys);
   summary::RankSource src{dev_samples, rows, chains, (size_t)entries * chains, entry, !std::isnan(centre), centre, nullptr, nullptr};
   CUDA_TRY(cudaMemset(hist, 0, 8 * 256 * sizeof(unsigned long long)));
   // one read of the block forms all eight digit histograms. A digit position where one bin holds every key has the same digit
   // in all keys: its pass would move nothing and is skipped. The first executed pass forms the keys from the block again, into
   // the half that makes the last pass end in the first half.
-  const unsigned gx = (unsigned)std::min<long long>((n + 255) / 256, summary::kChainCtas);
+  const unsigned gx = (unsigned)summary::chain_ctas(n);
   summary::amwg_rank_hist_kernel<<<gx, 256>>>(src, n, hist);
   CUDA_TRY(cudaGetLastError());
   std::vector<unsigned long long> h(8 * 256);
@@ -1067,8 +1025,7 @@ extern "C" int amwg_summary_rank_count(int device, const uint64_t* dev_q, int64_
   if (nq < 1 || nr < 1) return fail("amwg_summary_rank_count: empty key array");
   if (nq >= ((int64_t)1 << 32) || nr >= ((int64_t)1 << 32)) return fail("amwg_summary_rank_count: more than 2^32 - 1 keys");
   if (!dev_q || !dev_r || !dev_acc) return fail("amwg_summary_rank_count: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_rank_count: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_rank_count")) return -1;
   const unsigned grid = (unsigned)((nq + nr + summary::kMergeTile - 1) / summary::kMergeTile);
   auto* q = reinterpret_cast<const unsigned long long*>(dev_q);
   auto* r = reinterpret_cast<const unsigned long long*>(dev_r);
@@ -1084,9 +1041,8 @@ extern "C" int amwg_summary_rank_z(int device, const int64_t* dev_acc, const uin
   if (n < 1 || n >= ((int64_t)1 << 32)) return fail("amwg_summary_rank_z: n must be 1..2^32-1");
   if (total < n || total >= ((int64_t)1 << 52)) return fail("amwg_summary_rank_z: total must be at least n and below 2^52");
   if (!dev_acc || !dev_index || !dev_z) return fail("amwg_summary_rank_z: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_rank_z: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
-  const unsigned grid = (unsigned)std::min<long long>((n + 255) / 256, summary::kChainCtas);
+  if (summary::select_device(device, "amwg_summary_rank_z")) return -1;
+  const unsigned grid = (unsigned)summary::chain_ctas(n);
   summary::amwg_rank_z_kernel<<<grid, 256>>>(reinterpret_cast<const long long*>(dev_acc), dev_index, n, (double)total, dev_z);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
@@ -1097,12 +1053,11 @@ extern "C" int amwg_summary_finite_range(int device, const double* dev_samples, 
                                          double* dev_range, int64_t* dev_nonfinite) {
   if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_finite_range: empty sample block");
   if (!dev_samples || !dev_range || !dev_nonfinite) return fail("amwg_summary_finite_range: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_finite_range: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_finite_range")) return -1;
   auto* keys = reinterpret_cast<unsigned long long*>(dev_range);
   auto* nonfinite = reinterpret_cast<unsigned long long*>(dev_nonfinite);
   const unsigned small = (unsigned)std::min<int64_t>((entries + 255) / 256, 1024);
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
   summary::amwg_range_init_kernel<<<small, 256>>>(keys, nonfinite, entries);
   summary::amwg_finite_range_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, keys, nonfinite);
   summary::amwg_range_final_kernel<<<small, 256>>>(keys, entries);
@@ -1117,8 +1072,7 @@ extern "C" int amwg_summary_histogram(int device, const double* dev_samples, int
   if (bins < 1 || bins > summary::kMaxHistBins) return fail("amwg_summary_histogram: bins must be 1.." + std::to_string(summary::kMaxHistBins));
   if (rows >= (int64_t)1 << 32) return fail("amwg_summary_histogram: more than 2^32 rows");
   if (!dev_samples || !dev_edges || !dev_counts) return fail("amwg_summary_histogram: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_histogram: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_histogram")) return -1;
   const size_t smem = (size_t)(bins + 1) * sizeof(double) + (size_t)(bins + 3) * sizeof(unsigned);
   CUDA_TRY(cudaFuncSetAttribute(summary::amwg_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t bx = summary::count_ctas(chains, rows);
@@ -1136,7 +1090,6 @@ extern "C" int amwg_summary_histogram2d(int device, const double* dev_samples, i
   if (n_pairs < 1 || n_pairs > summary::kMaxPairs) return fail("amwg_summary_histogram2d: n_pairs must be 1.." + std::to_string(summary::kMaxPairs));
   if (rows >= (int64_t)1 << 32) return fail("amwg_summary_histogram2d: more than 2^32 rows");
   if (!dev_samples || !host_pairs || !dev_edges || !dev_counts) return fail("amwg_summary_histogram2d: null pointer");
-  if (device < 0 || device >= 64) return fail("amwg_summary_histogram2d: device index out of range");
   summary::PairList pl;
   for (int i = 0; i < n_pairs; ++i) {
     pl.a[i] = host_pairs[2 * i];
@@ -1144,7 +1097,7 @@ extern "C" int amwg_summary_histogram2d(int device, const double* dev_samples, i
     if (pl.a[i] < 0 || pl.a[i] >= entries || pl.b[i] < 0 || pl.b[i] >= entries)
       return fail("amwg_summary_histogram2d: pair " + std::to_string(i) + " names an entry outside [0, entries)");
   }
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_histogram2d")) return -1;
   const size_t smem = (size_t)2 * (bins + 1) * sizeof(double) + (size_t)bins * bins * sizeof(unsigned);
   CUDA_TRY(cudaFuncSetAttribute(summary::amwg_hist2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t bx = summary::count_ctas(chains, rows);
@@ -1153,14 +1106,6 @@ extern "C" int amwg_summary_histogram2d(int device, const double* dev_samples, i
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
   return 0;
-}
-
-// bytes of device scratch amwg_summary_comoments uses (include/amwg.h states the formula; sample_summary counts it)
-static size_t comoments_scratch_bytes(int32_t n_sel, int64_t chains) {
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t tiles = (size_t)summary::co_tiles(summary::co_blocks(n_sel));
-  const size_t reps = (size_t)summary::co_reps(summary::co_blocks(n_sel));
-  return up((size_t)n_sel * chains * 8) + up((size_t)n_sel * 8) + up((size_t)summary::co_ctas(chains) * reps * tiles * 64 * 8) + up(2 * tiles * 64 * 8);
 }
 
 extern "C" int amwg_summary_comoments(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
@@ -1175,34 +1120,20 @@ extern "C" int amwg_summary_comoments(int device, const double* dev_samples, int
     sel.e[i] = host_sel[i];
   }
   if (rows > (((int64_t)1 << 53) - 1) / chains) return fail("amwg_summary_comoments: rows * chains must be below 2^53");
-  if (device < 0 || device >= 64) return fail("amwg_summary_comoments: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_comoments")) return -1;
   const int nb = summary::co_blocks(n_sel), tiles = summary::co_tiles(nb), n_vals = tiles * 64;
   const long long gx = summary::co_ctas(chains), parts = gx * summary::co_reps(nb);
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_xbar = up((size_t)n_sel * chains * 8), b_m = up((size_t)n_sel * 8), b_part = up((size_t)parts * n_vals * 8);
-  const size_t need = comoments_scratch_bytes(n_sel, chains);
-  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
-  struct Scratch { void* p = nullptr; size_t bytes = 0; };
-  static Scratch scratch[64];
-  static std::mutex scratch_mu;
-  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
-  Scratch& sc = scratch[device];
-  if (sc.bytes < need) {
-    if (sc.p) cudaFree(sc.p);
-    sc.p = nullptr; sc.bytes = 0;
-    CUDA_TRY(cudaMalloc(&sc.p, need));
-    sc.bytes = need;
-  }
-  char* base = reinterpret_cast<char*>(sc.p);
-  auto* xbar = reinterpret_cast<double*>(base);
-  auto* m = reinterpret_cast<double*>(base + b_xbar);
-  auto* part = reinterpret_cast<double*>(base + b_xbar + b_m);
-  auto* tw = reinterpret_cast<double*>(base + b_xbar + b_m + b_part);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_comoments", {(size_t)n_sel * chains * 8, (size_t)n_sel * 8, (size_t)parts * n_vals * 8, (size_t)2 * n_vals * 8}))
+    return -1;
+  auto* xbar = sc.part<double>(0);
+  auto* m = sc.part<double>(1);
+  auto* part = sc.part<double>(2);
+  auto* tw = sc.part<double>(3);
   double* tb = tw + n_vals;
   summary::SelList ident{};
   for (int i = 0; i < n_sel; ++i) ident.e[i] = i;
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
   const unsigned sx = (unsigned)((n_vals + 255) / 256);
   summary::amwg_chain_means_kernel<<<dim3(bx, (unsigned)n_sel), 256>>>(dev_samples, rows, entries, chains, sel, xbar);
   summary::amwg_shard_mean_kernel<<<(unsigned)n_sel, 256>>>(xbar, chains, m);
@@ -1235,13 +1166,6 @@ extern "C" int amwg_summary_comoments(int device, const double* dev_samples, int
   return 0;
 }
 
-// bytes of device scratch amwg_summary_nested uses (include/amwg.h states the formula; sample_summary counts it)
-static size_t nested_scratch_bytes(int32_t entries, int64_t chains, int64_t n_seg) {
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t bx = (size_t)summary::nested_seg_ctas(n_seg);
-  return up((size_t)entries * chains * 16) + up((size_t)entries * bx * 32) + up((size_t)entries * 32) + up((size_t)entries * 64);
-}
-
 extern "C" int amwg_summary_nested(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int64_t first_chain,
                                    int64_t superchain_size, double* host_out) {
   if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_nested: empty sample block");
@@ -1249,33 +1173,19 @@ extern "C" int amwg_summary_nested(int device, const double* dev_samples, int64_
   if (superchain_size < 1) return fail("amwg_summary_nested: superchain_size must be >= 1");
   if (first_chain < 0) return fail("amwg_summary_nested: first_chain must be >= 0");
   if (first_chain > ((int64_t)1 << 53) - chains) return fail("amwg_summary_nested: first_chain + chains must be at most 2^53");
-  if (device < 0 || device >= 64) return fail("amwg_summary_nested: device index out of range");
-  CUDA_TRY(cudaSetDevice(device));
+  if (summary::select_device(device, "amwg_summary_nested")) return -1;
   const long long M = superchain_size, n_seg = summary::nested_segments(first_chain, chains, M);
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
   const unsigned sx = (unsigned)summary::nested_seg_ctas(n_seg);     // depends on n_seg only: a fixed merge order
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_chain = up((size_t)entries * chains * 16), b_part = up((size_t)entries * sx * sizeof(summary::Moments));
-  const size_t b_out = up((size_t)entries * 4 * sizeof(double));
-  const size_t need = nested_scratch_bytes(entries, chains, n_seg);
-  // scratch that lives as long as the process (per device, grown on demand), as in amwg_summary_moments
-  struct Scratch { void* p = nullptr; size_t bytes = 0; };
-  static Scratch scratch[64];
-  static std::mutex scratch_mu;
-  std::lock_guard<std::mutex> lock(scratch_mu);           // held for the call: the buffers are in use until the copy back
-  Scratch& sc = scratch[device];
-  if (sc.bytes < need) {
-    if (sc.p) cudaFree(sc.p);
-    sc.p = nullptr; sc.bytes = 0;
-    CUDA_TRY(cudaMalloc(&sc.p, need));
-    sc.bytes = need;
-  }
-  char* base = reinterpret_cast<char*>(sc.p);
-  auto* cm = reinterpret_cast<double*>(base);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_nested", {(size_t)entries * chains * 16, (size_t)entries * sx * sizeof(summary::Moments),
+                                                 (size_t)entries * 4 * sizeof(double), (size_t)entries * 2 * sizeof(summary::Moments)}))
+    return -1;
+  auto* cm = sc.part<double>(0);
   auto* cw = cm + (size_t)entries * chains;
-  auto* part = reinterpret_cast<summary::Moments*>(base + b_chain);
-  auto* d_out = reinterpret_cast<double*>(base + b_chain + b_part);
-  auto* cut = reinterpret_cast<summary::Moments*>(base + b_chain + b_part + b_out);
+  auto* part = sc.part<summary::Moments>(1);
+  auto* d_out = sc.part<double>(2);
+  auto* cut = sc.part<summary::Moments>(3);
   summary::amwg_nested_chain_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, cm, cw);
   summary::amwg_nested_seg_kernel<<<dim3(sx, (unsigned)entries), 256>>>(cm, cw, chains, first_chain, M, rows, n_seg, part, cut);
   summary::amwg_merge_moments_kernel<<<(unsigned)entries, 1024>>>(part, (int)sx, d_out);

@@ -12,7 +12,7 @@
 //                                     K_l3 sorts them)
 //   K_l3  amwg_loo_fit_kernel       : one CTA per point: the shards' tails gathered and sorted (bitonic, in global scratch), the
 //                                     generalised Pareto fit of amwg_loo.cuh, the smoothed tail weights and their two sums
-// Included at the end of amwg_kernels.cu, after amwg_summary.cuh (cta_sum, amwg_merge_sums_kernel, kChainCtas).
+// Included at the end of amwg_kernels.cu, after amwg_summary.cuh (cta_sum, amwg_merge_sums_kernel, chain_ctas).
 #pragma once
 
 #include "amwg_loo.cuh"
@@ -181,25 +181,7 @@ __global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double*
   if (t == 0) { out[4 * p] = k; out[4 * p + 1] = tw; out[4 * p + 2] = twl; out[4 * p + 3] = (double)total; }
 }
 
-// per-device scratch that lives as long as the process, grown on demand (as amwg_summary_moments')
-struct LooScratch { void* p = nullptr; size_t bytes = 0; };
-inline int loo_scratch(int device, size_t need, void** out, const char* who) {
-  static LooScratch pool[64];
-  if (device < 0 || device >= 64) return fail(std::string(who) + ": device index out of range");
-  LooScratch& sc = pool[device];
-  if (sc.bytes < need) {
-    if (sc.p) cudaFree(sc.p);
-    sc.p = nullptr; sc.bytes = 0;
-    CUDA_TRY(cudaMalloc(&sc.p, need));
-    sc.bytes = need;
-  }
-  *out = sc.p;
-  return 0;
-}
-
 }  // namespace summary
-
-static std::mutex g_loo_mu;               // the calls below share one scratch pool per device
 
 // The checks of amwg_loo_pointwise and amwg_ppc_pointwise, before anything runs: every program well formed and an expression (no
 // sum, plate, loop, store or cache word), each index inside its table and, for the body programs `bodies`, each data read inside
@@ -265,24 +247,20 @@ static int check_pointwise_programs(amwg_sampler* s, const char* who, const int3
   return 0;
 }
 
-// Copies the checked program, its constants, the fold table and the handle's data column pointers into the per-device pool and
-// folds the constants on the device (K_l0), for a pointwise kernel with `smem` bytes of dynamic shared memory. The caller holds
-// g_loo_mu and has selected the handle's device.
-static int stage_pointwise_program(amwg_sampler* s, const char* who, const void* kernel, size_t smem, const int32_t* host_code,
-                                   int32_t n_code, const double* host_consts, int32_t n_consts, const int32_t* host_fold_prog,
-                                   const int32_t* host_fold_dst, int32_t n_fold, int** d_code_out, double** d_consts_out,
-                                   summary::LooColumns** d_cols_out) {
-  const size_t b_code = ((size_t)n_code * 4 + 15) & ~(size_t)15, b_consts = ((size_t)n_consts * 8 + 15) & ~(size_t)15;
-  const size_t b_fold = (((size_t)std::max(n_fold, 1) * 4) + 15) & ~(size_t)15;
-  void* base = nullptr;
-  const size_t b_cols = (sizeof(summary::LooColumns) + 15) & ~(size_t)15;
-  if (summary::loo_scratch(s->device, b_code + b_consts + 2 * b_fold + b_cols, &base, who)) return -1;
-  char* cb = reinterpret_cast<char*>(base);
-  int* d_code = reinterpret_cast<int*>(cb);
-  double* d_consts = reinterpret_cast<double*>(cb + b_code);
-  int* d_fp = reinterpret_cast<int*>(cb + b_code + b_consts);
-  int* d_fd = reinterpret_cast<int*>(cb + b_code + b_consts + b_fold);
-  auto* d_cols = reinterpret_cast<summary::LooColumns*>(cb + b_code + b_consts + 2 * b_fold);
+// Copies the checked program, its constants, the fold table and the handle's data column pointers into the device's scratch pool
+// and folds the constants on the device (K_l0), for a pointwise kernel with `smem` bytes of dynamic shared memory. The caller has
+// selected the handle's device and passes its lease `sc`, which keeps the staged program locked until the kernel has finished.
+static int stage_pointwise_program(amwg_sampler* s, summary::Scratch& sc, const char* who, const void* kernel, size_t smem,
+                                   const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
+                                   const int32_t* host_fold_prog, const int32_t* host_fold_dst, int32_t n_fold, int** d_code_out,
+                                   double** d_consts_out, summary::LooColumns** d_cols_out) {
+  const size_t b_fold = (size_t)std::max(n_fold, 1) * 4;
+  if (sc.acquire(s->device, who, {(size_t)n_code * 4, (size_t)n_consts * 8, b_fold, b_fold, sizeof(summary::LooColumns)})) return -1;
+  int* d_code = sc.part<int>(0);
+  double* d_consts = sc.part<double>(1);
+  int* d_fp = sc.part<int>(2);
+  int* d_fd = sc.part<int>(3);
+  auto* d_cols = sc.part<summary::LooColumns>(4);
   CUDA_TRY(cudaMemcpy(d_code, host_code, (size_t)n_code * 4, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_consts, host_consts, (size_t)n_consts * 8, cudaMemcpyHostToDevice));
   if (n_fold > 0) {
@@ -314,13 +292,13 @@ extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int
   if (smem > kSmemBudget) return fail("amwg_loo_pointwise: the program and its constants exceed the shared memory budget");
   if (check_pointwise_programs(s, who, host_code, n_code, n_consts, {body_prog}, host_fold_prog, host_fold_dst, n_fold, entries, p0, n_points))
     return -1;
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (summary::select_device(s->device, who)) return -1;
   CUDA_TRY(cudaStreamSynchronize(s->stream));               // the sampler's stream wrote the block
   int* d_code = nullptr;
   double* d_consts = nullptr;
   summary::LooColumns* d_cols = nullptr;
-  if (stage_pointwise_program(s, who, (const void*)summary::amwg_loo_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
+  summary::Scratch sc;
+  if (stage_pointwise_program(s, sc, who, (const void*)summary::amwg_loo_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
                               host_fold_prog, host_fold_dst, n_fold, &d_code, &d_consts, &d_cols))
     return -1;
   const long long C = (long long)s->a.C;
@@ -340,19 +318,16 @@ extern "C" int amwg_loo_reduce(int device, const double* dev_ll, int64_t rows, i
   if (points > 65535) return fail("amwg_loo_reduce: at most 65535 points per call");
   if (tail_cap < 1 || tail_cap > loo::kMaxTail) return fail("amwg_loo_reduce: tail_cap must be 1.." + std::to_string(loo::kMaxTail));
   if (!dev_ll || !host_llmin || !host_llmax || !host_cut || !dev_tail || !dev_count || !host_sums) return fail("amwg_loo_reduce: null pointer");
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(device));
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);     // depends on `chains` only: a fixed merge order
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_vec = up((size_t)points * 8), b_part = up((size_t)points * 3 * bx * 8), b_sums = up((size_t)points * 3 * 8);
-  void* base = nullptr;
-  if (summary::loo_scratch(device, 3 * b_vec + b_part + b_sums, &base, "amwg_loo_reduce")) return -1;
-  char* cb = reinterpret_cast<char*>(base);
-  double* d_min = reinterpret_cast<double*>(cb);
-  double* d_max = reinterpret_cast<double*>(cb + b_vec);
-  double* d_cut = reinterpret_cast<double*>(cb + 2 * b_vec);
-  double* d_part = reinterpret_cast<double*>(cb + 3 * b_vec);
-  double* d_sums = reinterpret_cast<double*>(cb + 3 * b_vec + b_part);
+  if (summary::select_device(device, "amwg_loo_reduce")) return -1;
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
+  const size_t b_vec = (size_t)points * 8;
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_loo_reduce", {b_vec, b_vec, b_vec, (size_t)points * 3 * bx * 8, (size_t)points * 3 * 8})) return -1;
+  double* d_min = sc.part<double>(0);
+  double* d_max = sc.part<double>(1);
+  double* d_cut = sc.part<double>(2);
+  double* d_part = sc.part<double>(3);
+  double* d_sums = sc.part<double>(4);
   CUDA_TRY(cudaMemcpy(d_min, host_llmin, (size_t)points * 8, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_max, host_llmax, (size_t)points * 8, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_cut, host_cut, (size_t)points * 8, cudaMemcpyHostToDevice));
@@ -369,19 +344,16 @@ extern "C" int amwg_loo_fit(int device, const double* dev_tails, const int32_t* 
   if (shards < 1 || points < 1) return fail("amwg_loo_fit: shards and points must be >= 1");
   if (tail_cap < 8 || tail_cap > loo::kMaxTail || (tail_cap & (tail_cap - 1))) return fail("amwg_loo_fit: tail_cap must be a power of two in 8.." + std::to_string(loo::kMaxTail));
   if (!dev_tails || !dev_counts || !host_llmin || !host_cut || !host_skip || !host_out) return fail("amwg_loo_fit: null pointer");
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(device));
-  auto up = [](size_t b) { return ((b + 255) / 256) * 256; };
-  const size_t b_vec = up((size_t)points * 8), b_work = up((size_t)points * tail_cap * 8), b_out = up((size_t)points * 4 * 8);
-  void* base = nullptr;
-  if (summary::loo_scratch(device, 3 * b_vec + 2 * b_work + b_out, &base, "amwg_loo_fit")) return -1;
-  char* cb = reinterpret_cast<char*>(base);
-  double* d_min = reinterpret_cast<double*>(cb);
-  double* d_cut = reinterpret_cast<double*>(cb + b_vec);
-  int* d_skip = reinterpret_cast<int*>(cb + 2 * b_vec);
-  double* d_work = reinterpret_cast<double*>(cb + 3 * b_vec);
-  double* d_xs = reinterpret_cast<double*>(cb + 3 * b_vec + b_work);
-  double* d_out = reinterpret_cast<double*>(cb + 3 * b_vec + 2 * b_work);
+  if (summary::select_device(device, "amwg_loo_fit")) return -1;
+  const size_t b_vec = (size_t)points * 8, b_work = (size_t)points * tail_cap * 8;
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_loo_fit", {b_vec, b_vec, b_vec, b_work, b_work, (size_t)points * 4 * 8})) return -1;
+  double* d_min = sc.part<double>(0);
+  double* d_cut = sc.part<double>(1);
+  int* d_skip = sc.part<int>(2);
+  double* d_work = sc.part<double>(3);
+  double* d_xs = sc.part<double>(4);
+  double* d_out = sc.part<double>(5);
   CUDA_TRY(cudaMemcpy(d_min, host_llmin, (size_t)points * 8, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_cut, host_cut, (size_t)points * 8, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_skip, host_skip, (size_t)points * 4, cudaMemcpyHostToDevice));

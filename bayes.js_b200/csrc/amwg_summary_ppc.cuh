@@ -8,7 +8,7 @@
 //                                            chunk replaces M2 by sd, which makes T a sample block of (mean, sd, min, max).
 //   K_p2  amwg_threshold_counts_kernel     : grid (chain groups, entries): per entry the draws <, ==, > a threshold and NaN, summed
 //                                            in 64-bit integers (warp shuffles, then one atomic per warp): exact in any order.
-// Included at the end of amwg_kernels.cu, after amwg_summary_loo.cuh (the staging of pointwise programs, LooColumns, g_loo_mu).
+// Included at the end of amwg_kernels.cu, after amwg_summary_loo.cuh (the staging of pointwise programs, LooColumns).
 #pragma once
 
 #include "amwg_ppc.cuh"
@@ -112,13 +112,13 @@ extern "C" int amwg_ppc_pointwise(amwg_sampler* s, const int32_t* host_code, int
   std::vector<int> bodies(host_arg_progs, host_arg_progs + n_args);
   if (check_pointwise_programs(s, who, host_code, n_code, n_consts, bodies, host_fold_prog, host_fold_dst, n_fold, entries, p0, n_points))
     return -1;
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (summary::select_device(s->device, who)) return -1;
   CUDA_TRY(cudaStreamSynchronize(s->stream));               // the sampler's stream wrote the block
   int* d_code = nullptr;
   double* d_consts = nullptr;
   summary::LooColumns* d_cols = nullptr;
-  if (stage_pointwise_program(s, who, (const void*)summary::amwg_ppc_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
+  summary::Scratch sc;
+  if (stage_pointwise_program(s, sc, who, (const void*)summary::amwg_ppc_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
                               host_fold_prog, host_fold_dst, n_fold, &d_code, &d_consts, &d_cols))
     return -1;
   summary::PpcPrograms progs{{0, 0, 0}};
@@ -140,14 +140,13 @@ extern "C" int amwg_summary_threshold_counts(int device, const double* dev_sampl
   if (rows <= 0 || entries <= 0 || chains <= 0) return fail("amwg_summary_threshold_counts: empty block");
   if (entries > 65535) return fail("amwg_summary_threshold_counts: at most 65535 entries per call");
   if (!dev_samples || !host_thresholds || !dev_counts) return fail("amwg_summary_threshold_counts: null pointer");
-  std::lock_guard<std::mutex> lock(g_loo_mu);
-  CUDA_TRY(cudaSetDevice(device));
-  void* base = nullptr;
-  if (summary::loo_scratch(device, (size_t)entries * 8, &base, "amwg_summary_threshold_counts")) return -1;
-  double* d_thr = reinterpret_cast<double*>(base);
+  if (summary::select_device(device, "amwg_summary_threshold_counts")) return -1;
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_threshold_counts", {(size_t)entries * 8})) return -1;
+  double* d_thr = sc.part<double>(0);
   CUDA_TRY(cudaMemcpy(d_thr, host_thresholds, (size_t)entries * 8, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemset(dev_counts, 0, (size_t)entries * 4 * sizeof(int64_t)));
-  const unsigned bx = (unsigned)std::min<int64_t>((chains + 255) / 256, summary::kChainCtas);
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
   summary::amwg_threshold_counts_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, d_thr,
                                                                               reinterpret_cast<unsigned long long*>(dev_counts));
   CUDA_TRY(cudaGetLastError());

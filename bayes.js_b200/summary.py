@@ -12,7 +12,9 @@ amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R
 amwg_summary_rank_sort / _rank_count / _rank_z for the rank-normalised R-hat and bulk ESS of diagnostics="rank", and
 amwg_summary_finite_range / _histogram / _histogram2d for the posterior histograms of histogram=..., amwg_summary_comoments for
 the posterior covariance of covariance=..., and amwg_summary_nested for the nested R-hat of nested=...). There is no CPU fallback:
-without the library or a GPU the reducer raises.
+without the library or a GPU the reducer raises. Every reducer call first waits for torch's current stream, which wrote its
+inputs. The library's summary calls take their device scratch from one pool per device, grown on demand and held by each call
+until it returns; the memory checks add up the calls' requests, which bounds that pool from above.
 """
 from __future__ import annotations
 
@@ -148,10 +150,17 @@ class CudaBlockReducer:
         self._ffi = _ffi
         self.device = device
 
+    def _call(self, t, fn, *args) -> None:
+        """fn(device, *args), an ABI call on the library's default stream, once torch's current stream on t's device has finished
+        writing the tensors it reads (the caller's stream need not be the default one)."""
+        import torch
+        torch.cuda.current_stream(t.device).synchronize()
+        self._ffi.check(fn(self.device, *args))
+
     def moments(self, block) -> np.ndarray:
         rows, entries, chains = block.shape
         out = np.empty((entries, 4), dtype=np.float64)
-        self._ffi.check(self.L.amwg_summary_moments(self.device, block.data_ptr(), rows, entries, chains, out.ctypes.data))
+        self._call(block, self.L.amwg_summary_moments, block.data_ptr(), rows, entries, chains, out.ctypes.data)
         return out
 
     def digit_counts(self, block, npass: int, prefix_table: np.ndarray):
@@ -162,9 +171,8 @@ class CudaBlockReducer:
         dev = block.device
         pre = torch.from_numpy(prefix_table.view(np.int64).copy()).to(dev)
         counts = torch.zeros((entries, n_prefix, 256), dtype=torch.int64, device=dev)
-        torch.cuda.current_stream(dev).synchronize()
-        self._ffi.check(self.L.amwg_summary_digit_hist(self.device, block.data_ptr(), rows, entries, chains, npass,
-                                                       pre.data_ptr(), n_prefix, counts.data_ptr()))
+        self._call(block, self.L.amwg_summary_digit_hist, block.data_ptr(), rows, entries, chains, npass, pre.data_ptr(), n_prefix,
+                   counts.data_ptr())
         return counts
 
     def autocov(self, block, thresholds, lag0: int, n_lags: int) -> np.ndarray:
@@ -174,35 +182,27 @@ class CudaBlockReducer:
         ns = 1 if thresholds is None else 3
         out = np.empty((entries, ns, 4 + n_lags), dtype=np.float64)
         thr = None if thresholds is None else np.ascontiguousarray(thresholds, dtype=np.float64).reshape(entries, 2)
-        import torch
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_autocov(self.device, block.data_ptr(), rows, entries, chains,
-                                                    None if thr is None else thr.ctypes.data, lag0, n_lags, out.ctypes.data))
+        self._call(block, self.L.amwg_summary_autocov, block.data_ptr(), rows, entries, chains, None if thr is None else thr.ctypes.data,
+                   lag0, n_lags, out.ctypes.data)
         return out
 
     def rank_sort(self, block, entry: int, centre: float, keys, index) -> int:
         """Sorts the half-chain keys of `entry` (centre NaN: the draws; else |x - centre|) into keys[:n] (int64 tensor holding the
         uint64 keys, 2n long) with their positions in index[:n] (int32 tensor, 2n long); -> radix passes run. See
         amwg_summary_rank_sort in include/amwg.h."""
-        import torch
         rows, entries, chains = block.shape
         passes = C.c_int32(0)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_rank_sort(self.device, block.data_ptr(), rows, entries, chains, entry, centre,
-                                                      keys.data_ptr(), index.data_ptr(), C.byref(passes)))
+        self._call(block, self.L.amwg_summary_rank_sort, block.data_ptr(), rows, entries, chains, entry, centre, keys.data_ptr(),
+                   index.data_ptr(), C.byref(passes))
         return passes.value
 
     def rank_count(self, q, nq: int, r, nr: int, acc) -> None:
         """acc[:nq] += #(r[:nr] < q[i]) + #(r[:nr] <= q[i]) for sorted key tensors q and r."""
-        import torch
-        torch.cuda.current_stream(acc.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_rank_count(self.device, q.data_ptr(), nq, r.data_ptr(), nr, acc.data_ptr()))
+        self._call(acc, self.L.amwg_summary_rank_count, q.data_ptr(), nq, r.data_ptr(), nr, acc.data_ptr())
 
     def rank_z(self, acc, index, n: int, total: int, z) -> None:
         """z.view(-1)[index[i]] = Phi^-1(((acc[i] + 1) / 2 - 3/8) / (total + 1/4)) for i < n."""
-        import torch
-        torch.cuda.current_stream(acc.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_rank_z(self.device, acc.data_ptr(), index.data_ptr(), n, total, z.data_ptr()))
+        self._call(acc, self.L.amwg_summary_rank_z, acc.data_ptr(), index.data_ptr(), n, total, z.data_ptr())
 
     def finite_range(self, block):
         """-> (float64 tensor [entries, 2]: smallest and largest finite draw, +inf / -inf when there is none; int64 tensor
@@ -211,9 +211,7 @@ class CudaBlockReducer:
         rows, entries, chains = block.shape
         rng = torch.empty((entries, 2), dtype=torch.float64, device=block.device)
         nonfinite = torch.empty((entries, 3), dtype=torch.int64, device=block.device)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_finite_range(self.device, block.data_ptr(), rows, entries, chains, rng.data_ptr(),
-                                                         nonfinite.data_ptr()))
+        self._call(block, self.L.amwg_summary_finite_range, block.data_ptr(), rows, entries, chains, rng.data_ptr(), nonfinite.data_ptr())
         return rng, nonfinite
 
     def histogram(self, block, edges: np.ndarray, bins: int):
@@ -222,9 +220,7 @@ class CudaBlockReducer:
         rows, entries, chains = block.shape
         ed = torch.from_numpy(np.ascontiguousarray(edges, dtype=np.float64)).to(block.device)
         counts = torch.zeros((entries, bins + 3), dtype=torch.int64, device=block.device)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_histogram(self.device, block.data_ptr(), rows, entries, chains, ed.data_ptr(), bins,
-                                                      counts.data_ptr()))
+        self._call(block, self.L.amwg_summary_histogram, block.data_ptr(), rows, entries, chains, ed.data_ptr(), bins, counts.data_ptr())
         return counts
 
     def histogram2d(self, block, pairs: np.ndarray, edges: np.ndarray, bins: int):
@@ -234,33 +230,27 @@ class CudaBlockReducer:
         pr = np.ascontiguousarray(pairs, dtype=np.int32)
         ed = torch.from_numpy(np.ascontiguousarray(edges, dtype=np.float64)).to(block.device)
         counts = torch.zeros((len(pr), bins, bins), dtype=torch.int64, device=block.device)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_histogram2d(self.device, block.data_ptr(), rows, entries, chains, pr.ctypes.data, len(pr),
-                                                        ed.data_ptr(), bins, counts.data_ptr()))
+        self._call(block, self.L.amwg_summary_histogram2d, block.data_ptr(), rows, entries, chains, pr.ctypes.data, len(pr), ed.data_ptr(),
+                   bins, counts.data_ptr())
         return counts
 
     def comoments(self, block, sel) -> np.ndarray:
         """-> flat record [1 + n + 2 n^2] {chains, m[n], B[n][n], W[n][n]} of the n selected entries of this shard; see
         amwg_summary_comoments in include/amwg.h."""
-        import torch
         rows, entries, chains = block.shape
         s = np.ascontiguousarray(sel, dtype=np.int32)
         n = len(s)
         out = np.empty(1 + n + 2 * n * n, dtype=np.float64)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_comoments(self.device, block.data_ptr(), rows, entries, chains, s.ctypes.data, n,
-                                                      out.ctypes.data))
+        self._call(block, self.L.amwg_summary_comoments, block.data_ptr(), rows, entries, chains, s.ctypes.data, n, out.ctypes.data)
         return out
 
     def nested(self, block, first_chain: int, superchain_size: int) -> np.ndarray:
         """-> [entries, 14]: this shard's complete-superchain record and its two cut records; see amwg_summary_nested in
         include/amwg.h."""
-        import torch
         rows, entries, chains = block.shape
         out = np.empty((entries, NESTED_RECORD), dtype=np.float64)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_nested(self.device, block.data_ptr(), rows, entries, chains, first_chain, superchain_size,
-                                                   out.ctypes.data))
+        self._call(block, self.L.amwg_summary_nested, block.data_ptr(), rows, entries, chains, first_chain, superchain_size,
+                   out.ctypes.data)
         return out
 
     def threshold_counts(self, block, thresholds):
@@ -269,9 +259,7 @@ class CudaBlockReducer:
         rows, entries, chains = block.shape
         out = torch.empty((entries, 4), dtype=torch.int64, device=block.device)
         thr = np.ascontiguousarray(thresholds, dtype=np.float64)
-        torch.cuda.current_stream(block.device).synchronize()
-        self._ffi.check(self.L.amwg_summary_threshold_counts(self.device, block.data_ptr(), rows, entries, chains, thr.ctypes.data,
-                                                             out.data_ptr()))
+        self._call(block, self.L.amwg_summary_threshold_counts, block.data_ptr(), rows, entries, chains, thr.ctypes.data, out.data_ptr())
         return out
 
     def loo_reduce(self, ll, llmin, llmax, cut, cap: int):
@@ -283,22 +271,18 @@ class CudaBlockReducer:
         sums = np.empty((P, 3), dtype=np.float64)
         f = lambda a: np.ascontiguousarray(a, dtype=np.float64)
         mn, mx, ct = f(llmin), f(llmax), f(cut)
-        torch.cuda.current_stream(ll.device).synchronize()
-        self._ffi.check(self.L.amwg_loo_reduce(self.device, ll.data_ptr(), rows, P, chains, mn.ctypes.data, mx.ctypes.data, ct.ctypes.data, cap,
-                                               tails.data_ptr(), counts.data_ptr(), sums.ctypes.data))
+        self._call(ll, self.L.amwg_loo_reduce, ll.data_ptr(), rows, P, chains, mn.ctypes.data, mx.ctypes.data, ct.ctypes.data, cap,
+                   tails.data_ptr(), counts.data_ptr(), sums.ctypes.data)
         return sums, tails, counts
-
 
     def loo_fit(self, tails, counts, llmin, cut, skip) -> np.ndarray:
         """tails [shards, P, cap], counts int32 [shards, P] (device) -> [P, 4]; see amwg_loo_fit in include/amwg.h."""
-        import torch
         shards, P, cap = tails.shape
         out = np.empty((P, 4), dtype=np.float64)
         mn, ct = np.ascontiguousarray(llmin, dtype=np.float64), np.ascontiguousarray(cut, dtype=np.float64)
         sk = np.ascontiguousarray(skip, dtype=np.int32)
-        torch.cuda.current_stream(tails.device).synchronize()
-        self._ffi.check(self.L.amwg_loo_fit(self.device, tails.data_ptr(), counts.data_ptr(), shards, P, cap, mn.ctypes.data, ct.ctypes.data,
-                                            sk.ctypes.data, out.ctypes.data))
+        self._call(tails, self.L.amwg_loo_fit, tails.data_ptr(), counts.data_ptr(), shards, P, cap, mn.ctypes.data, ct.ctypes.data,
+                   sk.ctypes.data, out.ctypes.data)
         return out
 
 
@@ -1170,6 +1154,15 @@ def check_loo_size(S: int, r_eff: float) -> int:
     return M
 
 
+def _program_arrays(prog):
+    """(code, consts, fold_prog, fold_dst, n_fold) of a traced program as the pointwise ABI calls take them: contiguous arrays,
+    an empty table padded to one unused element so that its pointer is valid."""
+    consts = np.ascontiguousarray(prog.consts if prog.consts else [0.0], dtype=np.float64)
+    fold_prog = np.ascontiguousarray(prog.fold_prog if prog.fold_prog else [0], dtype=np.int32)
+    fold_dst = np.ascontiguousarray(prog.fold_dst if prog.fold_dst else [0], dtype=np.int32)
+    return np.ascontiguousarray(prog.code, dtype=np.int32), consts, fold_prog, fold_dst, len(prog.fold_prog)
+
+
 class CudaPointwise:
     """The pointwise log-likelihood chunks of one sample block: amwg_loo_pointwise over the handle's data columns."""
 
@@ -1177,11 +1170,7 @@ class CudaPointwise:
         from . import _ffi
         self.L, self._ffi = _ffi.lib(), _ffi
         self.h, self.block, self.device = handle, block, device
-        self.code = np.ascontiguousarray(prog.code, dtype=np.int32)
-        self.consts = np.ascontiguousarray(prog.consts if prog.consts else [0.0], dtype=np.float64)
-        self.fold_prog = np.ascontiguousarray(prog.fold_prog if prog.fold_prog else [0], dtype=np.int32)
-        self.fold_dst = np.ascontiguousarray(prog.fold_dst if prog.fold_dst else [0], dtype=np.int32)
-        self.n_fold = len(prog.fold_prog)
+        self.code, self.consts, self.fold_prog, self.fold_dst, self.n_fold = _program_arrays(prog)
         self.body = prog.logpost_prog
 
     def chunk(self, p0: int, P: int):
@@ -1389,11 +1378,7 @@ class CudaPpc:
         from . import _ffi
         self.L, self._ffi = _ffi.lib(), _ffi
         self.h, self.block, self.family, self.points = handle, block, family, points
-        self.code = np.ascontiguousarray(prog.code, dtype=np.int32)
-        self.consts = np.ascontiguousarray(prog.consts if prog.consts else [0.0], dtype=np.float64)
-        self.fold_prog = np.ascontiguousarray(prog.fold_prog if prog.fold_prog else [0], dtype=np.int32)
-        self.fold_dst = np.ascontiguousarray(prog.fold_dst if prog.fold_dst else [0], dtype=np.int32)
-        self.n_fold = len(prog.fold_prog)
+        self.code, self.consts, self.fold_prog, self.fold_dst, self.n_fold = _program_arrays(prog)
         self.args = np.ascontiguousarray(offsets, dtype=np.int32)
         rows, _, chains = block.shape
         self.T = torch.empty((rows, 4, chains), dtype=torch.float64, device=block.device)

@@ -303,6 +303,9 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  * The reference returns raw draws only (mcmc.js:1029; README.md:44-52 leaves the summary to the caller). With millions of
  * chains the summary is formed where the draws are. Both calls read a DEVICE-resident sample block in amwg_sample_device's
  * layout, x[row][entry][chain]; neither needs a sampler handle (they are reductions over the block).
+ * The summary pool: every amwg_summary_*, amwg_loo_* and amwg_ppc_pointwise call takes its device scratch from one pool per
+ * device, grown on demand, never shrunk, and held (locked) by the call until it returns. A device index outside 0..63 is refused
+ * with "<call>: device index out of range".
  *
  * amwg_summary_moments: host_stats[entry][4] = { chains, mean of the per-chain means, M2 of the per-chain means
  *   (sum_c (m_c - mean)^2), sum over chains of the within-chain M2 (sum_r (x_rc - m_c)^2) }, merged in a fixed order
@@ -364,7 +367,7 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   divided by rows; m sums the chain means in a fixed order. B and W are Gram matrices of the centred values, formed on the fp64
  *   tensor core (mma.sync m8n8k4) by a grid whose size depends on chains only and summed in a fixed order: two calls give the
  *   same bits. A NaN or +-inf draw of an entry makes that entry's rows and columns of B and W NaN. Records of shards merge like
- *   amwg_summary_moments' (Chan, in matrix form). Device scratch, from a per-device pool grown on demand: with T = nb (nb + 1) / 2
+ *   amwg_summary_moments' (Chan, in matrix form). Device scratch (the summary pool): with T = nb (nb + 1) / 2
  *   tiles, nb = ceil(n_sel / 8), R = 1 when T >= 16 else floor(16 / T) warps per tile and G = min(ceil(chains / 32), 264) CTAs,
  *   8 (n_sel chains + n_sel + 64 T R G + 128 T) bytes, each of the four parts rounded up to 256 bytes. Errors (nothing is touched): an empty block, n_sel outside 1..128, null
  *   pointers, a selected entry outside [0, entries), rows * chains >= 2^53.
@@ -378,7 +381,7 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   rows = 1), Chan-merged in a fixed order; then two cut records { superchain id, chains, mean of the chain means, M2 of the chain
  *   means, sum of the within-chain M2 } for the first and the last superchain when the range cuts them (id -1 and zeros when not).
  *   The grid depends on chains and the number of superchains touched only: two calls give the same bits. Records of shards merge
- *   like amwg_summary_moments' (summary.merge_nested_records). Device scratch, from a per-device pool grown on demand, with S the
+ *   like amwg_summary_moments' (summary.merge_nested_records). Device scratch (the summary pool), with S the
  *   superchains touched and G = min(ceil(S / 256), 1184): 16 entries chains + 32 entries G + 32 entries + 64 entries bytes, each
  *   part rounded up to 256 bytes. Errors (nothing is touched): an empty block, null pointers, superchain_size < 1,
  *   first_chain < 0, first_chain + chains > 2^53. */
@@ -424,7 +427,7 @@ AMWG_API int amwg_summary_nested(int device, const double* dev_samples, int64_t 
  *   replaced by the smoothed weights when k is finite, the tail draws over all shards }; a tail of <= 4 draws, or one where no
  *   candidate of the fit has a finite profile value, gives k = +inf and raw weights; host_skip[point] != 0 gives NaN. Deterministic. Errors: tail_cap not a power of two in 8..2^20, shards or points
  *   < 1, null pointers.
- * Device scratch of the three calls, from one per-device pool grown on demand: the program (pointwise), 3 x 8 points + 24 points
+ * Device scratch of the three calls (the summary pool): the program (pointwise), 3 x 8 points + 24 points
  *   G (G = min(ceil(chains / 256), 1184)) bytes (reduce), 3 x 8 points + 16 points tail_cap + 32 points bytes (fit). */
 AMWG_API int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
                                 int32_t body_prog, const int32_t* host_fold_prog, const int32_t* host_fold_dst, int32_t n_fold,
@@ -450,7 +453,7 @@ AMWG_API int amwg_loo_fit(int device, const double* dev_tails, const int32_t* de
  * amwg_summary_threshold_counts: dev_counts[entry][4] (int64, overwritten) = the draws of each entry of a sample block
  *   [rows][entries][chains] that are < host_thresholds[entry], ==, >, and NaN; exact and independent of order. Errors: an empty
  *   block, entries > 65535, null pointers.
- * Device scratch, from the pool of the LOO calls: the programs (pointwise), 8 entries bytes (counts). */
+ * Device scratch (the summary pool): the programs (pointwise), 8 entries bytes (counts). */
 AMWG_API int amwg_ppc_pointwise(amwg_sampler* s, const int32_t* host_code, int32_t n_code, const double* host_consts, int32_t n_consts,
                                 int32_t family, const int32_t* host_arg_progs, int32_t n_args, const int32_t* host_fold_prog,
                                 const int32_t* host_fold_dst, int32_t n_fold, const double* dev_samples, int64_t rows, int32_t entries,

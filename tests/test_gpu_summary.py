@@ -104,3 +104,33 @@ def test_c_abi_reductions_on_an_adversarial_block(gpu_pkg):
     assert L.amwg_summary_digit_hist(0, block.data_ptr(), rows, entries, chains, 0, block.data_ptr(), 33, block.data_ptr()) != 0
     assert b"n_prefix" in L.amwg_last_error()
     assert L.amwg_summary_moments(0, block.data_ptr(), 0, entries, chains, got.ctypes.data) != 0
+
+
+@pytest.mark.parametrize("device", [64, -1])
+def test_every_reduction_refuses_a_device_index_out_of_range(gpu_pkg, device):
+    """each device-taking summary entry point, with arguments that are otherwise valid, names itself and touches nothing"""
+    import torch
+    L = gpu_pkg._ffi.lib()
+    blk = torch.zeros((4, 5, 7), dtype=torch.float64, device="cuda:0")
+    p = blk.data_ptr()
+    host = np.zeros(64)
+    h = host.ctypes.data
+    pairs, sel, skip = np.array([[0, 1]], dtype=np.int32), np.array([0, 1], dtype=np.int32), np.zeros(5, dtype=np.int32)
+    calls = {"amwg_summary_moments": (p, 4, 5, 7, h),
+             "amwg_summary_digit_hist": (p, 4, 5, 7, 0, p, 1, p),
+             "amwg_summary_autocov": (p, 4, 5, 7, None, 0, 1, h),
+             "amwg_summary_rank_sort": (p, 4, 5, 7, 0, float("nan"), p, p, None),
+             "amwg_summary_rank_count": (p, 5, p, 5, p),
+             "amwg_summary_rank_z": (p, p, 5, 5, p),
+             "amwg_summary_finite_range": (p, 4, 5, 7, p, p),
+             "amwg_summary_histogram": (p, 4, 5, 7, p, 8, p),
+             "amwg_summary_histogram2d": (p, 4, 5, 7, pairs.ctypes.data, 1, p, 8, p),
+             "amwg_summary_comoments": (p, 4, 5, 7, sel.ctypes.data, 2, h),
+             "amwg_summary_nested": (p, 4, 5, 7, 0, 1, h),
+             "amwg_summary_threshold_counts": (p, 4, 5, 7, h, p),
+             "amwg_loo_reduce": (p, 4, 5, 7, h, h, h, 8, p, p, h),
+             "amwg_loo_fit": (p, p, 1, 5, 8, h, h, skip.ctypes.data, h)}
+    for name, args in calls.items():
+        assert getattr(L, name)(device, *args) != 0, name
+        assert L.amwg_last_error() == name.encode() + b": device index out of range"
+    assert np.all(host == 0) and not blk.any()
