@@ -4,7 +4,8 @@
 // Stream. y_rep of point i at kept row r (of this call) of global chain g takes the uniforms #(2^62 + (r N + i) 2^16 + k), k = 0, 1, ...,
 // of chain g's Philox stream (DESIGN.md §2). The region lies below the dispersal region (>= 2^63) and far above any position
 // sampling reaches; it is keyed by the global chain, so the draws do not depend on how the chains are sharded. A draw that would
-// need k >= 2^16 gives NaN (no sampler below comes near that). Repeated calls reuse these uniforms for new posterior draws.
+// need k >= 2^16 gives NaN (across the domains below no draw was seen to take 2^12). Repeated calls reuse these uniforms for new
+// posterior draws.
 //
 // Arithmetic. Only + - * /, sqrt, floor, comparisons, js_log, js_exp and js_rnorm (mcmc.js's Leva rnorm), each one IEEE-754
 // operation (the library is built with --fmad=false, the host shim with -ffp-contract=off), so the host-compiled header and a
@@ -18,21 +19,29 @@
 //   exp(rate)                                    rate > 0        E / rate
 //   weibull(shape, scale)                        both > 0        scale js_exp(js_log(E) / shape)
 //   pareto(scale, shape)                         both > 0        scale js_exp(E / shape)
-//   unif(min, max)                               min < max       min + (max - min) U
+//   unif(min, max)                               min < max       min + (max - min) U; in halves when max - min overflows
 //   gamma(shape, rate)                           both > 0        G(shape) / rate: Marsaglia & Tsang (2000) without the squeeze (Z,
-//                                                                then U); shape < 1: G(shape + 1) js_exp(js_log(U) / shape)
-//   invgamma(shape, scale)                       both > 0        scale / G(shape)
-//   beta(a, b)                                   both > 0        X / (X + Y), X = G(a) drawn first, Y = G(b)
-//   t(location, scale, df)                       scale, df > 0   location + scale Z / sqrt(2 G(df / 2) / df), Z first
+//                                                                then U); w < -708: js_exp(log G - js_log(rate))
+//   invgamma(shape, scale)                       both > 0        scale / G(shape); w < -708: js_exp(js_log(scale) - log G)
+//   beta(a, b)                                   both > 0        X / (X + Y), X = G(a) drawn first, Y = G(b); when a w < -708 or
+//                                                                Y / X is beyond e^+-30: from e = js_exp(-|log Y - log X|),
+//                                                                1 - e / (1 + e) or e / (1 + e)
+//   t(location, scale, df)                       scale, df > 0   location + scale Z / sqrt(2 G(df / 2) / df), Z first; w < -708:
+//                                                                the magnitude js_exp of its logarithm
 //   bern(prob)                                   0 <= prob <= 1  U < prob ? 1 : 0
 //   pois(lambda)                                 lambda >= 0     lambda < 10: multiplication against js_exp(-lambda); else PTRS
-//                                                                (Hoermann 1993)
+//                                                                (Hoermann 1993), log p(k) relative to lambda for k >= 128
 //   binom(size, prob)                            integer size >= 0, 0 <= prob <= 1: on q = min(prob, 1 - prob), inversion by
-//                                                                sequential search when size q < 10, else BTRS (Hoermann 1993);
-//                                                                size - x when prob > 1/2
+//                                                                sequential search from (1 - q)^size = js_exp(size log1p(-q)) when
+//                                                                size q < 10, else BTRS (Hoermann 1993) with log p(k) / p(mode)
+//                                                                from differences of log factorials; size - x when prob > 1/2
 //   nbinom(size, prob)                           size > 0, 0 < prob <= 1: pois(G(size) / (prob / (1 - prob))), the failures before
 //                                                                the size-th success as ld.nbinom counts them
-// Z: js_rnorm_ratio (one standard normal); U: one uniform; G(a): a Gamma(a, 1) draw as above.
+// Z: js_rnorm_ratio (one standard normal); U: one uniform; G(a): a Gamma(a, 1) draw as above, for shape < 1 kept as g e^w with
+// g = G(a + 1), w = js_log(U) / a (w = 0 for shape >= 1) and log G = js_log(g) + w, since G itself underflows with probability
+// about e^(-745 a). While w >= -708 the callers form g js_exp(w), as the plain formulas do.
+// What each algorithm gets right is the law of the fp64-rounded variate: 0, +-inf and beta's 1.0 come with the probability that the
+// exact variate rounds there (tests/test_ppc_sampler_domain_host.py).
 #pragma once
 
 #include "amwg_math.cuh"
@@ -108,10 +117,31 @@ __device__ const double kLogFactorial[128] = {
     477.04466549258564, 481.87297922988796, 486.7092611368394, 491.553448223298,
 };
 
+// log k! - ((k + 1/2) log k - k + log sqrt(2 pi)): the tail of Stirling's series, three terms
+__device__ inline double stirling_tail(double k) {
+  const double r = 1.0 / k, r2 = r * r;
+  return r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0)));
+}
+
 __device__ inline double log_factorial(double k) {
   if (k < 128.0) return kLogFactorial[(int)k];
-  const double r = 1.0 / k, r2 = r * r;
-  return (k + 0.5) * js_log(k) - k + 0.91893853320467274178 + r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0)));
+  return (k + 0.5) * js_log(k) - k + 0.91893853320467274178 + stirling_tail(k);
+}
+
+// log(1 + x), x > -1, to a few ulp: Goldberg (1991), "What every computer scientist should know about floating-point arithmetic",
+// Theorem 4. js_log(1 + x) alone loses the bits of x below the ulp of 1.
+__device__ inline double log1p_g(double x) {
+  const double u = 1.0 + x;
+  return u == 1.0 ? x : js_log(u) * x / (u - 1.0);
+}
+
+// log (i + e)! - log i! for integers i, i + e >= 0, e given exactly. When i and j = i + e are both >= 128 it is formed relative to
+// i, e log i + (j + 1/2) log1p(e / i) - e plus the difference of the Stirling tails, so its error is a few ulp of e log i, not of
+// log i! (3.5e16 at i = 1e15). Above 2^53 i may be the rounded value of an integer: that moves the result by about e / i.
+__device__ inline double log_factorial_diff(double i, double e) {
+  const double j = i + e;
+  if (j < 128.0 || i < 128.0) return log_factorial(j) - log_factorial(i);
+  return e * js_log(i) + (j + 0.5) * log1p_g(e / i) - e + (stirling_tail(j) - stirling_tail(i));
 }
 
 template <class S> __device__ inline double expo(S& s) { return -js_log(1.0 - s.u()); }
@@ -129,11 +159,19 @@ template <class S> __device__ double gamma_mt(S& s, double a) {
   return CUDART_NAN;
 }
 
-// G(a): Gamma(a, 1), a > 0
-template <class S> __device__ double gamma1(S& s, double a) {
-  if (a >= 1.0) return gamma_mt(s, a);
+// G(a) = g e^w, a Gamma(a, 1) draw: for a >= 1, g = G(a) and w = 0; for a < 1, g = G(a + 1) and w = log(U) / a. The two are
+// kept apart because G(a) itself lies below the smallest subnormal with probability about e^(-745 a) (one half at a = 1e-3).
+// While w >= kExpNormal, e^w is a normal number and the callers form g e^w directly; below it they work from the logarithm
+// log g + w, whose rounding (a few ulp of |w| > 708) they can afford only there.
+struct ScaledGamma {
+  double g, w;
+};
+constexpr double kExpNormal = -708.0;
+
+template <class S> __device__ ScaledGamma gamma_scaled(S& s, double a) {
+  if (a >= 1.0) return {gamma_mt(s, a), 0.0};
   const double g = gamma_mt(s, a + 1.0);
-  return g * js_exp(js_log(s.u()) / a);
+  return {g, js_log(s.u()) / a};
 }
 
 template <class S> __device__ double pois(S& s, double lam) {
@@ -152,7 +190,12 @@ template <class S> __device__ double pois(S& s, double lam) {
     if (k < 0.0) continue;
     if (us >= 0.07 && V <= vr) return k;
     if (us < 0.013 && V > us) continue;
-    if (js_log(V) + lia - js_log(a / (us * us) + b) <= -lam + k * loglam - log_factorial(k)) return k;
+    // log p(k) = k log lam - lam - log k!; for k >= 128 with Stirling's series relative to lam (d = k - lam), so that no term of
+    // size lam log lam is subtracted: d - k log1p(d / lam) - log(k) / 2 - log sqrt(2 pi) - stirling_tail(k)
+    const double d = k - lam;
+    const double lp = k < 128.0 ? -lam + k * loglam - log_factorial(k)
+                                : d - k * log1p_g(d / lam) - 0.5 * js_log(k) - 0.91893853320467274178 - stirling_tail(k);
+    if (js_log(V) + lia - js_log(a / (us * us) + b) <= lp) return k;
   }
   return CUDART_NAN;
 }
@@ -160,7 +203,7 @@ template <class S> __device__ double pois(S& s, double lam) {
 // binomial on q <= 1/2
 template <class S> __device__ double binom_low(S& s, double n, double q) {
   if (n * q < 10.0) {                                        // inversion by sequential search from 0
-    const double qn = js_exp(n * js_log(1.0 - q)), r = q / (1.0 - q), g = r * (n + 1.0);
+    const double qn = js_exp(n * log1p_g(-q)), r = q / (1.0 - q), g = r * (n + 1.0);   // (1 - q)^n without rounding 1 - q
     while (!s.spent()) {
       double U = s.u(), f = qn, k = 0.0;
       for (;;) {
@@ -175,14 +218,16 @@ template <class S> __device__ double binom_low(S& s, double n, double q) {
   }
   // BTRS, Hoermann (1993), "The generation of binomial random variates"
   const double spq = sqrt(n * q * (1.0 - q)), b = 1.15 + 2.53 * spq, a = -0.0873 + 0.0248 * b + 0.01 * q, c = n * q + 0.5,
-               vr = 0.92 - 4.2 / b, alpha = (2.83 + 5.1 / b) * spq, lpq = js_log(q / (1.0 - q)), m = floor((n + 1.0) * q),
-               h = log_factorial(m) + log_factorial(n - m);
+               vr = 0.92 - 4.2 / b, alpha = (2.83 + 5.1 / b) * spq, lpq = js_log(q / (1.0 - q)), m = floor((n + 1.0) * q);
   while (!s.spent()) {
     const double U = s.u() - 0.5, V = s.u(), us = 0.5 - fabs(U);
     const double k = floor((2.0 * a / us + b) * U + c);
     if (k < 0.0 || k > n) continue;
     if (us >= 0.07 && V <= vr) return k;
-    if (js_log(V * alpha / (a / (us * us) + b)) <= h - log_factorial(k) - log_factorial(n - k) + (k - m) * lpq) return k;
+    // log p(k) / p(m) = [log (n - m)! - log (n - k)!] - [log k! - log m!] + (k - m) lpq, each bracket by log_factorial_diff with
+    // the exact step k - m, so that no term of size n log n is subtracted and n - k need not be exact (it is not above 2^53)
+    const double e = k - m;
+    if (js_log(V * alpha / (a / (us * us) + b)) <= log_factorial_diff(n - k, e) - log_factorial_diff(m, e) + e * lpq) return k;
   }
   return CUDART_NAN;
 }
@@ -235,26 +280,52 @@ template <class S> __device__ double draw(int fam, const double* a, S& s) {
       break;
     case kUnif:
       if (!(a0 < a1)) return CUDART_NAN;
-      x = a0 + (a1 - a0) * s.u();
+      // when max - min overflows, the same in halves (exact: both ends are then far above the subnormals)
+      x = finite(a1 - a0) ? a0 + (a1 - a0) * s.u() : 2.0 * (0.5 * a0 + (0.5 * a1 - 0.5 * a0) * s.u());
       break;
-    case kGamma:
+    case kGamma: {
       if (!(a0 > 0.0 && a1 > 0.0)) return CUDART_NAN;
-      x = gamma1(s, a0) / a1;
+      const ScaledGamma G = gamma_scaled(s, a0);
+      x = G.w >= kExpNormal ? G.g * js_exp(G.w) / a1 : js_exp(js_log(G.g) + G.w - js_log(a1));
       break;
-    case kInvgamma:
+    }
+    case kInvgamma: {
       if (!(a0 > 0.0 && a1 > 0.0)) return CUDART_NAN;
-      x = a1 / gamma1(s, a0);
+      const ScaledGamma G = gamma_scaled(s, a0);
+      x = G.w >= kExpNormal ? a1 / (G.g * js_exp(G.w)) : js_exp(js_log(a1) - (js_log(G.g) + G.w));
       break;
+    }
     case kBeta: {
       if (!(a0 > 0.0 && a1 > 0.0)) return CUDART_NAN;
-      const double X = gamma1(s, a0), Y = gamma1(s, a1);
-      x = X / (X + Y);
+      const ScaledGamma X = gamma_scaled(s, a0), Y = gamma_scaled(s, a1);
+      const double dl = (js_log(Y.g) + Y.w) - (js_log(X.g) + X.w);
+      if (X.w >= kExpNormal && Y.w >= kExpNormal && dl >= -30.0 && dl <= 30.0) {
+        // neither factor underflows and Y / X lies within e^+-30: the ratio is far from 0 and 1, formed directly
+        const double xv = X.g * js_exp(X.w), yv = Y.g * js_exp(Y.w);
+        x = xv / (xv + yv);
+      } else if (dl <= 0.0) {
+        // from the logs, e = min(X, Y) / max(X, Y): X / (X + Y) = 1 - e / (1 + e) or e / (1 + e). The result is 1.0 when
+        // Y / (X + Y) <= 2^-54 and 0 when X / (X + Y) underflows, as rounding the exact ratio would give.
+        const double e = js_exp(dl);
+        x = 1.0 - e / (1.0 + e);
+      } else {
+        const double e = js_exp(-dl);
+        x = e / (1.0 + e);
+      }
       break;
     }
     case kT: {
       if (!(a1 > 0.0 && a2 > 0.0)) return CUDART_NAN;
-      const double z = s.z(), g = gamma1(s, a2 / 2.0);
-      x = a0 + a1 * z / sqrt(2.0 * g / a2);
+      const double z = s.z();
+      const ScaledGamma G = gamma_scaled(s, a2 / 2.0);
+      if (G.w >= kExpNormal) {
+        x = a0 + a1 * z / sqrt(2.0 * (G.g * js_exp(G.w)) / a2);
+        break;
+      }
+      // G(df / 2) may underflow: scale |z| / sqrt(2 G / df) from the logs; past DBL_MAX it is +-inf
+      const double lt = js_log(a1) + js_log(fabs(z)) - 0.5 * (js_log(G.g) + G.w + 0.6931471805599453 - js_log(a2));
+      const double v = js_exp(lt);
+      x = a0 + (z < 0.0 ? -v : v);
       break;
     }
     case kBern:
@@ -274,7 +345,9 @@ template <class S> __device__ double draw(int fam, const double* a, S& s) {
     }
     case kNbinom: {
       if (!(a0 > 0.0 && a1 > 0.0 && a1 <= 1.0)) return CUDART_NAN;
-      const double lam = gamma1(s, a0) / (a1 / (1.0 - a1));
+      const ScaledGamma G = gamma_scaled(s, a0);
+      const double rate = a1 / (1.0 - a1);
+      const double lam = G.w >= kExpNormal ? G.g * js_exp(G.w) / rate : js_exp(js_log(G.g) + G.w - js_log(rate));
       x = pois(s, lam);
       break;
     }

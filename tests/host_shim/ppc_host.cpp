@@ -39,13 +39,18 @@ double hs_ppc_draw(int fam, const double* a, uint64_t seed, uint64_t chain, uint
   return x;
 }
 
-// n draws at consecutive stream positions (for the distribution tests: draw j at row 0, point j of n)
-void hs_ppc_draws(int fam, const double* a, uint64_t seed, uint64_t chain, uint64_t n, double* out) {
+// n draws at consecutive stream positions (for the distribution tests: draw j at row 0, point j of n); returns the largest number
+// of uniforms any of them took
+uint64_t hs_ppc_draws(int fam, const double* a, uint64_t seed, uint64_t chain, uint64_t n, double* out) {
+  uint64_t most = 0;
   for (uint64_t j = 0; j < n; ++j) {
     ppc::PhiloxSource s;
-    s.init(seed, chain, ppc::stream_position(0, n, j));
+    const uint64_t pos = ppc::stream_position(0, n, j);
+    s.init(seed, chain, pos);
     out[j] = ppc::draw(fam, a, s);
+    if (s.g.n - pos > most) most = s.g.n - pos;
   }
+  return most;
 }
 
 double hs_ppc_draw_tape(int fam, const double* a, const double* tape, uint64_t len, uint64_t* used) {
@@ -56,5 +61,7 @@ double hs_ppc_draw_tape(int fam, const double* a, const double* tape, uint64_t l
 }
 
 double hs_ppc_log_factorial(double k) { return ppc::log_factorial(k); }
+double hs_ppc_log1p(double x) { return ppc::log1p_g(x); }
+double hs_ppc_log_factorial_diff(double i, double e) { return ppc::log_factorial_diff(i, e); }
 
 }

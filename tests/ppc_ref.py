@@ -70,12 +70,31 @@ def rnorm(s):
             return v / u
 
 
+def stirling_tail(k):
+    """log k! - ((k + 1/2) log k - k + log sqrt(2 pi)), three terms of Stirling's series"""
+    r = 1.0 / k
+    r2 = r * r
+    return r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0)))
+
+
 def log_factorial(O, k):
     if k < 128.0:
         return LOG_FACTORIAL[int(k)]
-    r = 1.0 / k
-    r2 = r * r
-    return (k + 0.5) * O.orc_log(k) - k + 0.91893853320467274178 + r * (1.0 / 12.0 - r2 * (1.0 / 360.0 - r2 * (1.0 / 1260.0)))
+    return (k + 0.5) * O.orc_log(k) - k + 0.91893853320467274178 + stirling_tail(k)
+
+
+def log1p(O, x):
+    """log(1 + x) from one logarithm and one division: Goldberg (1991), Theorem 4"""
+    u = 1.0 + x
+    return x if u == 1.0 else O.orc_log(u) * x / (u - 1.0)
+
+
+def log_factorial_diff(O, i, e):
+    """log (i + e)! - log i! with the step e exact; for i, i + e >= 128 relative to i, so that log i! itself is never formed"""
+    j = i + e
+    if j < 128.0 or i < 128.0:
+        return log_factorial(O, j) - log_factorial(O, i)
+    return e * O.orc_log(i) + (j + 0.5) * log1p(O, e / i) - e + (stirling_tail(j) - stirling_tail(i))
 
 
 def expo(s):
@@ -101,11 +120,16 @@ def gamma_mt(s, a):
     return NAN
 
 
-def gamma1(s, a):
+EXP_NORMAL = -708.0
+
+
+def gamma_scaled(s, a):
+    """a Gamma(a, 1) draw as (g, w), G = g e^w: (G, 0) for a >= 1, else (G(a + 1), log(U) / a). The callers form g e^w while
+    w >= EXP_NORMAL, where e^w is normal, and work from log g + w below it, where G may underflow."""
     if a >= 1.0:
-        return gamma_mt(s, a)
+        return gamma_mt(s, a), 0.0
     g = gamma_mt(s, a + 1.0)
-    return g * s.O.orc_exp(s.O.orc_log(s.u()) / a)
+    return g, s.O.orc_log(s.u()) / a
 
 
 def pois(s, lam):
@@ -136,7 +160,12 @@ def pois(s, lam):
             return k
         if us < 0.013 and V > us:
             continue
-        if O.orc_log(V) + lia - O.orc_log(a / (us * us) + b) <= -lam + k * loglam - log_factorial(O, k):
+        d = k - lam
+        if k < 128.0:
+            lp = -lam + k * loglam - log_factorial(O, k)
+        else:
+            lp = d - k * log1p(O, d / lam) - 0.5 * O.orc_log(k) - 0.91893853320467274178 - stirling_tail(k)
+        if O.orc_log(V) + lia - O.orc_log(a / (us * us) + b) <= lp:
             return k
     return NAN
 
@@ -144,7 +173,7 @@ def pois(s, lam):
 def binom_low(s, n, q):
     O = s.O
     if n * q < 10.0:
-        qn = O.orc_exp(n * O.orc_log(1.0 - q))
+        qn = O.orc_exp(n * log1p(O, -q))
         r = q / (1.0 - q)
         g = r * (n + 1.0)
         while not s.spent():
@@ -167,7 +196,6 @@ def binom_low(s, n, q):
     alpha = (2.83 + 5.1 / b) * spq
     lpq = O.orc_log(q / (1.0 - q))
     m = float(math.floor((n + 1.0) * q))
-    h = log_factorial(O, m) + log_factorial(O, n - m)
     while not s.spent():
         U = s.u() - 0.5
         V = s.u()
@@ -177,7 +205,8 @@ def binom_low(s, n, q):
             continue
         if us >= 0.07 and V <= vr:
             return k
-        if O.orc_log(V * alpha / (a / (us * us) + b)) <= h - log_factorial(O, k) - log_factorial(O, n - k) + (k - m) * lpq:
+        e = k - m
+        if O.orc_log(V * alpha / (a / (us * us) + b)) <= log_factorial_diff(O, n - k, e) - log_factorial_diff(O, m, e) + e * lpq:
             return k
     return NAN
 
@@ -232,28 +261,49 @@ def draw(family, args, s):
     elif f == "unif":
         if not a0 < a1:
             return NAN
-        x = a0 + (a1 - a0) * s.u()
+        w = a1 - a0
+        x = a0 + w * s.u() if math.isfinite(w) else 2.0 * (0.5 * a0 + (0.5 * a1 - 0.5 * a0) * s.u())
     elif f == "gamma":
         if not (a0 > 0 and a1 > 0):
             return NAN
-        x = gamma1(s, a0) / a1
+        g, w = gamma_scaled(s, a0)
+        x = g * O.orc_exp(w) / a1 if w >= EXP_NORMAL else O.orc_exp(O.orc_log(g) + w - O.orc_log(a1))
     elif f == "invgamma":
         if not (a0 > 0 and a1 > 0):
             return NAN
-        g = gamma1(s, a0)
-        x = a1 / g if g != 0 else math.inf
+        g, w = gamma_scaled(s, a0)
+        if w >= EXP_NORMAL:
+            G = g * O.orc_exp(w)
+            x = a1 / G if G != 0 else math.inf
+        else:
+            x = O.orc_exp(O.orc_log(a1) - (O.orc_log(g) + w))
     elif f == "beta":
         if not (a0 > 0 and a1 > 0):
             return NAN
-        X = gamma1(s, a0)
-        Y = gamma1(s, a1)
-        x = X / (X + Y) if X + Y != 0 else NAN
+        gx, wx = gamma_scaled(s, a0)
+        gy, wy = gamma_scaled(s, a1)
+        dl = (O.orc_log(gy) + wy) - (O.orc_log(gx) + wx)
+        if wx >= EXP_NORMAL and wy >= EXP_NORMAL and -30.0 <= dl <= 30.0:
+            X = gx * O.orc_exp(wx)
+            Y = gy * O.orc_exp(wy)
+            x = X / (X + Y)
+        elif dl <= 0.0:
+            e = O.orc_exp(dl)
+            x = 1.0 - e / (1.0 + e)
+        else:
+            e = O.orc_exp(-dl)
+            x = e / (1.0 + e)
     elif f == "t":
         if not (a1 > 0 and a2 > 0):
             return NAN
         z = rnorm(s)
-        g = gamma1(s, a2 / 2.0)
-        x = a0 + a1 * z / math.sqrt(2.0 * g / a2)
+        g, w = gamma_scaled(s, a2 / 2.0)
+        if w >= EXP_NORMAL:
+            x = a0 + a1 * z / math.sqrt(2.0 * (g * O.orc_exp(w)) / a2)
+        else:
+            lt = O.orc_log(a1) + O.orc_log(abs(z)) - 0.5 * (O.orc_log(g) + w + 0.6931471805599453 - O.orc_log(a2))
+            v = O.orc_exp(lt)
+            x = a0 + (-v if z < 0.0 else v)
     elif f == "bern":
         if not 0.0 <= a0 <= 1.0:
             return NAN
@@ -272,7 +322,8 @@ def draw(family, args, s):
         if not (a0 > 0 and 0.0 < a1 <= 1.0):
             return NAN
         rate = a1 / (1.0 - a1) if a1 < 1.0 else math.inf
-        lam = gamma1(s, a0) / rate
+        g, w = gamma_scaled(s, a0)
+        lam = g * O.orc_exp(w) / rate if w >= EXP_NORMAL else O.orc_exp(O.orc_log(g) + w - O.orc_log(rate))
         x = pois(s, lam)
     else:
         raise ValueError(family)
