@@ -33,6 +33,7 @@
 // Included at the end of amwg_kernels.cu (same translation unit: shares CUDA_TRY / fail()).
 #pragma once
 
+#include "amwg_autocov.cuh"      // the half-chain walk of K_a1
 #include "amwg_comoments.cuh"
 #include "amwg_hist.cuh"
 #include "amwg_nested.cuh"      // Moments and merge
@@ -324,10 +325,7 @@ __global__ void __launch_bounds__(256) amwg_hist2d_kernel(const double* __restri
 
 // ---- split-chain autocovariances (effective sample size, split R-hat) ------------------------------------------------------
 // Every chain of `rows` kept draws is split into a first half (rows [0, h)) and a second half (rows [rows-h, rows)), h = rows/2.
-// Per half-chain m and series y (the draws, or an indicator 1[x <= q] of them), centred by the half-chain's own mean:
-//   record  {1, mean_m, 0, sum_n d_n^2}                 merged like Moments (Chan, fixed order)
-//   lag sum sum_n d_n d_{n+t} = h * acov_m(t)           summed in a fixed order, for t in the lag window
-constexpr int kLagSlots = 16;         // lags per kernel pass: the ring of centred lead values a thread keeps in registers
+// The per-half-chain records and lag sums, and the scaling of the draws series, are autocov_half's (amwg_autocov.cuh).
 
 template <int THREADS>
 __device__ __forceinline__ double cta_sum(double* sh, double mine) {            // fixed tree, like cta_merge
@@ -343,10 +341,8 @@ __device__ __forceinline__ double cta_sum(double* sh, double mine) {            
   return r;
 }
 
-// K_a1: one thread per chain (grid-stride), both halves. Pass 1 reads the half for its means; pass 2 reads it again and keeps
-// the kLagSlots centred values at positions n+lag0 .. n+lag0+15 in a register ring, so every loaded value serves all lags of the
-// window. NS = 1: the draws only; NS = 3: also 1[x <= thr[e][0]] and 1[x <= thr[e][1]], formed from the same loads (the ring holds
-// their bits). Positions at or past h count as 0, so a product exists exactly when both ends lie in the half.
+// K_a1: one thread per chain (grid-stride), both halves, each by autocov_half. NS = 1: the draws only; NS = 3: also the two
+// indicators of thr[e][0] and thr[e][1], and the draws scaled by autocov_scale(thr[e][0], thr[e][1]).
 // pmom[(e*NS + s)][block] (skipped when null), psum[((e*NS + s)*n_total + k_base + k)][block] for k < n_lags.
 template <int NS>
 __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
@@ -356,8 +352,8 @@ __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restr
   const int e = blockIdx.y;
   const long long h = rows / 2;
   const size_t stride = (size_t)entries * C;
-  double q0 = 0.0, q1 = 0.0;
-  if constexpr (NS == 3) { q0 = thr[2 * e]; q1 = thr[2 * e + 1]; }
+  double q0 = 0.0, q1 = 0.0, sc = 1.0;
+  if constexpr (NS == 3) { q0 = thr[2 * e]; q1 = thr[2 * e + 1]; sc = autocov_scale(q0, q1); }
   double acc[NS][kLagSlots];
 #pragma unroll
   for (int s = 0; s < NS; ++s)
@@ -368,90 +364,8 @@ __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restr
   for (int s = 0; s < NS; ++s) mom[s] = Moments{0.0, 0.0, 0.0, 0.0};
 
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
-    for (int half = 0; half < 2; ++half) {
-      const double* p = x + (size_t)e * C + c + (size_t)(half ? rows - h : 0) * stride;
-      const double x0 = p[0];
-      const unsigned long long x0_bits = run_bits(x0);
-      unsigned long long diff = 0;
-      double s0 = 0.0;
-      long long n0 = 0, n1 = 0;
-      long long r = 0;
-      for (; r + 8 <= h; r += 8) {                           // eight loads in flight per thread, the sum stays sequential
-        double v[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          s0 += v[u];
-          diff |= run_bits(v[u]) ^ x0_bits;
-          if constexpr (NS == 3) { n0 += v[u] <= q0; n1 += v[u] <= q1; }
-        }
-      }
-      for (; r < h; ++r) {
-        const double v = p[r * stride];
-        s0 += v;
-        diff |= run_bits(v) ^ x0_bits;
-        if constexpr (NS == 3) { n0 += v <= q0; n1 += v <= q1; }
-      }
-      double m[NS];
-      m[0] = run_mean(s0, h, x0, diff);                      // a constant half-chain is centred on its value (amwg_nested.cuh)
-      if constexpr (NS == 3) { m[1] = (double)n0 / (double)h; m[2] = (double)n1 / (double)h; }
-
-      double ring[kLagSlots];
-      unsigned valid = 0u, b0 = 0u, b1 = 0u;                  // bit k: slot k lies in the half / its draw is <= q0 / <= q1
-#pragma unroll
-      for (int k = 0; k < kLagSlots; ++k) {
-        const long long pp = lag0 + k;
-        ring[k] = 0.0;
-        if (pp < h) {
-          const double v = p[pp * stride];
-          ring[k] = v - m[0];
-          valid |= 1u << k;
-          if constexpr (NS == 3) { b0 |= (unsigned)(v <= q0) << k; b1 |= (unsigned)(v <= q1) << k; }
-        }
-      }
-      double sw[NS];
-#pragma unroll
-      for (int s = 0; s < NS; ++s) sw[s] = 0.0;
-      for (long long j = 0; j < h; j += kLagSlots) {
-#pragma unroll
-        for (int u = 0; u < kLagSlots; ++u) {                 // unrolled: the ring's slot indices are compile-time constants
-          const long long n = j + u;
-          if (n < h) {
-            const double v = p[n * stride];
-            double cur[NS];
-            cur[0] = v - m[0];
-            if constexpr (NS == 3) { cur[1] = v <= q0 ? 1.0 - m[1] : -m[1]; cur[2] = v <= q1 ? 1.0 - m[2] : -m[2]; }
-#pragma unroll
-            for (int s = 0; s < NS; ++s) sw[s] = fma(cur[s], cur[s], sw[s]);
-#pragma unroll
-            for (int k = 0; k < kLagSlots; ++k) {
-              const int slot = (u + k) % kLagSlots;         // holds position n + lag0 + k
-              acc[0][k] = fma(cur[0], ring[slot], acc[0][k]);
-              if constexpr (NS == 3) {
-                const bool in = (valid >> slot) & 1u;
-                const double a0 = in ? (((b0 >> slot) & 1u) ? 1.0 - m[1] : -m[1]) : 0.0;
-                const double a1 = in ? (((b1 >> slot) & 1u) ? 1.0 - m[2] : -m[2]) : 0.0;
-                acc[1][k] = fma(cur[1], a0, acc[1][k]);
-                acc[2][k] = fma(cur[2], a1, acc[2][k]);
-              }
-            }
-            const long long pp = n + lag0 + kLagSlots;        // slot u moves on to position n + lag0 + kLagSlots
-            const unsigned bit = 1u << u;
-            ring[u] = 0.0;
-            valid &= ~bit; b0 &= ~bit; b1 &= ~bit;
-            if (pp < h) {
-              const double w = p[pp * stride];
-              ring[u] = w - m[0];
-              valid |= bit;
-              if constexpr (NS == 3) { if (w <= q0) b0 |= bit; if (w <= q1) b1 |= bit; }
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int s = 0; s < NS; ++s) mom[s] = merge(mom[s], Moments{1.0, m[s], 0.0, sw[s]});
-    }
+    for (int half = 0; half < 2; ++half)
+      autocov_half<NS>(x + (size_t)e * C + c + (size_t)(half ? rows - h : 0) * stride, h, stride, q0, q1, sc, lag0, acc, mom);
   }
   if (pmom) {
 #pragma unroll

@@ -306,7 +306,8 @@ def merge_autocov_records(records: Sequence[np.ndarray]) -> np.ndarray:
 
 class GeyerESS:
     """ESS of one series from its merged split-chain record, one lag window at a time. Geyer's initial positive sequence and
-    then the initial monotone sequence, exactly as written in the docstring of `split_chain_diagnostics`. `need()` is the first
+    then the initial monotone sequence, exactly as written in the docstring of `split_chain_diagnostics`; NaN at once when W is 0
+    or not finite (the caller settles constant series before). `need()` is the first
     lag it has not got yet (None once done); `add(sums)` appends the lag sums of the next window."""
 
     def __init__(self, record: np.ndarray, h: int):
@@ -334,6 +335,9 @@ class GeyerESS:
 
     def _run(self) -> None:
         h, rho, r = self.h, self.rho, self.r
+        if not (0.0 < self.W < np.inf):
+            self.ess = np.nan                                     # no within-chain spread to measure (or its sums overflowed)
+            return
         if self.od is None:
             if len(rho) < 2:
                 return
@@ -375,11 +379,17 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
       ess_tail   min of the ESS of 1[x <= q05] and of 1[x <= q95] (lo, hi: the pooled exact quantiles; ties count as <=)
       mcse_mean  sd / sqrt(ess_mean), sd the pooled sd
       rhat_split sqrt(var+ / W) of the draws (not rank-normalised)
+    The device scales the draws series by a power of two taken from q95/2 - q05/2 (autocov_scale in csrc/amwg_autocov.cuh; 1 when
+    q05 == q95), applied to the centred values and the half-chain means alike. Scaling by a power of two is exact, and every value
+    above is a ratio of these sums, so draws x and x * 2^j give the same bits of ess_mean, ess_tail and rhat_split while the
+    scaled values stay normal: tiny or huge draws (1e-170, 1e160) neither underflow nor overflow their squares. The scale leaves
+    about 2^511 of headroom between that spread and the largest |x - mean|: draws with a narrow centre and far outliers (spread
+    1e-10, outliers near 1e150) overflow once scaled and give NaN where the unscaled squares were finite.
     Edge cases: fewer than 10 rows (h < 5): all NaN. A constant entry (vmin == vmax) has ESS = M h, MCSE 0 and rhat_split NaN
     (its half-chains are centred on their value, so W = 0 and B = 0); half-chains each constant at a value of their own give
-    rhat_split +inf. An indicator
-    that is constant (all 1 when the quantile equals the maximum) has ESS = M h. A non-finite minimum or maximum (an infinite or
-    NaN draw) makes all four values NaN.
+    rhat_split +inf and ESS NaN. An indicator that is constant (all 1 when the quantile equals the maximum) has ESS = M h. Any other
+    series whose W is 0 or not finite (its sums underflowed or overflowed) has ESS NaN, never a finite value, and ess_tail is NaN
+    when either indicator's ESS is. A non-finite minimum or maximum (an infinite or NaN draw) makes all four values NaN.
     Lag windows of at most `max_lags` lags are asked for only while some series' Geyer loop still needs a lag it has not got,
     the way RadixSelect asks for its next pass. Distributed: each window's per-rank records are all-gathered and merged in rank
     order, so every rank returns the same numbers."""
@@ -414,7 +424,7 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
         const = (vmin[e] == vmax[e], thr[e, 0] >= vmax[e] or thr[e, 0] < vmin[e], thr[e, 1] >= vmax[e] or thr[e, 1] < vmin[e])
         ess = [Mh if c else g.ess for g, c in zip(est[e], const)]
         out["ess_mean"][e] = ess[0]
-        out["ess_tail"][e] = min(ess[1], ess[2])
+        out["ess_tail"][e] = np.minimum(ess[1], ess[2])
         with np.errstate(invalid="ignore", divide="ignore"):
             out["mcse_mean"][e] = 0.0 if vmin[e] == vmax[e] else sd[e] / np.sqrt(ess[0])
             out["rhat_split"][e] = np.sqrt(est[e][0].varplus / est[e][0].W)
@@ -453,7 +463,8 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
     Edge cases: fewer than 10 rows: NaN. A NaN draw anywhere in the kept rows (vmin or vmax NaN): both NaN. +-inf draws are
     ranked like any other value, so both stay finite. A constant entry (all ranked draws equal): ess_bulk = M h (M = 2 * chains),
     rhat_rank NaN. A constant folded series (for example draws +-1 with median 0): rhat_rank is the R-hat of z alone. med not
-    finite (+-inf, or NaN when numpy.quantile's rule interpolates towards an infinite draw): rhat_rank NaN.
+    finite (+-inf, or NaN when numpy.quantile's rule interpolates towards an infinite draw): rhat_rank NaN. Half-chains each
+    constant at a value of their own (W = 0 for z): ess_bulk NaN (GeyerESS) and rhat_rank +inf.
     Device work per entry and series (CudaBlockReducer): a radix sort of the shard's keys, rank counts against every shard's
     sorted keys, and z written into a [2h][1][chains] block that amwg_summary_autocov splits into exactly the ranked halves.
     Distributed: the sorted key arrays travel around a ring of torch.distributed send / recv (W - 1 steps, two buffers); the

@@ -324,7 +324,12 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   is centred by its own mean. host_out[entry][series][4 + n_lags] = { M, mean of the half-chain means, M2 of the half-chain
  *   means, sum over half-chains of sum_n d_n^2, then for t = lag0 .. lag0+n_lags-1 the sum over half-chains of
  *   sum_{n<h-t} d_n d_{n+t} (= h * acov(t)) }. The first four merge like amwg_summary_moments' records, the lag sums add;
- *   both are formed in a fixed order (deterministic). Errors: rows < 2, n_lags outside 1..32, lag0 + n_lags > h, null
+ *   both are formed in a fixed order (deterministic). With thresholds, the draws series' centred values d and half-chain means
+ *   are multiplied by 2^k, k = -ilogb(thresholds[entry][1]/2 - thresholds[entry][0]/2) clamped to [-1022, 1023] (k = 0 when that
+ *   spread is 0 or not finite), so its fields 1..3 and lag sums are in units of 2^k (squared for M2, sum_w and the lag sums).
+ *   Powers of two scale exactly: the ESS and split R-hat, ratios of these sums, do not depend on the scale of the draws, and
+ *   tiny or huge draws with a spread of their own size do not underflow or overflow. The scale leaves about 2^511 between the
+ *   spread and the largest |x - mean|: outliers further out (spread 1e-10, outliers near 1e150) overflow once scaled. Errors: rows < 2, n_lags outside 1..32, lag0 + n_lags > h, null
  *   dev_samples / host_out.
  *
  * Ranks over the pooled half-chain draws (rank-normalised R-hat and bulk ESS, Vehtari et al. 2021, §4). One entry per call; the

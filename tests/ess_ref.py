@@ -4,9 +4,21 @@
 - `NumpyAutocovReducer`: a numpy stand-in for amwg_summary_autocov (plus the two reductions of summary_ref.NumpyBlockReducer),
   so the host path runs on CPU tensors.
 Never imported by the product."""
+import math
+
 import numpy as np
 
 from summary_ref import NumpyBlockReducer, run_means
+
+
+def autocov_scale(q05, q95) -> float:
+    """the power of two amwg_summary_autocov scales the draws series by (autocov_scale, csrc/amwg_autocov.cuh): 2^-ilogb(q95/2 -
+    q05/2) clamped to [2^-1022, 2^1023]; 1 when that spread is 0 or not finite"""
+    s = float(q95) * 0.5 - float(q05) * 0.5
+    if not (0.0 < s <= 1.7976931348623157e308):
+        return 1.0
+    k = 1 - math.frexp(s)[1]                                  # -ilogb(s), subnormal s included
+    return math.ldexp(1.0, min(max(k, -1022), 1023))
 
 
 def halves(x):
@@ -94,7 +106,8 @@ def fft_diagnostics(x):
 
 
 def autocov_records(x, thresholds, lag0, n_lags):
-    """numpy restatement of amwg_summary_autocov on x [rows, entries, chains] -> [entries, series, 4 + n_lags]."""
+    """numpy restatement of amwg_summary_autocov on x [rows, entries, chains] -> [entries, series, 4 + n_lags]; with thresholds,
+    the draws series' centred values and means scaled by autocov_scale, as the device does."""
     rows, entries, chains = x.shape
     h = rows // 2
     ns = 1 if thresholds is None else 3
@@ -107,6 +120,10 @@ def autocov_records(x, thresholds, lag0, n_lags):
             y = halves(ys)
             m = run_means(y.T)                                 # a constant half-chain of draws is centred on its value
             d = y - m[:, None]
+            if s == 0 and thresholds is not None:
+                sc = autocov_scale(*thresholds[e])
+                with np.errstate(over="ignore", invalid="ignore"):
+                    m, d = m * sc, d * sc
             mean = run_means(m)                                # equal means: that value, as the Chan merge gives
             out[e, s, :4] = (y.shape[0], mean, ((m - mean) ** 2).sum(), (d * d).sum())
             for k in range(n_lags):

@@ -8,7 +8,7 @@ import sys
 import numpy as np
 import pytest
 
-from ess_ref import (NumpyAutocovReducer, ar1, autocov_records, ess_fft, fft_diagnostics, geyer_tau, halves, rho_fft)
+from ess_ref import (NumpyAutocovReducer, ar1, autocov_records, autocov_scale, ess_fft, fft_diagnostics, geyer_tau, halves, rho_fft)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PROBS = (0.025, 0.25, 0.5, 0.75, 0.975)
@@ -68,7 +68,8 @@ def test_autocorrelations_match_the_fft_restatement(pkg):
             g = GeyerESS(rec[e, s], h)
             want, varplus, W = rho_fft(halves(ys))
             assert np.allclose(g._rho(rec[e, s, 4:]), want, rtol=0, atol=1e-12), (e, s)
-            assert np.isclose(g.varplus, varplus, rtol=1e-12) and np.isclose(g.W, W, rtol=1e-12)
+            sc2 = autocov_scale(*thr[e]) ** 2 if s == 0 else 1.0      # the draws series is recorded scaled by a power of two
+            assert np.isclose(g.varplus, varplus * sc2, rtol=1e-12) and np.isclose(g.W, W * sc2, rtol=1e-12)
 
 
 @pytest.mark.parametrize("rows,chains", [(10, 30), (11, 30), (12, 1), (33, 1), (57, 19), (100, 64)])
