@@ -664,13 +664,10 @@ class AmwgSampler(Sampler):
 
     def sample(self, n_iterations):
         """mcmc.js:1005-1030 -- {name: draws}; rows = ceil(n/thin); row r is the state before sweep r*thin."""
+        from .summary import entry_spans
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
-        entries: List[int] = []
-        spans = {}
-        for name in monitored:
-            e = self._entries(name)
-            spans[name] = (len(entries), len(e))
-            entries.extend(e)
+        entries = [i for name in monitored for i in self._entries(name)]
+        spans = entry_spans(monitored, {name: [len(self._entries(name))] for name in monitored})
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))                 # `i % thin === 0` (mcmc.js:1021): the sign of thin does not matter ...
         if thin == 0:                                           # ... and i % 0 is NaN: nothing is ever recorded, the chains still step
@@ -794,17 +791,13 @@ class AmwgSampler(Sampler):
         (summary.resolve_ppc, summary.check_ppc_call, tracer.LogLik.observed_call)."""
         import torch
         from .summary import (CudaBlockReducer, CudaPointwise, CudaPpc, check_diagnostics, check_loo_size, check_ppc_call, comoments_scratch_bytes,
-                              covariance_block, histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block, nested_scratch_bytes,
-                              ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance, resolve_histogram, resolve_loo, resolve_nested,
-                              resolve_ppc, summarise_block)
+                              covariance_block, entry_spans, histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block,
+                              nested_scratch_bytes, ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance, resolve_histogram, resolve_loo,
+                              resolve_nested, resolve_ppc, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
-        entries: List[int] = []
-        spans = {}
-        for name in monitored:
-            e = self._entries(name)
-            spans[name] = (len(entries), len(e))
-            entries.extend(e)
+        entries = [i for name in monitored for i in self._entries(name)]
+        spans = entry_spans(monitored, {name: [len(self._entries(name))] for name in monitored})
         named = [name for name in monitored if spans[name][1] > 0]
         dims = {name: list(self.params[name]["dim"]) if name in self.params else [1] for name in named}
         plan = resolve_histogram(histogram, named, dims)
@@ -861,7 +854,8 @@ class AmwgSampler(Sampler):
         if superchain is not None:
             need += nested_scratch_bytes(len(entries), self.local_chains, self.first_chain, superchain)
         free, _total = torch.cuda.mem_get_info(dev)
-        if need + 2 * len(entries) * self.local_chains * 8 > 0.9 * free:
+        base = need + 2 * len(entries) * self.local_chains * 8      # and the base summary's scratch: two doubles per entry and chain
+        if base > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
         if diagnostics == "rank" and rows >= 10:
             # rank_diagnostics, per entry: keys 2 x 8 B, indices 2 x 4 B, rank sums 8 B, a ring buffer 8 B and two z-blocks 2 x 8 B per
@@ -869,11 +863,11 @@ class AmwgSampler(Sampler):
             # tables (2 x 256 x 4 B per 2048 keys)
             ranked = 2 * (rows // 2) * (self.local_chains + (1 if self.distributed else 0))
             scratch = 56 * ranked + 2 * 256 * 4 * (-(-ranked // 2048))
-            if need + 2 * len(entries) * self.local_chains * 8 + scratch > 0.9 * free:
+            if base + scratch > 0.9 * free:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
                               "device memory; raise thin() or lower n" % (need / 1e9, scratch / 1e9))
         def chunk_size(per_point, points, what):
-            chunk_points = int((0.9 * free - need - 2 * len(entries) * self.local_chains * 8) // per_point)
+            chunk_points = int((0.9 * free - base) // per_point)
             if chunk_points < 1:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and one point of the %s (%.1f GB) do not fit "
                               "in device memory; raise thin() or lower n" % (need / 1e9, what, per_point / 1e9))
@@ -895,22 +889,22 @@ class AmwgSampler(Sampler):
         rc = L.amwg_sample_device(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(sampled), block.data_ptr())
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
+        reducer = CudaBlockReducer(self.device)
         loo_out = None
         if loo_plan is not None:
-            loo_out = loo_block(CudaBlockReducer(self.device), CudaPointwise(self._handle, loo_prog, block, self.device), rows, self.n_chains,
-                                loo_plan.points, loo_plan.r_eff, chunk_points, self.distributed)
+            loo_out = loo_block(reducer, CudaPointwise(self._handle, loo_prog, block, self.device), rows, self.n_chains, loo_plan.points,
+                                loo_plan.r_eff, chunk_points, self.distributed)
         ppc_out = None
         if ppc_plan is not None:
-            ppc_out = ppc_block(CudaBlockReducer(self.device), CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points),
-                                rows, self.n_chains, ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed)
+            ppc_out = ppc_block(reducer, CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points), rows, self.n_chains,
+                                ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed)
         if len(sampled) > len(entries):
             block = block[:, :len(entries)].contiguous()
-        res = summarise_block(CudaBlockReducer(self.device), block, rows, self.n_chains, probs, self.distributed, diagnostics)
+        res = summarise_block(reducer, block, rows, self.n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
-        hist = None if plan is None else histogram_block(CudaBlockReducer(self.device), block, rows, plan, self.distributed)
-        cov = None if cov_plan is None else covariance_block(CudaBlockReducer(self.device), block, rows, cov_plan, self.distributed)
-        rn = None if superchain is None else nested_block(CudaBlockReducer(self.device), block, rows, self.first_chain, superchain,
-                                                          self.distributed)
+        hist = None if plan is None else histogram_block(reducer, block, rows, plan, self.distributed)
+        cov = None if cov_plan is None else covariance_block(reducer, block, rows, cov_plan, self.distributed)
+        rn = None if superchain is None else nested_block(reducer, block, rows, self.first_chain, superchain, self.distributed)
         del block
         out = {}
         for name in monitored:

@@ -3,9 +3,9 @@ statistic per monitored entry, over all chains and kept rows of one `sample()` b
 
 The reference returns raw draws (mcmc.js:1029) and its README summarises them on the caller's side (README.md:44-52); at
 2^20..2^22 chains the raw block is GBs per call, so `AmwgSampler.sample_summary(n)` keeps it on the GPU and moves a few
-hundred bytes instead. Multi-GPU (one process per GPU): every rank reduces its own shard; the shards are combined with two
-small collectives -- an all-gather of the per-rank moment records (merged exactly, in rank order) and a sum all-reduce of the
-radix-select digit counts (integers) -- so every rank returns the same numbers as a single GPU holding all chains.
+hundred bytes instead. Multi-GPU (one process per GPU): every rank reduces its own shard, and the functions under "combining
+shards" below (gather, gather_tensor, sum_counts, merged_extremes, pooled_moment_record) are the only code here that combines
+shards, so every rank returns the same numbers as a single GPU holding all chains.
 
 Host logic here is plain numpy (tested on CPU); the device work is behind `CudaBlockReducer` (C ABI: amwg_summary_moments,
 amwg_summary_digit_hist, amwg_summary_autocov for the split-chain ESS / MCSE / R-hat of diagnostics=True, and
@@ -138,6 +138,59 @@ class RadixSelect:
     def values(self) -> np.ndarray:
         assert self.npass == 8
         return key_to_double(self.prefix)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# combining shards: every rank ends with the same bits. Records are gathered and merged in rank order, integer counts are
+# summed, extremes are taken as the maximum of order-preserving keys. The collectives run on the device of the tensor they are
+# given (NCCL for CUDA tensors, gloo for the CPU stand-in of the tests); with distributed=False each function is the identity.
+def gather_tensor(t, distributed: bool):
+    """This rank's tensor -> [world, *t.shape] in rank order ([1, *t.shape] when not distributed), on t's device."""
+    if not distributed:
+        return t[None]
+    import torch
+    import torch.distributed as dist
+    ws = dist.get_world_size()
+    out = torch.empty((ws * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+    dist.all_gather_into_tensor(out, t.contiguous())
+    return out.reshape((ws,) + tuple(t.shape))
+
+
+def gather(rec: np.ndarray, like, distributed: bool) -> np.ndarray:
+    """This rank's numpy record -> [world, *rec.shape] in rank order ([1, *rec.shape] when not distributed); it travels on
+    `like`'s device."""
+    rec = np.ascontiguousarray(rec)
+    if not distributed:
+        return rec[None]
+    import torch
+    return gather_tensor(torch.from_numpy(rec).to(like.device), True).cpu().numpy()
+
+
+def sum_counts(t, distributed: bool):
+    """In-place SUM all-reduce of an integer tensor: exact, independent of the number of GPUs. -> t"""
+    if distributed:
+        import torch.distributed as dist
+        dist.all_reduce(t)
+    return t
+
+
+def merged_extremes(rng: np.ndarray, like, distributed: bool) -> np.ndarray:
+    """This rank's [entries, 2] (smallest, largest) -> the smallest and the largest over all ranks: one MAX all-reduce of
+    [-key(smallest), key(largest)], the keys of double_to_key as signed integers, on `like`'s device."""
+    if not distributed:
+        return rng
+    import torch
+    import torch.distributed as dist
+    k = (double_to_key(rng) ^ _SIGN).view(np.int64)
+    t = torch.from_numpy(np.concatenate([-k[:, 0], k[:, 1]])).to(like.device)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    k = t.cpu().numpy()
+    return key_to_double(np.stack([-k[:len(rng)], k[len(rng):]], axis=1).view(np.uint64) ^ _SIGN)
+
+
+def pooled_moment_record(reducer, block, distributed: bool) -> np.ndarray:
+    """reducer.moments of every shard, merged in rank order (merge_moment_records)."""
+    return merge_moment_records(gather(reducer.moments(block), block, distributed))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -390,9 +443,7 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
     rhat_split +inf and ESS NaN. An indicator that is constant (all 1 when the quantile equals the maximum) has ESS = M h. Any other
     series whose W is 0 or not finite (its sums underflowed or overflowed) has ESS NaN, never a finite value, and ess_tail is NaN
     when either indicator's ESS is. A non-finite minimum or maximum (an infinite or NaN draw) makes all four values NaN.
-    Lag windows of at most `max_lags` lags are asked for only while some series' Geyer loop still needs a lag it has not got,
-    the way RadixSelect asks for its next pass. Distributed: each window's per-rank records are all-gathered and merged in rank
-    order, so every rank returns the same numbers."""
+    The lag windows are those of `geyer_windows`."""
     entries = block.shape[1]
     h = rows // 2
     nan = np.full(entries, np.nan)
@@ -400,22 +451,7 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
     if rows < MIN_ROWS:
         return out, 0
     thr = np.stack([np.asarray(lo, dtype=np.float64), np.asarray(hi, dtype=np.float64)], axis=1)
-    est: List[List[GeyerESS]] = []
-    windows = 0
-    lag0 = 0
-    while True:
-        n_lags = min(max_lags, h - lag0)
-        rec = _gather_autocov(reducer.autocov(block, thr, lag0, n_lags), block, distributed)
-        windows += 1
-        if not est:
-            est = [[GeyerESS(rec[e, s], h) for s in range(3)] for e in range(entries)]
-        for e in range(entries):
-            for s in range(3):
-                if est[e][s].need() is not None:
-                    est[e][s].add(rec[e, s, 4:])
-        lag0 += n_lags
-        if all(g.need() is None for row in est for g in row) or lag0 >= h:
-            break
+    est, windows = geyer_windows(reducer, block, thr, h, distributed, max_lags)
     Mh = est[0][0].M * h
     finite = np.isfinite(np.asarray(vmin, dtype=np.float64)) & np.isfinite(np.asarray(vmax, dtype=np.float64))
     for e in range(entries):
@@ -431,18 +467,29 @@ def split_chain_diagnostics(reducer, block, rows: int, sd: np.ndarray, lo: np.nd
     return out, windows
 
 
-def _gather_autocov(rec: np.ndarray, block, distributed: bool) -> np.ndarray:
-    if not distributed:
-        return rec
-    import torch
-    import torch.distributed as dist
-    ws = dist.get_world_size()
-    mine = torch.from_numpy(np.ascontiguousarray(rec))
-    if block.is_cuda:
-        mine = mine.to(block.device)
-    gathered = torch.empty((ws * rec.shape[0],) + rec.shape[1:], dtype=mine.dtype, device=mine.device)
-    dist.all_gather_into_tensor(gathered, mine)
-    return merge_autocov_records(list(gathered.cpu().numpy().reshape((ws,) + rec.shape)))
+def autocov_record(reducer, block, thresholds, lag0: int, n_lags: int, distributed: bool) -> np.ndarray:
+    """reducer.autocov of every shard, merged in rank order (merge_autocov_records)."""
+    return merge_autocov_records(gather(reducer.autocov(block, thresholds, lag0, n_lags), block, distributed))
+
+
+def geyer_windows(reducer, block, thresholds, h: int, distributed: bool, max_lags: int = MAX_LAGS):
+    """-> (the GeyerESS of every entry and series of reducer.autocov(block, thresholds, ...) [entries][series], the number of
+    lag windows used). The first window holds lags [0, min(max_lags, h)); the next window of at most `max_lags` consecutive
+    lags is asked for only while some estimator still needs a lag it has not got, the way RadixSelect asks for its next pass."""
+    est: Optional[List[List[GeyerESS]]] = None
+    windows = lag0 = 0
+    while est is None or (lag0 < h and any(g.need() is not None for row in est for g in row)):
+        n_lags = min(max_lags, h - lag0)
+        rec = autocov_record(reducer, block, thresholds, lag0, n_lags, distributed)
+        if est is None:
+            est = [[GeyerESS(r, h) for r in series] for series in rec]
+        for row, series in zip(est, rec):
+            for g, r in zip(row, series):
+                if g.need() is not None:
+                    g.add(r[4:])
+        lag0 += n_lags
+        windows += 1
+    return est, windows
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -467,9 +514,10 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
     constant at a value of their own (W = 0 for z): ess_bulk NaN (GeyerESS) and rhat_rank +inf.
     Device work per entry and series (CudaBlockReducer): a radix sort of the shard's keys, rank counts against every shard's
     sorted keys, and z written into a [2h][1][chains] block that amwg_summary_autocov splits into exactly the ranked halves.
-    Distributed: the sorted key arrays travel around a ring of torch.distributed send / recv (W - 1 steps, two buffers); the
-    counts are integers, so the ranks and z do not depend on the number of GPUs. The autocovariance records of z merge across
-    ranks as in `split_chain_diagnostics`, so every rank returns the same numbers."""
+    Distributed: the sorted key arrays travel around a ring of torch.distributed send / recv (W - 1 steps, two buffers,
+    `_ring_counts`); the counts are integers, so the ranks and z do not depend on the number of GPUs. The shard sizes and the
+    end keys are gathered, and the autocovariance records of z merged, by the functions of "combining shards", so every rank
+    returns the same numbers."""
     import torch
     entries, chains = block.shape[1], block.shape[2]
     h = rows // 2
@@ -478,7 +526,7 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
         return out
     dev = block.device
     n = 2 * h * chains
-    sizes = _gather_ints([n], block, distributed)[:, 0]
+    sizes = gather(np.array([n], dtype=np.int64), block, distributed)[:, 0]
     total = int(sizes.sum())
     M = total // h
     keys = torch.empty(n + int(sizes.max()), dtype=torch.int64, device=dev)     # sorted keys + the sort's scratch / a ring buffer
@@ -490,15 +538,11 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
     def ranked(e: int, centre: float, zb) -> bool:
         """z-scaled ranks of one series into zb; -> whether all its keys are equal over all shards."""
         reducer.rank_sort(block, e, centre, keys, index)
-        ends = keys[[0, n - 1]].cpu().numpy().view(np.uint64)
-        ends = _gather_ints(ends.view(np.int64), block, distributed).view(np.uint64)
+        ends = gather(keys[[0, n - 1]].cpu().numpy(), block, distributed).view(np.uint64)
         acc.zero_()
         _ring_counts(reducer, keys, n, sizes, acc, ring, distributed)
         reducer.rank_z(acc, index, n, total, zb)
         return bool(ends[:, 0].min() == ends[:, 1].max())
-
-    def records(zb, lag0: int, n_lags: int) -> np.ndarray:
-        return _gather_autocov(reducer.autocov(zb, None, lag0, n_lags), zb, distributed)[0, 0]
 
     for e in range(entries):
         if np.isnan(vmin[e]) or np.isnan(vmax[e]):
@@ -506,14 +550,7 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
         if vmin[e] == vmax[e] or ranked(e, float("nan"), z[0]):
             out["ess_bulk"][e] = M * h
             continue
-        rec = records(z[0], 0, min(max_lags, h))
-        g = GeyerESS(rec, h)
-        g.add(rec[4:])
-        lag0 = len(g.rho)
-        while g.need() is not None and lag0 < h:
-            n_lags = min(max_lags, h - lag0)
-            g.add(records(z[0], lag0, n_lags)[4:])
-            lag0 += n_lags
+        g = geyer_windows(reducer, z[0], None, h, distributed, max_lags)[0][0][0]
         out["ess_bulk"][e] = g.ess
         with np.errstate(invalid="ignore", divide="ignore"):
             rhat = np.sqrt(g.varplus / g.W)
@@ -522,25 +559,9 @@ def rank_diagnostics(reducer, block, rows: int, med: np.ndarray, vmin: np.ndarra
             if ranked(e, float(med[e]), z[1]):
                 out["rhat_rank"][e] = rhat
                 continue
-            gf = GeyerESS(records(z[1], 0, 1), h)
+            gf = GeyerESS(autocov_record(reducer, z[1], None, 0, 1, distributed)[0, 0], h)     # W and var+ only: one lag
             out["rhat_rank"][e] = max(rhat, np.sqrt(gf.varplus / gf.W))
     return out
-
-
-def _gather_ints(vals, block, distributed: bool) -> np.ndarray:
-    """int64 values of this rank -> [world, len(vals)] in rank order ([1, len] when not distributed)."""
-    mine = np.asarray(vals, dtype=np.int64).reshape(1, -1)
-    if not distributed:
-        return mine
-    import torch
-    import torch.distributed as dist
-    ws = dist.get_world_size()
-    t = torch.from_numpy(np.ascontiguousarray(mine[0]))
-    if block.is_cuda:
-        t = t.to(block.device)
-    gathered = torch.empty(ws * t.numel(), dtype=torch.int64, device=t.device)
-    dist.all_gather_into_tensor(gathered, t)
-    return gathered.cpu().numpy().reshape(ws, -1)
 
 
 def _ring_counts(reducer, keys, n: int, sizes: np.ndarray, acc, ring, distributed: bool) -> None:
@@ -573,30 +594,19 @@ def check_diagnostics(diagnostics) -> None:
 
 
 def summarise_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], distributed: bool, diagnostics=False):
-    """-> (mean, sd, rhat, quantiles[len(probs)]) per entry, over all shards. `reducer` does the per-shard device work;
-    the collectives run on the tensors it returns (NCCL for CUDA tensors, gloo for the CPU stand-in used in the tests).
-    diagnostics=True appends (split_chain_diagnostics' dict, lag windows used): the select also forms the minimum, q05, q95 and
-    the maximum (each quantile is its own order statistics, so the requested ones are unchanged). diagnostics="rank" also forms
+    """-> (mean, sd, rhat, quantiles[len(probs)]) per entry, over all shards. `reducer` does the per-shard device work; the
+    moment records merge by pooled_moment_record and the select's digit counts add up by sum_counts. diagnostics=True appends
+    (split_chain_diagnostics' dict, lag windows used): the select also forms the minimum, q05, q95 and the maximum (each
+    quantile is its own order statistics, so the requested ones are unchanged). diagnostics="rank" also forms
     the median and adds rank_diagnostics' "ess_bulk" and "rhat_rank" to that dict; every other value is the same bits. The mean
     and the returned quantiles of an entry with NaN or infinite draws are numpy's (nonfinite_as_numpy); the internal order
     statistics that feed the diagnostics keep their bits."""
-    import torch
     check_diagnostics(diagnostics)
     entries = block.shape[1]
     user_probs = [float(p) for p in probs]
     if diagnostics:
         probs = user_probs + list(DIAGNOSTIC_PROBS) + (list(RANK_PROBS) if diagnostics == "rank" else [])
-    rec = reducer.moments(block)
-    if distributed:
-        import torch.distributed as dist
-        ws = dist.get_world_size()
-        mine = torch.from_numpy(rec.copy())
-        if block.is_cuda:
-            mine = mine.to(block.device)
-        gathered = torch.empty((ws * entries, 4), dtype=mine.dtype, device=mine.device)     # concatenated on dim 0
-        dist.all_gather_into_tensor(gathered, mine)
-        rec = merge_moment_records(list(gathered.cpu().numpy().reshape(ws, entries, 4)))
-    mean, sd, rhat = finalize_moments(rec, rows)
+    mean, sd, rhat = finalize_moments(pooled_moment_record(reducer, block, distributed), rows)
 
     probs = [float(p) for p in probs]
     q = np.empty((len(probs), entries))
@@ -627,11 +637,7 @@ def _select(reducer, block, ranks: np.ndarray, distributed: bool) -> RadixSelect
     sel = RadixSelect(block.shape[1], ranks)
     for npass in range(8):
         table, which = sel.prefixes()
-        counts = reducer.digit_counts(block, npass, table)
-        if distributed:
-            import torch.distributed as dist
-            dist.all_reduce(counts)                           # integer sums: exact, independent of the number of GPUs
-        sel.advance(counts.cpu().numpy(), which)
+        sel.advance(sum_counts(reducer.digit_counts(block, npass, table), distributed).cpu().numpy(), which)
     return sel
 
 
@@ -687,6 +693,37 @@ def _is_int(v) -> bool:
     return isinstance(v, numbers.Integral) and not isinstance(v, bool)
 
 
+def entry_spans(names: Sequence[str], dims) -> dict:
+    """{name: (first entry, number of entries)} of the names laid out in order in a sample block, prod(dims[name]) entries each
+    (row-major). A name listed twice in monitor: its last block, as sample_summary returns it."""
+    spans = {}
+    first = 0
+    for name in names:
+        n = int(np.prod(dims[name]))
+        spans[name] = (first, n)
+        first += n
+    return spans
+
+
+def selector(sel, spans: dict, what: str) -> Tuple[object, int]:
+    """One entry selector, a scalar's name or (name, flat_index) -> (label, block entry); the label is the name, or
+    (name, int(flat_index)). `what` starts every error message."""
+    if isinstance(sel, str):
+        if sel not in spans:
+            raise ValueError("%s: %r is not a monitored parameter or derived quantity" % (what, sel))
+        if spans[sel][1] != 1:
+            raise ValueError("%s: %r has %d components; select one as (%r, flat_index)" % (what, sel, spans[sel][1], sel))
+        return sel, spans[sel][0]
+    if isinstance(sel, (tuple, list)) and len(sel) == 2 and isinstance(sel[0], str) and _is_int(sel[1]):
+        name, i = sel
+        if name not in spans:
+            raise ValueError("%s: %r is not a monitored parameter or derived quantity" % (what, name))
+        if not 0 <= i < spans[name][1]:
+            raise ValueError("%s: component %d of %r is outside [0, %d)" % (what, i, name, spans[name][1]))
+        return (name, int(i)), spans[name][0] + int(i)
+    raise ValueError("%s selector must be a name or (name, flat_index), not %r" % (what, sel))
+
+
 def resolve_histogram(spec, names: Sequence[str], dims) -> Optional[HistogramPlan]:
     """Checks the `histogram=` argument of sample_summary against the monitored names (in sample-block order, only those with
     entries) and their dims ({name: dim list}; the entries of a name are prod(dim), row-major) and returns the plan, or None for
@@ -700,12 +737,8 @@ def resolve_histogram(spec, names: Sequence[str], dims) -> Optional[HistogramPla
     unknown = [k for k in spec if k not in _HIST_KEYS]
     if unknown:
         raise ValueError("histogram has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(_HIST_KEYS)))
-    span = {}
-    entries = 0
-    for name in names:                                        # a name listed twice in monitor: its last block, as sample_summary
-        n = int(np.prod(dims[name]))
-        span[name] = (entries, n)
-        entries += n
+    span = entry_spans(names, dims)
+    entries = sum(span[name][1] for name in names)
 
     bins = spec.get("bins")
     if "bins" in spec and not (_is_int(bins) and 1 <= bins <= MAX_HIST_BINS):
@@ -728,20 +761,8 @@ def resolve_histogram(spec, names: Sequence[str], dims) -> Optional[HistogramPla
         fixed[s0:s0 + n] = (float(r[0]), float(r[1]))
 
     def entry(sel) -> Tuple[object, int]:
-        if isinstance(sel, str):
-            if sel not in span:
-                raise ValueError("histogram pair: %r is not a monitored parameter or derived quantity" % (sel,))
-            if span[sel][1] != 1:
-                raise ValueError("histogram pair: %r has %d components; select one as (%r, flat_index)" % (sel, span[sel][1], sel))
-            return sel, span[sel][0]
-        if isinstance(sel, (tuple, list)) and len(sel) == 2 and isinstance(sel[0], str) and _is_int(sel[1]):
-            name, i = sel
-            if name not in span:
-                raise ValueError("histogram pair: %r is not a monitored parameter or derived quantity" % (name,))
-            if not 0 <= i < span[name][1]:
-                raise ValueError("histogram pair: component %d of %r is outside [0, %d)" % (i, name, span[name][1]))
-            return (name, int(i)) if isinstance(sel, list) else sel, span[name][0] + int(i)
-        raise ValueError("histogram pair selector must be a name or (name, flat_index), not %r" % (sel,))
+        label, e = selector(sel, span, "histogram pair")
+        return label if isinstance(sel, list) else sel, e          # a tuple selector keys the pair as given
 
     given = spec.get("pairs", [])
     if not isinstance(given, (tuple, list)):
@@ -761,17 +782,6 @@ def resolve_histogram(spec, names: Sequence[str], dims) -> Optional[HistogramPla
     return HistogramPlan(bins, fixed, pairs, pair_bins)
 
 
-def _sortable(x: np.ndarray) -> np.ndarray:
-    """float64 -> int64 whose signed order is the order of the doubles (-0 below +0)."""
-    u = np.ascontiguousarray(x, dtype=np.float64).view(np.int64)
-    return np.where(u < 0, u ^ np.int64(0x7FFFFFFFFFFFFFFF), u)
-
-
-def _unsortable(k: np.ndarray) -> np.ndarray:
-    k = np.asarray(k, dtype=np.int64)
-    return np.where(k < 0, k ^ np.int64(0x7FFFFFFFFFFFFFFF), k).view(np.float64)
-
-
 def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed: bool) -> dict:
     """-> {"hist" [entries, bins] int64, "hist_edges" [entries, bins + 1], "hist_outside" [entries, 3] int64 (when plan.bins),
     "pairs": {key: {"hist" [pair_bins, pair_bins] int64, "xedges", "yedges"}}} over all shards; only reads the block.
@@ -782,8 +792,8 @@ def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed:
     the draws < lo (-inf included), > hi (+inf included) and NaN, so hist.sum() + hist_outside.sum() is the number of draws.
     A pair's axes are its two entries' ranges at plan.pair_bins; a draw counts when both values lie inside their axis's edges,
     each binned as numpy.histogramdd bins it (searchsorted right, the last edge in the last bin).
-    Distributed: one MAX all-reduce of the extremes (as order-preserving integers, the minimum negated) and one SUM all-reduce of
-    all the counts, so every rank returns the same bits whatever the number of GPUs."""
+    Distributed: the extremes combine by merged_extremes and all the counts add up in one sum_counts, so every rank returns the
+    same bits whatever the number of GPUs."""
     import torch
     entries = block.shape[1]
     lo, hi = plan.fixed[:, 0].copy(), plan.fixed[:, 1].copy()
@@ -793,16 +803,7 @@ def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed:
         used[a] = used[b] = True
     auto = np.isnan(lo)
     if np.any(auto & used):
-        rng = reducer.finite_range(block)[0].cpu().numpy()
-        if distributed:
-            import torch.distributed as dist
-            keys = np.concatenate([-_sortable(rng[:, 0]), _sortable(rng[:, 1])])
-            t = torch.from_numpy(keys)
-            if block.is_cuda:
-                t = t.to(block.device)
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            keys = t.cpu().numpy()
-            rng = np.stack([_unsortable(-keys[:entries]), _unsortable(keys[entries:])], axis=1)
+        rng = merged_extremes(reducer.finite_range(block)[0].cpu().numpy(), block, distributed)
         for e in np.flatnonzero(auto):
             a, b = rng[e]
             lo[e], hi[e] = (0.0, 1.0) if not a <= b else (a - 0.5, b + 0.5) if a == b else (a, b)
@@ -819,10 +820,8 @@ def histogram_block(reducer, block, rows: int, plan: HistogramPlan, distributed:
         e2 = edges(plan.pair_bins)
         pair_idx = np.array([(a, b) for _k, a, b in plan.pairs], dtype=np.int32)
         parts.append(reducer.histogram2d(block, pair_idx, e2, plan.pair_bins))
-    if distributed:
-        import torch.distributed as dist
-        flat = torch.cat([p.reshape(-1) for p in parts])
-        dist.all_reduce(flat)                                 # integer sums: exact, independent of the number of GPUs
+    if distributed:                                           # one all-reduce for all the counts
+        flat = sum_counts(torch.cat([p.reshape(-1) for p in parts]), distributed)
         parts = list(torch.split(flat, [p.numel() for p in parts]))
     counts = [p.cpu().numpy().astype(np.int64, copy=False) for p in parts]
     out = {"pairs": {}}
@@ -855,35 +854,15 @@ def resolve_covariance(spec, names: Sequence[str], dims) -> Optional[CovarianceP
     device work."""
     if spec is None or spec is False:
         return None
-    if "covariance" in names:
-        raise ValueError("covariance: a monitored parameter or derived quantity is named 'covariance', the key the result would use")
-    span = {}
-    entries = 0
-    for name in names:                                        # a name listed twice in monitor: its last block, as sample_summary
-        n = int(np.prod(dims[name]))
-        span[name] = (entries, n)
-        entries += n
+    _check_result_key("covariance", names)
+    span = entry_spans(names, dims)
     if spec is True:
         labels = [name if span[name][1] == 1 else (name, i) for name in span for i in range(span[name][1])]
         idx = [span[name][0] + i for name in span for i in range(span[name][1])]
     elif isinstance(spec, (list, tuple)):
         labels, idx = [], []
         for sel in spec:
-            if isinstance(sel, str):
-                if sel not in span:
-                    raise ValueError("covariance: %r is not a monitored parameter or derived quantity" % (sel,))
-                if span[sel][1] != 1:
-                    raise ValueError("covariance: %r has %d components; select one as (%r, flat_index)" % (sel, span[sel][1], sel))
-                label, e = sel, span[sel][0]
-            elif isinstance(sel, (tuple, list)) and len(sel) == 2 and isinstance(sel[0], str) and _is_int(sel[1]):
-                name, i = sel
-                if name not in span:
-                    raise ValueError("covariance: %r is not a monitored parameter or derived quantity" % (name,))
-                if not 0 <= i < span[name][1]:
-                    raise ValueError("covariance: component %d of %r is outside [0, %d)" % (i, name, span[name][1]))
-                label, e = (name, int(i)), span[name][0] + int(i)
-            else:
-                raise ValueError("covariance selector must be a name or (name, flat_index), not %r" % (sel,))
+            label, e = selector(sel, span, "covariance")
             if e in idx:
                 raise ValueError("covariance: %r selects an entry already selected" % (sel,))
             labels.append(label)
@@ -972,19 +951,9 @@ def finalize_comoments(rec: np.ndarray, rows: int) -> dict:
 
 def covariance_block(reducer, block, rows: int, plan: CovariancePlan, distributed: bool) -> dict:
     """-> finalize_comoments' dict plus "labels", over all shards; only reads the block. Each shard's record comes from
-    reducer.comoments; distributed: one all_gather_into_tensor of the fixed-size records, merged on the host in rank order,
-    so every rank returns the same bits."""
-    rec = reducer.comoments(block, plan.entries)
-    if distributed:
-        import torch
-        import torch.distributed as dist
-        ws = dist.get_world_size()
-        mine = torch.from_numpy(np.ascontiguousarray(rec))
-        if block.is_cuda:
-            mine = mine.to(block.device)
-        gathered = torch.empty(ws * rec.size, dtype=mine.dtype, device=mine.device)
-        dist.all_gather_into_tensor(gathered, mine)
-        rec = merge_comoment_records(list(gathered.cpu().numpy().reshape(ws, rec.size)))
+    reducer.comoments; distributed: the fixed-size records are gathered (gather) and merged on the host in rank order
+    (merge_comoment_records), so every rank returns the same bits."""
+    rec = merge_comoment_records(gather(reducer.comoments(block, plan.entries), block, distributed))
     out = {"labels": list(plan.labels)}
     out.update(finalize_comoments(rec, rows))
     return out
@@ -1075,22 +1044,9 @@ def finalize_nested(rec: np.ndarray) -> np.ndarray:
 
 def nested_block(reducer, block, rows: int, first_chain: int, M: int, distributed: bool) -> np.ndarray:
     """-> rhat_nested per entry over all shards; only reads the block. Each shard's record comes from reducer.nested;
-    distributed: one all_gather_into_tensor of the fixed-size records, merged on the host in rank order (merge_nested_records),
-    so every rank returns the same bits."""
-    rec = reducer.nested(block, first_chain, M)
-    if distributed:
-        import torch
-        import torch.distributed as dist
-        ws = dist.get_world_size()
-        mine = torch.from_numpy(np.ascontiguousarray(rec))
-        if block.is_cuda:
-            mine = mine.to(block.device)
-        gathered = torch.empty((ws * rec.shape[0], NESTED_RECORD), dtype=mine.dtype, device=mine.device)
-        dist.all_gather_into_tensor(gathered, mine)
-        recs = list(gathered.cpu().numpy().reshape(ws, rec.shape[0], NESTED_RECORD))
-    else:
-        recs = [rec]
-    return finalize_nested(merge_nested_records(recs, M, rows))
+    distributed: the fixed-size records are gathered (gather) and merged on the host in rank order (merge_nested_records), so
+    every rank returns the same bits."""
+    return finalize_nested(merge_nested_records(gather(reducer.nested(block, first_chain, M), block, distributed), M, rows))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1113,22 +1069,33 @@ def resolve_loo(spec, names: Sequence[str]) -> Optional[LooPlan]:
     before any device work (tracing log_lik is the caller's next check)."""
     if spec is None:
         return None
-    if not isinstance(spec, dict):
-        raise ValueError("loo must be None or a dict {\"log_lik\": ..., \"points\": ...}, not %r" % (spec,))
-    unknown = [k for k in spec if k not in LOO_KEYS]
-    if unknown:
-        raise ValueError("loo has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(LOO_KEYS)))
-    if not callable(spec.get("log_lik")):
-        raise ValueError("loo needs \"log_lik\": a function (state, data, i) -> the log-likelihood of point i")
-    points = spec.get("points")
-    if not (_is_int(points) and points >= 1):
-        raise ValueError("loo points must be an int >= 1, not %r" % (points,))
+    log_lik, points = _log_lik_spec(spec, "loo", LOO_KEYS, "the log-likelihood of point i")
     r_eff = spec.get("r_eff", 1.0)
     if not (isinstance(r_eff, numbers.Real) and not isinstance(r_eff, bool) and np.isfinite(r_eff) and r_eff > 0):
         raise ValueError("loo r_eff must be a finite number > 0, not %r" % (r_eff,))
-    if "loo" in names:
-        raise ValueError("loo: a monitored parameter or derived quantity is named 'loo', the key the result would use")
-    return LooPlan(spec["log_lik"], int(points), float(r_eff))
+    _check_result_key("loo", names)
+    return LooPlan(log_lik, points, float(r_eff))
+
+
+def _log_lik_spec(spec, what: str, keys: Sequence[str], value: str) -> Tuple[object, int]:
+    """The checks `loo=` and `ppc=` share: a dict of `keys` with a callable "log_lik" and an int "points" >= 1; -> (log_lik,
+    points). `value` says what log_lik returns."""
+    if not isinstance(spec, dict):
+        raise ValueError("%s must be None or a dict {\"log_lik\": ..., \"points\": ...}, not %r" % (what, spec))
+    unknown = [k for k in spec if k not in keys]
+    if unknown:
+        raise ValueError("%s has unknown key(s) %s; the keys are %s" % (what, ", ".join(map(repr, unknown)), ", ".join(keys)))
+    if not callable(spec.get("log_lik")):
+        raise ValueError("%s needs \"log_lik\": a function (state, data, i) -> %s" % (what, value))
+    points = spec.get("points")
+    if not (_is_int(points) and points >= 1):
+        raise ValueError("%s points must be an int >= 1, not %r" % (what, points))
+    return spec["log_lik"], int(points)
+
+
+def _check_result_key(key: str, names: Sequence[str]) -> None:
+    if key in names:
+        raise ValueError("%s: a monitored parameter or derived quantity is named '%s', the key the result would use" % (key, key))
 
 
 def loo_tail_length(S: int, r_eff: float) -> int:
@@ -1198,41 +1165,6 @@ class CudaPointwise:
         return out
 
 
-
-
-def _merged_range(reducer, ll, distributed: bool):
-    """-> (llmin, llmax, any non-finite) per point over all shards: the finite extremes and the non-finite counts."""
-    import torch
-    rng, nonfinite = reducer.finite_range(ll)
-    if distributed:
-        import torch.distributed as dist
-        P = ll.shape[1]
-        r = rng.cpu().numpy()
-        keys = torch.from_numpy(np.concatenate([-_sortable(r[:, 0]), _sortable(r[:, 1])]))
-        if ll.is_cuda:
-            keys = keys.to(ll.device)
-        dist.all_reduce(keys, op=dist.ReduceOp.MAX)
-        keys = keys.cpu().numpy()
-        rng = np.stack([_unsortable(-keys[:P]), _unsortable(keys[P:])], axis=1)
-        dist.all_reduce(nonfinite)
-    else:
-        rng = rng.cpu().numpy()
-    nf = nonfinite.cpu().numpy().sum(axis=1) > 0
-    return rng[:, 0].copy(), rng[:, 1].copy(), nf
-
-
-def _gather_tensor(t, distributed: bool):
-    """this rank's tensor -> [world, *shape] in rank order ([1, *shape] when not distributed)."""
-    if not distributed:
-        return t[None]
-    import torch
-    import torch.distributed as dist
-    ws = dist.get_world_size()
-    out = torch.empty((ws * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
-    dist.all_gather_into_tensor(out, t.contiguous())
-    return out.reshape((ws,) + tuple(t.shape))
-
-
 def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff: float, chunk_points: int, distributed: bool) -> dict:
     """-> the "loo" dict of sample_summary over all shards: PSIS-LOO and WAIC from the pointwise log-likelihood ll[s, i] of the
     S = rows x total_chains kept draws. `source.chunk(p0, P)` gives ll of points p0 .. p0 + P - 1 as a [rows, P, chains] block
@@ -1249,10 +1181,10 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
       pareto_k_i  the fitted k (+inf for a tail of <= 4 draws, or when no candidate of the fit has a finite profile value)
     A point with any non-finite ll gets NaN in every value. Totals: sums of the pointwise values, se_* = sqrt(points var_i(elpd_*_i))
     (ddof 0), looic = -2 elpd_loo, waic = -2 elpd_waic, pareto_k_threshold = min(1 - 1 / log10 S, 0.7), n_high_k = #{k > threshold}.
-    Distributed: extremes and counts all-reduce, moment records all-gather and merge in rank order, the select's counts
-    all-reduce, sums all-gather and add in rank order, tails all-gather (at most M values per point in all); the fit runs on the
-    merged tail, so every rank returns the same numbers."""
-    import torch
+    Distributed: the extremes combine by merged_extremes, the non-finite counts and the select's counts add up by sum_counts,
+    the moment records merge by pooled_moment_record, the sums are gathered and added in rank order, and the tails are gathered
+    (gather_tensor; at most M values per point in all); the fit runs on the merged tail, so every rank returns the same
+    numbers."""
     S = rows * total_chains
     M = check_loo_size(S, r_eff)
     cap = loo_tail_cap(M)
@@ -1260,10 +1192,10 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
     for p0 in range(0, points, chunk_points):
         P = min(chunk_points, points - p0)
         ll = source.chunk(p0, P)
-        llmin, llmax, skip = _merged_range(reducer, ll, distributed)
-        rec = reducer.moments(ll)
-        if distributed:
-            rec = merge_moment_records(list(_gather_tensor(torch.from_numpy(rec).to(ll.device), True).cpu().numpy()))
+        rng, nonfinite = reducer.finite_range(ll)
+        llmin, llmax = merged_extremes(rng.cpu().numpy(), ll, distributed).T
+        skip = sum_counts(nonfinite, distributed).cpu().numpy().sum(axis=1) > 0
+        rec = pooled_moment_record(reducer, ll, distributed)
         var = (rec[:, 3] + rows * rec[:, 2]) / S
         llM = _select(reducer, ll, np.array([M], dtype=np.int64), distributed).values()[:, 0]
         with np.errstate(invalid="ignore"):
@@ -1272,12 +1204,11 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
         mn, mx, ct = np.where(skip, 0.0, llmin), np.where(skip, 0.0, llmax), np.where(skip, np.inf, cut)
         sums, tails, counts = reducer.loo_reduce(ll, mn, mx, ct, cap)
         del ll
-        if distributed:
-            parts = _gather_tensor(torch.from_numpy(np.ascontiguousarray(sums)).to(tails.device), True).cpu().numpy()
-            sums = parts[0].copy()
-            for q in parts[1:]:
-                sums = sums + q
-        fit = reducer.loo_fit(_gather_tensor(tails, distributed), _gather_tensor(counts, distributed), mn, ct, skip.astype(np.int32))
+        parts = gather(sums, tails, distributed)
+        sums = parts[0]
+        for q in parts[1:]:
+            sums = sums + q
+        fit = reducer.loo_fit(gather_tensor(tails, distributed), gather_tensor(counts, distributed), mn, ct, skip.astype(np.int32))
         del tails, counts
         if np.any(fit[~skip, 3] > M):
             raise RuntimeError("loo: a point's tail holds more than M = %d draws (inconsistent select)" % M)
@@ -1322,19 +1253,9 @@ def resolve_ppc(spec, names: Sequence[str]) -> Optional[PpcPlan]:
     check_ppc_call are the caller's next checks)."""
     if spec is None:
         return None
-    if not isinstance(spec, dict):
-        raise ValueError("ppc must be None or a dict {\"log_lik\": ..., \"points\": ...}, not %r" % (spec,))
-    unknown = [k for k in spec if k not in PPC_KEYS]
-    if unknown:
-        raise ValueError("ppc has unknown key(s) %s; the keys are %s" % (", ".join(map(repr, unknown)), ", ".join(PPC_KEYS)))
-    if not callable(spec.get("log_lik")):
-        raise ValueError("ppc needs \"log_lik\": a function (state, data, i) -> one ld.* call at data point i")
-    points = spec.get("points")
-    if not (_is_int(points) and points >= 1):
-        raise ValueError("ppc points must be an int >= 1, not %r" % (points,))
-    if "ppc" in names:
-        raise ValueError("ppc: a monitored parameter or derived quantity is named 'ppc', the key the result would use")
-    return PpcPlan(spec["log_lik"], int(points))
+    log_lik, points = _log_lik_spec(spec, "ppc", PPC_KEYS, "one ld.* call at data point i")
+    _check_result_key("ppc", names)
+    return PpcPlan(log_lik, points)
 
 
 def check_ppc_call(family: str, rows: int, points: int) -> int:
@@ -1413,25 +1334,6 @@ class CudaPpc:
         return self.T
 
 
-def _pooled_moments(reducer, block, rows: int, distributed: bool):
-    """(mean, sd) per entry over all shards, as summarise_block forms them (finalize_moments of the merged records)"""
-    import torch
-    rec = reducer.moments(block)
-    if distributed:
-        rec = merge_moment_records(list(_gather_tensor(torch.from_numpy(rec).to(block.device), True).cpu().numpy()))
-    mean, sd, _ = finalize_moments(rec, rows)
-    return mean, sd
-
-
-def _counts(reducer, block, thresholds, distributed: bool) -> np.ndarray:
-    """-> int64 [entries, 4] (<, ==, >, NaN) over all shards: integer sums, exact on any number of GPUs"""
-    c = reducer.threshold_counts(block, np.ascontiguousarray(thresholds, dtype=np.float64))
-    if distributed:
-        import torch.distributed as dist
-        dist.all_reduce(c)
-    return c.cpu().numpy().astype(np.int64)
-
-
 def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family: str, y, probs: Sequence[float], chunk_points: int,
               distributed: bool) -> dict:
     """-> the "ppc" dict of sample_summary over all shards, for the S = rows x total_chains kept draws. `source.chunk(p0, P)` gives
@@ -1442,8 +1344,9 @@ def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family
     "n_below" / "n_equal" / "n_nan" (int64: y_rep_i < y_i, == y_i, NaN), "pit" = (n_below + n_equal) / S (ArviZ's u-value).
     stats: per T, "observed" T(y) (dataset_stats), "mean", "sd" and "quantiles" (`probs`) of T(y_rep) from summarise_block,
     "n_greater", "n_equal", "n_nan" and "p_value" = (n_greater + n_equal) / S, Pr(T(y_rep) >= T(y)) with a NaN draw counted as
-    not >= (and with T(y) NaN, no draw is). Distributed: moment records all-gather and merge in rank order, counts all-reduce,
-    summarise_block takes its distributed path; every rank returns the same numbers."""
+    not >= (and with T(y) NaN, no draw is). Distributed: the moment records merge by pooled_moment_record, the threshold counts
+    (int64 [entries, 4]: <, ==, >, NaN) add up by sum_counts, and summarise_block takes its distributed path; every rank returns
+    the same numbers."""
     S = rows * total_chains
     y = np.ascontiguousarray(y, dtype=np.float64)
     pw = {"mean": np.empty(points), "sd": np.empty(points)}
@@ -1452,14 +1355,14 @@ def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family
         P = min(chunk_points, points - p0)
         yrep = source.chunk(p0, P)
         sl = slice(p0, p0 + P)
-        pw["mean"][sl], pw["sd"][sl] = _pooled_moments(reducer, yrep, rows, distributed)
-        cnt[sl] = _counts(reducer, yrep, y[sl], distributed)
+        pw["mean"][sl], pw["sd"][sl], _rhat = finalize_moments(pooled_moment_record(reducer, yrep, distributed), rows)
+        cnt[sl] = sum_counts(reducer.threshold_counts(yrep, y[sl]), distributed).cpu().numpy()
         del yrep
     pw.update(n_below=cnt[:, 0], n_equal=cnt[:, 1], pit=(cnt[:, 0] + cnt[:, 1]) / S, n_nan=cnt[:, 3])
     T = source.stats()
     obs = dataset_stats(y)
     mean, sd, _rhat, q = summarise_block(reducer, T, rows, total_chains, probs, distributed)
-    tc = _counts(reducer, T, obs, distributed)
+    tc = sum_counts(reducer.threshold_counts(T, obs), distributed).cpu().numpy()
     stats = {}
     for k, name in enumerate(PPC_STATS):
         stats[name] = {"observed": float(obs[k]), "mean": float(mean[k]), "sd": float(sd[k]), "quantiles": q[:, k].copy(),
