@@ -70,7 +70,8 @@ EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_samp
            "amwg_summary_rank_count", "amwg_summary_rank_z", "amwg_peak_fp64", "amwg_jit_status", "amwg_jit_compile_check",
            "amwg_plate_sources", "amwg_get_term_cache", "amwg_summary_finite_range", "amwg_summary_histogram", "amwg_summary_histogram2d",
            "amwg_summary_comoments", "amwg_disperse_state_superchains", "amwg_summary_nested",
-           "amwg_loo_pointwise", "amwg_loo_reduce", "amwg_loo_fit", "amwg_ppc_pointwise", "amwg_summary_threshold_counts"]
+           "amwg_loo_pointwise", "amwg_loo_reduce", "amwg_loo_fit", "amwg_ppc_pointwise", "amwg_summary_threshold_counts",
+           "amwg_loo_pit_reduce", "amwg_loo_pit_fit"]
 
 _lib = None
 
@@ -128,6 +129,8 @@ def lib():
     L.amwg_loo_pointwise.argtypes = [vp, pi, i32, pd, i32, i32, pi, pi, i32, vp, i64, i32, i64, i32, vp]; L.amwg_loo_pointwise.restype = C.c_int
     L.amwg_loo_reduce.argtypes = [C.c_int, vp, i64, i32, i64, vp, vp, vp, i32, vp, vp, vp]; L.amwg_loo_reduce.restype = C.c_int
     L.amwg_loo_fit.argtypes = [C.c_int, vp, vp, i32, i32, i32, vp, vp, vp, vp]; L.amwg_loo_fit.restype = C.c_int
+    L.amwg_loo_pit_reduce.argtypes = [C.c_int, vp, vp, i64, i32, i64, vp, vp, vp, i32, vp, vp, vp, vp]; L.amwg_loo_pit_reduce.restype = C.c_int
+    L.amwg_loo_pit_fit.argtypes = [C.c_int, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp]; L.amwg_loo_pit_fit.restype = C.c_int
     L.amwg_ppc_pointwise.argtypes = [vp, pi, i32, pd, i32, i32, pi, i32, pi, pi, i32, vp, i64, i32, i64, i64, i32, vp, vp]
     L.amwg_ppc_pointwise.restype = C.c_int
     L.amwg_summary_threshold_counts.argtypes = [C.c_int, vp, i64, i32, i64, vp, vp]; L.amwg_summary_threshold_counts.restype = C.c_int

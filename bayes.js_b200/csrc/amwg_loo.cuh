@@ -2,7 +2,8 @@
 // Vehtari et al., JMLR 2024) for sample_summary(..., loo=...), DESIGN.md §4.7: the generalised Pareto fit of Zhang & Stephens
 // (2009) with the weakly informative prior on k, and the smoothed tail weights, in ArviZ's operations. The fit kernel of
 // amwg_summary_loo.cuh forms its sums in parallel with these element functions; loo_fit_seq is the same fit with sequential sums,
-// which tests/host_shim/loo_host.cpp compiles for the host. Plain __host__ __device__ code: no CUDA intrinsics.
+// which tests/host_shim/loo_host.cpp compiles for the host. The run-mean step of LOO-PIT (run_mean_sums) is here for the same
+// reason (tests/host_shim/loo_pit_host.cpp). Plain __host__ __device__ code: no CUDA intrinsics.
 #pragma once
 
 #include <cmath>
@@ -92,6 +93,26 @@ __host__ __device__ inline void loo_fit_seq(const double* x, int n, double* b, d
   const double k = s / (double)n;
   *sigma_out = -k / bp;
   *k_out = fit_prior_k(k, n);
+}
+
+// LOO-PIT (DESIGN.md §4.9): the flag bits of a tail draw, its y_rep <= y and y_rep == y
+constexpr unsigned char kPitLe = 1, kPitEq = 2;
+
+// The run-mean rule of LOO-PIT over one run of tied ll: w[0 .. len) the smoothed weights of the run's ranks, f[0 .. len) the
+// flags of the draws sorted into them. Every draw of the run gets the run's mean weight (sum of w) / len, so the run adds
+// mean x (its draws with y_rep <= y) to *le and mean x (its draws with y_rep == y) to *eq. The weights are summed in rank order
+// and the flags only counted: the result does not depend on how the sort ordered the tied draws.
+__host__ __device__ inline void run_mean_sums(const double* w, const unsigned char* f, int len, double* le, double* eq) {
+  double s = 0.0;
+  int n_le = 0, n_eq = 0;
+  for (int j = 0; j < len; ++j) {
+    s += w[j];
+    n_le += f[j] & kPitLe;
+    n_eq += (f[j] & kPitEq) >> 1;
+  }
+  const double mean = s / (double)len;
+  *le = mean * (double)n_le;
+  *eq = mean * (double)n_eq;
 }
 
 }  // namespace loo

@@ -12,6 +12,11 @@
 //                                     K_l3 sorts them)
 //   K_l3  amwg_loo_fit_kernel       : one CTA per point: the shards' tails gathered and sorted (bitonic, in global scratch), the
 //                                     generalised Pareto fit of amwg_loo.cuh, the smoothed tail weights and their two sums
+// LOO-PIT of sample_summary(..., ppc={..., "loo_pit": ...}) (DESIGN.md §4.9) runs the same two bodies with y_rep beside ll:
+//   K_q1  amwg_loo_pit_reduce_kernel: K_l2 with sum exp(lw) and its parts where y_rep <= y and y_rep == y; each tail draw's two
+//                                     flag bits stored at its slot beside its ll
+//   K_q2  amwg_loo_pit_fit_kernel   : K_l3 with the flags sorted along with the ll, and the flag sums formed by the run-mean
+//                                     rule (every draw of a run of tied ll weighted by the run's mean weight)
 // Included at the end of amwg_kernels.cu, after amwg_summary.cuh (cta_sum, amwg_merge_sums_kernel, chain_ctas).
 #pragma once
 
@@ -67,32 +72,52 @@ __global__ void __launch_bounds__(kThreads) amwg_loo_pointwise_kernel(const int*
   for (int i = p0; o != end; o += C, ++i) *o = run_program_t<false>(code_sa, consts_sa, ctx, es, body_pc, nullptr, true, i);
 }
 
-// K_l2. Grid (chain groups, points). partial[point][3][gridDim.x]; tail[point][cap], count[point] (zeroed by the caller).
-__global__ void __launch_bounds__(256) amwg_loo_reduce_kernel(const double* __restrict__ x, long long rows, int P, long long C,
-                                                              const double* __restrict__ llmin, const double* __restrict__ llmax,
-                                                              const double* __restrict__ cut, int cap, double* __restrict__ tail,
-                                                              int* __restrict__ count, double* __restrict__ partial) {
+// K_l2 and its LOO-PIT twin K_q1 (PIT = true), one body. Grid (chain groups, points). partial[point][3][gridDim.x]; tail[point][cap],
+// count[point] (zeroed by the caller). aux[point] is llmax for PSIS-LOO and the observation y for LOO-PIT. The three sums are
+//   PSIS-LOO: { sum exp(ll - llmax) over all draws, sum exp(lw), sum exp((lw + ll) - llmin) over the draws with lw <= cut }
+//   LOO-PIT : { sum exp(lw), sum exp(lw) [y_rep <= y], sum exp(lw) [y_rep == y] over the draws with lw <= cut }
+// The sum exp(lw) of both is accumulated by the same operations in the same order, so the two give it with the same bits. LOO-PIT
+// reads y_rep[rows][points][chains] beside ll and stores each tail draw's flags (kPitLe, kPitEq) in flags[point][cap] at its slot.
+template <bool PIT>
+__device__ __forceinline__ void loo_reduce_body(const double* __restrict__ x, const double* __restrict__ yrep, long long rows, int P, long long C,
+                                                const double* __restrict__ llmin, const double* __restrict__ aux, const double* __restrict__ cut,
+                                                int cap, double* __restrict__ tail, unsigned char* __restrict__ flags, int* __restrict__ count,
+                                                double* __restrict__ partial) {
   __shared__ double sh[256];
   const int p = blockIdx.y;
-  const double mn = llmin[p], mx = llmax[p], ct = cut[p];
+  const double mn = llmin[p], ax = aux[p], ct = cut[p];
   const size_t stride = (size_t)P * C;
-  double s_all = 0.0, s_w = 0.0, s_wl = 0.0;
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0;
   for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
     const double* q = x + (size_t)p * C + c;
     for (long long r = 0; r < rows; ++r) {
       const double v = q[r * stride];
-      s_all += exp(v - mx);
+      if (!PIT) s0 += exp(v - ax);
+      bool le = false, eq = false;
+      if (PIT) {
+        const double yr = yrep[(size_t)p * C + c + r * stride];
+        le = yr <= ax;
+        eq = yr == ax;
+      }
       const double lw = mn - v;                         // the reference's lw, in the same fp64 operation
       if (lw > ct) {
         const int slot = atomicAdd(&count[p], 1);
-        if (slot < cap) tail[(size_t)p * cap + slot] = v;
+        if (slot < cap) {
+          tail[(size_t)p * cap + slot] = v;
+          if (PIT) flags[(size_t)p * cap + slot] = (unsigned char)((le ? loo::kPitLe : 0) | (eq ? loo::kPitEq : 0));
+        }
+      } else if (PIT) {
+        const double w = exp(lw);
+        s0 += w;
+        s1 += le ? w : 0.0;
+        s2 += eq ? w : 0.0;
       } else {
-        s_w += exp(lw);
-        s_wl += exp((lw + v) - mn);
+        s1 += exp(lw);
+        s2 += exp((lw + v) - mn);
       }
     }
   }
-  const double a = cta_sum<256>(sh, s_all), b = cta_sum<256>(sh, s_w), d = cta_sum<256>(sh, s_wl);
+  const double a = cta_sum<256>(sh, s0), b = cta_sum<256>(sh, s1), d = cta_sum<256>(sh, s2);
   if (threadIdx.x == 0) {
     partial[((size_t)p * 3 + 0) * gridDim.x + blockIdx.x] = a;
     partial[((size_t)p * 3 + 1) * gridDim.x + blockIdx.x] = b;
@@ -100,31 +125,59 @@ __global__ void __launch_bounds__(256) amwg_loo_reduce_kernel(const double* __re
   }
 }
 
-// K_l3. One CTA per point. tails[shard][point][cap] with counts[shard][point]; work and xs: [point][cap] scratch, cap a power of two.
-// out[point][4] = { k (+inf for a tail of <= 4 draws or one where no candidate of the fit has a finite profile value, NaN for a
-// skipped point), sum exp(lw), sum exp(lw + ll - llmin) over the
-// tail with lw smoothed when k is finite, the number of tail draws over all shards }.
-__global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double* __restrict__ tails, const int* __restrict__ counts, int shards,
-                                                                   int P, int cap, const double* __restrict__ llmin, const double* __restrict__ cut,
-                                                                   const int* __restrict__ skip, double* __restrict__ work, double* __restrict__ xs,
-                                                                   double* __restrict__ out) {
+__global__ void __launch_bounds__(256) amwg_loo_reduce_kernel(const double* __restrict__ x, long long rows, int P, long long C,
+                                                              const double* __restrict__ llmin, const double* __restrict__ llmax,
+                                                              const double* __restrict__ cut, int cap, double* __restrict__ tail,
+                                                              int* __restrict__ count, double* __restrict__ partial) {
+  loo_reduce_body<false>(x, nullptr, rows, P, C, llmin, llmax, cut, cap, tail, nullptr, count, partial);
+}
+
+__global__ void __launch_bounds__(256) amwg_loo_pit_reduce_kernel(const double* __restrict__ x, const double* __restrict__ yrep, long long rows,
+                                                                  int P, long long C, const double* __restrict__ llmin,
+                                                                  const double* __restrict__ y, const double* __restrict__ cut, int cap,
+                                                                  double* __restrict__ tail, unsigned char* __restrict__ flags,
+                                                                  int* __restrict__ count, double* __restrict__ partial) {
+  loo_reduce_body<true>(x, yrep, rows, P, C, llmin, y, cut, cap, tail, flags, count, partial);
+}
+
+// K_l3 and its LOO-PIT twin K_q2 (PIT = true), one body. One CTA per point. tails[shard][point][cap] with counts[shard][point]
+// (and for LOO-PIT tflags[shard][point][cap]); work and xs: [point][cap] scratch, cap a power of two (and fwork [point][cap]).
+// PSIS-LOO: out[point][4] = { k (+inf for a tail of <= 4 draws or one where no candidate of the fit has a finite profile value, NaN
+// for a skipped point), sum exp(lw), sum exp(lw + ll - llmin) over the tail with lw smoothed when k is finite, the number of tail
+// draws over all shards }.
+// LOO-PIT: out[point][5] = { k, sum w, sum w [y_rep <= y], sum w [y_rep == y], the number of tail draws over all shards }, w the
+// weight exp(lw) (lw smoothed when k is finite). k and sum w are PSIS-LOO's, by the same code on the same sorted ll; the flag sums
+// give each draw of a run of tied ll the run's mean weight (loo::run_mean_sums), one thread per run.
+template <bool PIT>
+__device__ __forceinline__ void loo_fit_body(const double* __restrict__ tails, const unsigned char* __restrict__ tflags,
+                                             const int* __restrict__ counts, int shards, int P, int cap, const double* __restrict__ llmin,
+                                             const double* __restrict__ cut, const int* __restrict__ skip, double* __restrict__ work,
+                                             double* __restrict__ xs, unsigned char* __restrict__ fwork, double* __restrict__ out) {
+  constexpr int W = PIT ? 5 : 4;
   __shared__ double sh[kFitThreads];
   __shared__ double sb[loo::kMaxM], sL[loo::kMaxM], sw[loo::kMaxM];
   __shared__ double s_bp;
   const int p = blockIdx.x, t = threadIdx.x, T = blockDim.x;
   double* a = work + (size_t)p * cap;
   double* xp = xs + (size_t)p * cap;
+  unsigned char* fl = PIT ? fwork + (size_t)p * cap : nullptr;
   long long total = 0;
   for (int r = 0; r < shards; ++r) {
     const long long cnt = counts[(size_t)r * P + p];
     const long long have = cnt < cap ? cnt : cap;
     for (long long i = t; i < have; i += T)
-      if (total + i < cap) a[total + i] = tails[((size_t)r * P + p) * cap + i];
+      if (total + i < cap) {
+        a[total + i] = tails[((size_t)r * P + p) * cap + i];
+        if (PIT) fl[total + i] = tflags[((size_t)r * P + p) * cap + i];
+      }
     total += cnt;
   }
   const int n = (int)(total < cap ? total : cap);
   if (skip[p]) {
-    if (t == 0) { out[4 * p] = CUDART_NAN; out[4 * p + 1] = CUDART_NAN; out[4 * p + 2] = CUDART_NAN; out[4 * p + 3] = (double)total; }
+    if (t == 0) {
+      for (int j = 0; j < W - 1; ++j) out[W * p + j] = CUDART_NAN;
+      out[W * p + W - 1] = (double)total;
+    }
     return;
   }
   for (int i = n + t; i < cap; i += T) a[i] = -CUDART_INF;
@@ -135,7 +188,10 @@ __global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double*
         const int l = i ^ j;
         if (l > i) {
           const double ai = a[i], al = a[l];
-          if ((i & k) == 0 ? (ai < al) : (ai > al)) { a[i] = al; a[l] = ai; }
+          if ((i & k) == 0 ? (ai < al) : (ai > al)) {
+            a[i] = al; a[l] = ai;
+            if (PIT) { const unsigned char fi = fl[i]; fl[i] = fl[l]; fl[l] = fi; }
+          }
         }
       }
       __syncthreads();
@@ -175,10 +231,43 @@ __global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double*
   for (int i = t; i < n; i += T) {
     const double lw = smooth ? loo::smoothed(i, n, k, sigma, expcut) : mn - a[i];
     s_w += exp(lw);
-    s_wl += exp((lw + a[i]) - mn);
+    if (PIT) xp[i] = exp(lw);                                 // the fit is done with xp (every read of it is behind a barrier)
+    else s_wl += exp((lw + a[i]) - mn);
   }
-  const double tw = cta_sum<kFitThreads>(sh, s_w), twl = cta_sum<kFitThreads>(sh, s_wl);
-  if (t == 0) { out[4 * p] = k; out[4 * p + 1] = tw; out[4 * p + 2] = twl; out[4 * p + 3] = (double)total; }
+  const double tw = cta_sum<kFitThreads>(sh, s_w);           // its barrier also publishes the weights in xp
+  if (PIT) {
+    double s_le = 0.0, s_eq = 0.0;
+    for (int i = t; i < n; i += T) {
+      if (i > 0 && a[i] == a[i - 1]) continue;                // not the first rank of its run
+      int e = i + 1;
+      while (e < n && a[e] == a[i]) ++e;
+      double le, eq;
+      loo::run_mean_sums(xp + i, fl + i, e - i, &le, &eq);
+      s_le += le;
+      s_eq += eq;
+    }
+    const double tle = cta_sum<kFitThreads>(sh, s_le), teq = cta_sum<kFitThreads>(sh, s_eq);
+    if (t == 0) { out[5 * p] = k; out[5 * p + 1] = tw; out[5 * p + 2] = tle; out[5 * p + 3] = teq; out[5 * p + 4] = (double)total; }
+  } else {
+    const double twl = cta_sum<kFitThreads>(sh, s_wl);
+    if (t == 0) { out[4 * p] = k; out[4 * p + 1] = tw; out[4 * p + 2] = twl; out[4 * p + 3] = (double)total; }
+  }
+}
+
+__global__ void __launch_bounds__(kFitThreads) amwg_loo_fit_kernel(const double* __restrict__ tails, const int* __restrict__ counts, int shards,
+                                                                   int P, int cap, const double* __restrict__ llmin, const double* __restrict__ cut,
+                                                                   const int* __restrict__ skip, double* __restrict__ work, double* __restrict__ xs,
+                                                                   double* __restrict__ out) {
+  loo_fit_body<false>(tails, nullptr, counts, shards, P, cap, llmin, cut, skip, work, xs, nullptr, out);
+}
+
+__global__ void __launch_bounds__(kFitThreads) amwg_loo_pit_fit_kernel(const double* __restrict__ tails, const unsigned char* __restrict__ tflags,
+                                                                       const int* __restrict__ counts, int shards, int P, int cap,
+                                                                       const double* __restrict__ llmin, const double* __restrict__ cut,
+                                                                       const int* __restrict__ skip, double* __restrict__ work,
+                                                                       double* __restrict__ xs, unsigned char* __restrict__ fwork,
+                                                                       double* __restrict__ out) {
+  loo_fit_body<true>(tails, tflags, counts, shards, P, cap, llmin, cut, skip, work, xs, fwork, out);
 }
 
 }  // namespace summary
@@ -361,5 +450,63 @@ extern "C" int amwg_loo_fit(int device, const double* dev_tails, const int32_t* 
                                                                           d_work, d_xs, d_out);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaMemcpy(host_out, d_out, (size_t)points * 4 * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// LOO-PIT (sample_summary(..., ppc={..., "loo_pit": ...}), DESIGN.md §4.9): the reduce and the fit of PSIS-LOO with the flags of
+// each draw's y_rep against the observation carried alongside (K_q1, K_q2 above).
+extern "C" int amwg_loo_pit_reduce(int device, const double* dev_ll, const double* dev_yrep, int64_t rows, int32_t points, int64_t chains,
+                                   const double* host_llmin, const double* host_cut, const double* host_y, int32_t tail_cap, double* dev_tail,
+                                   uint8_t* dev_tail_flags, int32_t* dev_count, double* host_sums) {
+  if (rows <= 0 || points <= 0 || chains <= 0) return fail("amwg_loo_pit_reduce: empty block");
+  if (points > 65535) return fail("amwg_loo_pit_reduce: at most 65535 points per call");
+  if (tail_cap < 1 || tail_cap > loo::kMaxTail) return fail("amwg_loo_pit_reduce: tail_cap must be 1.." + std::to_string(loo::kMaxTail));
+  if (!dev_ll || !dev_yrep || !host_llmin || !host_cut || !host_y || !dev_tail || !dev_tail_flags || !dev_count || !host_sums)
+    return fail("amwg_loo_pit_reduce: null pointer");
+  if (summary::select_device(device, "amwg_loo_pit_reduce")) return -1;
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
+  const size_t b_vec = (size_t)points * 8;
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_loo_pit_reduce", {b_vec, b_vec, b_vec, (size_t)points * 3 * bx * 8, (size_t)points * 3 * 8})) return -1;
+  double* d_min = sc.part<double>(0);
+  double* d_y = sc.part<double>(1);
+  double* d_cut = sc.part<double>(2);
+  double* d_part = sc.part<double>(3);
+  double* d_sums = sc.part<double>(4);
+  CUDA_TRY(cudaMemcpy(d_min, host_llmin, (size_t)points * 8, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_y, host_y, (size_t)points * 8, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_cut, host_cut, (size_t)points * 8, cudaMemcpyHostToDevice));
+  summary::amwg_loo_pit_reduce_kernel<<<dim3(bx, (unsigned)points), 256>>>(dev_ll, dev_yrep, rows, points, chains, d_min, d_y, d_cut, tail_cap,
+                                                                           dev_tail, dev_tail_flags, dev_count, d_part);
+  summary::amwg_merge_sums_kernel<<<(unsigned)points * 3, 256>>>(d_part, (int)bx, d_sums);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpy(host_sums, d_sums, (size_t)points * 3 * 8, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int amwg_loo_pit_fit(int device, const double* dev_tails, const uint8_t* dev_flags, const int32_t* dev_counts, int32_t shards,
+                                int32_t points, int32_t tail_cap, const double* host_llmin, const double* host_cut, const int32_t* host_skip,
+                                double* host_out) {
+  if (shards < 1 || points < 1) return fail("amwg_loo_pit_fit: shards and points must be >= 1");
+  if (tail_cap < 8 || tail_cap > loo::kMaxTail || (tail_cap & (tail_cap - 1))) return fail("amwg_loo_pit_fit: tail_cap must be a power of two in 8.." + std::to_string(loo::kMaxTail));
+  if (!dev_tails || !dev_flags || !dev_counts || !host_llmin || !host_cut || !host_skip || !host_out) return fail("amwg_loo_pit_fit: null pointer");
+  if (summary::select_device(device, "amwg_loo_pit_fit")) return -1;
+  const size_t b_vec = (size_t)points * 8, b_work = (size_t)points * tail_cap * 8;
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_loo_pit_fit", {b_vec, b_vec, b_vec, b_work, b_work, (size_t)points * tail_cap, (size_t)points * 5 * 8})) return -1;
+  double* d_min = sc.part<double>(0);
+  double* d_cut = sc.part<double>(1);
+  int* d_skip = sc.part<int>(2);
+  double* d_work = sc.part<double>(3);
+  double* d_xs = sc.part<double>(4);
+  unsigned char* d_fwork = sc.part<unsigned char>(5);
+  double* d_out = sc.part<double>(6);
+  CUDA_TRY(cudaMemcpy(d_min, host_llmin, (size_t)points * 8, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_cut, host_cut, (size_t)points * 8, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(d_skip, host_skip, (size_t)points * 4, cudaMemcpyHostToDevice));
+  summary::amwg_loo_pit_fit_kernel<<<(unsigned)points, summary::kFitThreads>>>(dev_tails, dev_flags, dev_counts, shards, points, tail_cap, d_min,
+                                                                              d_cut, d_skip, d_work, d_xs, d_fwork, d_out);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpy(host_out, d_out, (size_t)points * 5 * 8, cudaMemcpyDeviceToHost));
   return 0;
 }

@@ -788,12 +788,31 @@ class AmwgSampler(Sampler):
         The points run in chunks sized to the free device memory. Every other key keeps its bits. A refused ppc (not a dict,
         unknown keys, points not an int >= 1, anything loo refuses in f, a value that is not one ld.* call with data[i] first, a
         family without a sampler, kept rows x points >= 2^46, or a monitored name "ppc") raises ValueError before the chains move
-        (summary.resolve_ppc, summary.check_ppc_call, tracer.LogLik.observed_call)."""
+        (summary.resolve_ppc, summary.check_ppc_call, tracer.LogLik.observed_call).
+        ppc={..., "loo_pit": True} (or {"r_eff": r}, r a finite float > 0; True means r = 1.0, as in loo=) adds "loo_pit" to the
+        "ppc" dict: the PIT of each observation under its leave-one-out predictive (LOO-PIT; Gabry et al. 2019, Säilynoja, Bürkner &
+        Vehtari 2022; ArviZ's loo_pit), which the in-sample "pit" cannot give: there y_i shapes the posterior that predicts it. It
+        holds {"pit", "pit_equal", "pareto_k" (float64 [N] each), "pareto_k_threshold", "n_high_k", "r_eff"}. The log-likelihood is
+        ppc's own f, the ld.* call y_rep is drawn from, evaluated on the device as loo= evaluates its body (loo= is not needed).
+        Definition, per point i over the S draws: ll_s, lw_s = llmin - ll_s, M, cut, the tail T = {s : lw_s > cut}, k^, sigma^ and
+        the smoothed weights are those of loo= (DESIGN.md §4.7). The tail sorted by ascending lw has ranks j = 0..n-1; its smoothed
+        weight is w'_j = exp(min(0, log(gpinv((j + 0.5)/n; k^, sigma^) + exp(cut)))) when k^ is finite, and exp(lw) otherwise.
+        Ties: the sorted tail splits into maximal runs of equal ll, and every draw of run R gets the run's mean weight
+        (sum_{j in R} w'_j) / |R|; a draw outside the tail gets exp(lw_s). D is the sum of all weights (elpd_loo's normaliser: a run's
+        mean keeps its total), LE the sum of the weights of draws with y_rep_s <= y_i and EQ of those with y_rep_s == y_i (a NaN
+        y_rep counts in D only); pit_i = min(1, LE / D) and pit_equal_i = min(1, EQ / D), so pit - U pit_equal (U uniform) is the
+        randomised PIT of a count family. pareto_k is loo='s k^ (+inf for a tail of <= 4 draws or when no candidate of the fit
+        has a finite profile value); the threshold and n_high_k are loo='s. A point with any non-finite ll gets NaN in pit,
+        pit_equal and pareto_k. Without ties this is ArviZ's min(1, exp(logsumexp(lw_norm[y_rep <= y]))); the run means make it
+        independent of the order of tied draws (a rejected step repeats its ll), and so of sharding, chunking and the sort. See
+        summary.loo_pit_chunk. Every other key, and the chains' state, keep their bits. A refused loo_pit (anything but True or
+        {"r_eff": ...}, an r_eff not finite and > 0, fewer than 2 draws, a tail of more than 2^20 draws) raises ValueError before
+        the chains move."""
         import torch
         from .summary import (CudaBlockReducer, CudaPointwise, CudaPpc, check_diagnostics, check_loo_size, check_ppc_call, comoments_scratch_bytes,
-                              covariance_block, entry_spans, histogram_block, loo_block, loo_point_bytes, loo_tail_cap, nested_block,
-                              nested_scratch_bytes, ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance, resolve_histogram, resolve_loo,
-                              resolve_nested, resolve_ppc, summarise_block)
+                              covariance_block, entry_spans, histogram_block, loo_block, loo_pit_point_bytes, loo_point_bytes, loo_tail_cap,
+                              nested_block, nested_scratch_bytes, ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance,
+                              resolve_histogram, resolve_loo, resolve_nested, resolve_ppc, summarise_block)
         check_diagnostics(diagnostics)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries = [i for name in monitored for i in self._entries(name)]
@@ -829,6 +848,8 @@ class AmwgSampler(Sampler):
             lik = trace_log_lik(loo_plan.log_lik, self.params, self._offsets, self.data, loo_plan.points)
         if ppc_plan is not None:
             from .tracer import trace_log_lik
+            if ppc_plan.loo_pit is not None:
+                pit_m = check_loo_size(rows * self.n_chains, ppc_plan.loo_pit, "ppc loo_pit")
             ppc_lik = trace_log_lik(ppc_plan.log_lik, self.params, self._offsets, self.data, ppc_plan.points, what="ppc")
             ppc_family, ppc_y, ppc_args = ppc_lik.observed_call(ppc_plan.points)
             ppc_code = check_ppc_call(ppc_family, rows, ppc_plan.points)
@@ -838,6 +859,8 @@ class AmwgSampler(Sampler):
         if ppc_plan is not None:
             block_entries(ppc_lik.reads)
             ppc_prog, ppc_offs = ppc_lik.lower_exprs(ppc_args, start)
+            if ppc_plan.loo_pit is not None:
+                pit_prog = ppc_lik.lower(start)                   # the log-likelihood of the same ld.* call, as loo= lowers its body
         L = _ffi.lib()
         dev = torch.device("cuda", self.device)
         need = rows * len(sampled) * self.local_chains * 8
@@ -877,12 +900,15 @@ class AmwgSampler(Sampler):
                 torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MIN)
                 chunk_points = int(t.item())
             return chunk_points
+        world = torch.distributed.get_world_size() if self.distributed else 1
         if loo_plan is not None:
-            world = torch.distributed.get_world_size() if self.distributed else 1
             chunk_points = chunk_size(loo_point_bytes(rows, self.local_chains, loo_tail_cap(loo_m), world), loo_plan.points,
                                       "pointwise log-likelihood")
         if ppc_plan is not None:
-            ppc_chunk = chunk_size(ppc_point_bytes(rows, self.local_chains), ppc_plan.points, "replicated data")
+            per_point = ppc_point_bytes(rows, self.local_chains)
+            if ppc_plan.loo_pit is not None:                      # LOO-PIT holds a chunk of ll beside the chunk of y_rep
+                per_point += loo_pit_point_bytes(rows, self.local_chains, loo_tail_cap(pit_m), world)
+            ppc_chunk = chunk_size(per_point, ppc_plan.points, "replicated data")
         block = torch.empty((rows, len(sampled), self.local_chains), dtype=torch.float64, device=dev)
         mon = np.asarray(sampled, dtype=np.int32)
         torch.cuda.current_stream(dev).synchronize()   # the library writes `block` on its own stream: torch's queued work goes first
@@ -896,8 +922,11 @@ class AmwgSampler(Sampler):
                                 loo_plan.r_eff, chunk_points, self.distributed)
         ppc_out = None
         if ppc_plan is not None:
+            pit = None
+            if ppc_plan.loo_pit is not None:
+                pit = (CudaPointwise(self._handle, pit_prog, block, self.device), ppc_plan.loo_pit)
             ppc_out = ppc_block(reducer, CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points), rows, self.n_chains,
-                                ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed)
+                                ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed, loo_pit=pit)
         if len(sampled) > len(entries):
             block = block[:, :len(entries)].contiguous()
         res = summarise_block(reducer, block, rows, self.n_chains, probs, self.distributed, diagnostics)

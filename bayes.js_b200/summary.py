@@ -338,6 +338,33 @@ class CudaBlockReducer:
                    sk.ctypes.data, out.ctypes.data)
         return out
 
+    def loo_pit_reduce(self, ll, yrep, llmin, cut, y, cap: int):
+        """-> (sums [P, 3], tails float64 tensor [P, cap], flags uint8 tensor [P, cap], counts int32 tensor [P]) of this shard; see
+        amwg_loo_pit_reduce in include/amwg.h."""
+        import torch
+        rows, P, chains = ll.shape
+        assert tuple(yrep.shape) == tuple(ll.shape)
+        tails = torch.empty((P, cap), dtype=torch.float64, device=ll.device)
+        flags = torch.empty((P, cap), dtype=torch.uint8, device=ll.device)
+        counts = torch.zeros(P, dtype=torch.int32, device=ll.device)
+        sums = np.empty((P, 3), dtype=np.float64)
+        f = lambda a: np.ascontiguousarray(a, dtype=np.float64)
+        mn, ct, yy = f(llmin), f(cut), f(y)
+        self._call(ll, self.L.amwg_loo_pit_reduce, ll.data_ptr(), yrep.data_ptr(), rows, P, chains, mn.ctypes.data, ct.ctypes.data,
+                   yy.ctypes.data, cap, tails.data_ptr(), flags.data_ptr(), counts.data_ptr(), sums.ctypes.data)
+        return sums, tails, flags, counts
+
+    def loo_pit_fit(self, tails, flags, counts, llmin, cut, skip) -> np.ndarray:
+        """tails [shards, P, cap], flags uint8 [shards, P, cap], counts int32 [shards, P] (device) -> [P, 5]; see amwg_loo_pit_fit in
+        include/amwg.h."""
+        shards, P, cap = tails.shape
+        out = np.empty((P, 5), dtype=np.float64)
+        mn, ct = np.ascontiguousarray(llmin, dtype=np.float64), np.ascontiguousarray(cut, dtype=np.float64)
+        sk = np.ascontiguousarray(skip, dtype=np.int32)
+        self._call(tails, self.L.amwg_loo_pit_fit, tails.data_ptr(), flags.data_ptr(), counts.data_ptr(), shards, P, cap, mn.ctypes.data,
+                   ct.ctypes.data, sk.ctypes.data, out.ctypes.data)
+        return out
+
 
 # ---------------------------------------------------------------------------------------------------------------------
 # split-chain effective sample size (Vehtari et al. 2021, §3; Stan's `ess` on split chains, ArviZ's method="mean"/"tail")
@@ -1122,14 +1149,28 @@ def loo_point_bytes(rows: int, chains: int, cap: int, world: int) -> int:
     return 8 * rows * chains + tails + 16 * cap + 56 + (32 * G + 32) + (24 * G + 48) + (8 + 8 * 256) + 80
 
 
-def check_loo_size(S: int, r_eff: float) -> int:
-    """-> M, or ValueError when S < 2 or the tail exceeds what the fit kernel holds."""
+def check_loo_size(S: int, r_eff: float, what: str = "loo") -> int:
+    """-> M, or ValueError when S < 2 or the tail exceeds what the fit kernel holds. `what` names the option in the message."""
     if S < 2:
-        raise ValueError("loo needs at least 2 draws (kept rows x chains), not %d" % S)
+        raise ValueError("%s needs at least 2 draws (kept rows x chains), not %d" % (what, S))
     M = loo_tail_length(S, r_eff)
     if M > MAX_LOO_TAIL:
-        raise ValueError("loo: a Pareto tail of %d draws per point (S = %d, r_eff = %g) exceeds %d" % (M, S, r_eff, MAX_LOO_TAIL))
+        raise ValueError("%s: a Pareto tail of %d draws per point (S = %d, r_eff = %g) exceeds %d" % (what, M, S, r_eff, MAX_LOO_TAIL))
     return M
+
+
+def loo_cut(reducer, ll, M: int, distributed: bool):
+    """The steps of PSIS-LOO before the tail pass, over a chunk ll [rows, P, chains] of every shard: -> (llmin, llmax, skip, cut),
+    [P] each. llmin / llmax: the smallest / largest finite ll (merged_extremes over the shards' finite ranges); skip: the points
+    with a non-finite ll (sum_counts of the non-finite counts); cut = max(llmin - (the M-th smallest ll, 0-based, by the radix
+    select), log(DBL_MIN)), so the tail holds the draws with lw = llmin - ll > cut."""
+    rng, nonfinite = reducer.finite_range(ll)
+    llmin, llmax = merged_extremes(rng.cpu().numpy(), ll, distributed).T
+    skip = sum_counts(nonfinite, distributed).cpu().numpy().sum(axis=1) > 0
+    llM = _select(reducer, ll, np.array([M], dtype=np.int64), distributed).values()[:, 0]
+    with np.errstate(invalid="ignore"):
+        cut = np.maximum(llmin - llM, LOG_TINY)
+    return llmin, llmax, skip, cut
 
 
 def _program_arrays(prog):
@@ -1192,14 +1233,9 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
     for p0 in range(0, points, chunk_points):
         P = min(chunk_points, points - p0)
         ll = source.chunk(p0, P)
-        rng, nonfinite = reducer.finite_range(ll)
-        llmin, llmax = merged_extremes(rng.cpu().numpy(), ll, distributed).T
-        skip = sum_counts(nonfinite, distributed).cpu().numpy().sum(axis=1) > 0
+        llmin, llmax, skip, cut = loo_cut(reducer, ll, M, distributed)
         rec = pooled_moment_record(reducer, ll, distributed)
         var = (rec[:, 3] + rows * rec[:, 2]) / S
-        llM = _select(reducer, ll, np.array([M], dtype=np.int64), distributed).values()[:, 0]
-        with np.errstate(invalid="ignore"):
-            cut = np.maximum(llmin - llM, LOG_TINY)
         # a point with a non-finite ll is NaN throughout: keep its draws out of the tail
         mn, mx, ct = np.where(skip, 0.0, llmin), np.where(skip, 0.0, llmax), np.where(skip, np.inf, cut)
         sums, tails, counts = reducer.loo_reduce(ll, mn, mx, ct, cap)
@@ -1233,7 +1269,7 @@ def loo_block(reducer, source, rows: int, total_chains: int, points: int, r_eff:
 
 # ---------------------------------------------------------------------------------------------------------------------
 # posterior predictive checks (BDA3 ch. 6; ArviZ's plot_ppc / plot_bpv): DESIGN.md §4.8
-PPC_KEYS = ("log_lik", "points")
+PPC_KEYS = ("log_lik", "points", "loo_pit")
 # the families with a sampler, in the order of the family codes of csrc/amwg_ppc.cuh (amwg_ppc_pointwise)
 PPC_FAMILIES = ("norm", "lnorm", "cauchy", "laplace", "logis", "exp", "weibull", "pareto", "unif", "gamma", "invgamma", "beta", "t",
                 "bern", "pois", "binom", "nbinom")
@@ -1242,20 +1278,33 @@ MAX_PPC_DRAWS = 1 << 46                # rows x points: the stream region of amw
 
 
 class PpcPlan(NamedTuple):
-    """A checked `ppc=` argument."""
+    """A checked `ppc=` argument; loo_pit is the r_eff of LOO-PIT, None without it."""
     log_lik: object
     points: int
+    loo_pit: Optional[float] = None
 
 
 def resolve_ppc(spec, names: Sequence[str]) -> Optional[PpcPlan]:
-    """Checks the `ppc=` argument of sample_summary: None, or {"log_lik": callable (state, data, i), "points": int >= 1}, with no
-    monitored name "ppc" (the key the result uses). Pure: raises ValueError before any device work (tracing log_lik and
-    check_ppc_call are the caller's next checks)."""
+    """Checks the `ppc=` argument of sample_summary: None, or {"log_lik": callable (state, data, i), "points": int >= 1, optional
+    "loo_pit": True (r_eff = 1.0) or {"r_eff": finite float > 0}}, with no monitored name "ppc" (the key the result uses). Pure:
+    raises ValueError before any device work (tracing log_lik and check_ppc_call are the caller's next checks)."""
     if spec is None:
         return None
     log_lik, points = _log_lik_spec(spec, "ppc", PPC_KEYS, "one ld.* call at data point i")
+    r_eff = None
+    if "loo_pit" in spec:
+        pit = spec["loo_pit"]
+        if pit is True:
+            r_eff = 1.0
+        elif isinstance(pit, dict) and list(pit) == ["r_eff"]:
+            r_eff = pit["r_eff"]
+            if not (isinstance(r_eff, numbers.Real) and not isinstance(r_eff, bool) and np.isfinite(r_eff) and r_eff > 0):
+                raise ValueError("ppc loo_pit r_eff must be a finite number > 0, not %r" % (r_eff,))
+            r_eff = float(r_eff)
+        else:
+            raise ValueError("ppc loo_pit must be True or {\"r_eff\": a finite number > 0}, not %r" % (pit,))
     _check_result_key("ppc", names)
-    return PpcPlan(log_lik, points)
+    return PpcPlan(log_lik, points, r_eff)
 
 
 def check_ppc_call(family: str, rows: int, points: int) -> int:
@@ -1293,6 +1342,17 @@ def ppc_point_bytes(rows: int, chains: int) -> int:
     amwg_summary_threshold_counts (8 + 32)."""
     G = min(-(-chains // 256), 1184)
     return 8 * rows * chains + (32 * G + 32) + 40
+
+
+def loo_pit_point_bytes(rows: int, chains: int, cap: int, world: int) -> int:
+    """Device bytes one point of a chunk takes for LOO-PIT on top of ppc_point_bytes, from the sizes the calls allocate
+    (include/amwg.h): its ll column of the chunk; its tail buffer, flags and count (this rank's, and with world > 1 every rank's
+    gathered); the fit's sort, value and flag scratch (17 cap) and its llmin / cut / skip / out (64); the llmin / cut / y and the
+    sums of amwg_loo_pit_reduce (24 G + 48), G = min(ceil(chains / 256), 1184) CTAs; the select's prefix and digit counts
+    (8 + 8 x 256); the finite range and non-finite counts (16 + 24 + 16 + 24: the device keys and the returned tensors)."""
+    G = min(-(-chains // 256), 1184)
+    tails = (9 * cap + 4) * (1 + (world if world > 1 else 0))
+    return 8 * rows * chains + tails + 17 * cap + 64 + (24 * G + 48) + (8 + 8 * 256) + 80
 
 
 def ppc_fixed_bytes(rows: int, chains: int) -> int:
@@ -1335,7 +1395,7 @@ class CudaPpc:
 
 
 def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family: str, y, probs: Sequence[float], chunk_points: int,
-              distributed: bool) -> dict:
+              distributed: bool, loo_pit=None) -> dict:
     """-> the "ppc" dict of sample_summary over all shards, for the S = rows x total_chains kept draws. `source.chunk(p0, P)` gives
     y_rep of points p0 .. p0 + P - 1 as a [rows, P, chains] block (this shard's chains; chunks of at most `chunk_points`, in
     order), and `source.stats()` after the last chunk the [rows, 4, chains] block of each draw's T(y_rep) = (mean, sd, min,
@@ -1346,17 +1406,26 @@ def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family
     "n_greater", "n_equal", "n_nan" and "p_value" = (n_greater + n_equal) / S, Pr(T(y_rep) >= T(y)) with a NaN draw counted as
     not >= (and with T(y) NaN, no draw is). Distributed: the moment records merge by pooled_moment_record, the threshold counts
     (int64 [entries, 4]: <, ==, >, NaN) add up by sum_counts, and summarise_block takes its distributed path; every rank returns
-    the same numbers."""
+    the same numbers.
+    loo_pit = (ll_source, r_eff) adds "loo_pit" (loo_pit_chunk): ll_source.chunk(p0, P) gives the log-likelihood of the same ld.*
+    call as a [rows, P, chains] block, taken while that chunk's y_rep is resident."""
     S = rows * total_chains
     y = np.ascontiguousarray(y, dtype=np.float64)
     pw = {"mean": np.empty(points), "sd": np.empty(points)}
     cnt = np.empty((points, 4), dtype=np.int64)
+    if loo_pit is not None:
+        ll_source, r_eff = loo_pit
+        M = check_loo_size(S, r_eff, "ppc loo_pit")
+        pit = {k: np.full(points, np.nan) for k in ("pit", "pit_equal", "pareto_k")}
     for p0 in range(0, points, chunk_points):
         P = min(chunk_points, points - p0)
         yrep = source.chunk(p0, P)
         sl = slice(p0, p0 + P)
         pw["mean"][sl], pw["sd"][sl], _rhat = finalize_moments(pooled_moment_record(reducer, yrep, distributed), rows)
         cnt[sl] = sum_counts(reducer.threshold_counts(yrep, y[sl]), distributed).cpu().numpy()
+        if loo_pit is not None:
+            pit["pit"][sl], pit["pit_equal"][sl], pit["pareto_k"][sl] = loo_pit_chunk(reducer, ll_source.chunk(p0, P), yrep, y[sl], M,
+                                                                                     distributed)
         del yrep
     pw.update(n_below=cnt[:, 0], n_equal=cnt[:, 1], pit=(cnt[:, 0] + cnt[:, 1]) / S, n_nan=cnt[:, 3])
     T = source.stats()
@@ -1368,4 +1437,43 @@ def ppc_block(reducer, source, rows: int, total_chains: int, points: int, family
         stats[name] = {"observed": float(obs[k]), "mean": float(mean[k]), "sd": float(sd[k]), "quantiles": q[:, k].copy(),
                        "n_greater": int(tc[k, 2]), "n_equal": int(tc[k, 1]), "n_nan": int(tc[k, 3]),
                        "p_value": float((tc[k, 2] + tc[k, 1]) / S)}
-    return {"family": family, "points": int(points), "n_draws": int(S), "pointwise": pw, "stats": stats}
+    out = {"family": family, "points": int(points), "n_draws": int(S), "pointwise": pw, "stats": stats}
+    if loo_pit is not None:
+        thr = min(1.0 - 1.0 / np.log10(S), 0.7)
+        with np.errstate(invalid="ignore"):
+            n_high = int(np.sum(pit["pareto_k"] > thr))
+        pit.update(pareto_k_threshold=float(thr), n_high_k=n_high, r_eff=float(r_eff))
+        out["loo_pit"] = pit
+    return out
+
+
+def loo_pit_chunk(reducer, ll, yrep, y, M: int, distributed: bool):
+    """LOO-PIT of one chunk of points (DESIGN.md §4.9): ll and yrep [rows, P, chains] of this shard, y [P] the observations, M the
+    tail length of every shard's S draws. -> (pit, pit_equal, pareto_k), [P] each. The steps of PSIS-LOO (loo_cut) give llmin, cut
+    and the points with a non-finite ll; one pass (reducer.loo_pit_reduce) sums the weights exp(lw) of the draws outside the tail,
+    in all and where y_rep <= y and y_rep == y, and collects the tail's ll with those two flags; the fit over the merged tail
+    (reducer.loo_pit_fit) gives k, the tail's weights and their flag sums, each draw of a run of tied ll weighted by the run's mean
+    weight. With D, LE and EQ the three sums over all draws: pit = min(1, LE / D), pit_equal = min(1, EQ / D); a point with a
+    non-finite ll gets NaN in all three. Distributed: loo_cut's steps, the sums gathered and added in rank order, and the tails,
+    flags and counts gathered (gather_tensor), so every rank returns the same numbers."""
+    llmin, _llmax, skip, cut = loo_cut(reducer, ll, M, distributed)
+    mn, ct = np.where(skip, 0.0, llmin), np.where(skip, np.inf, cut)
+    sums, tails, flags, counts = reducer.loo_pit_reduce(ll, yrep, mn, ct, y, loo_tail_cap(M))
+    del ll
+    parts = gather(sums, tails, distributed)
+    sums = parts[0]
+    for q in parts[1:]:
+        sums = sums + q
+    fit = reducer.loo_pit_fit(gather_tensor(tails, distributed), gather_tensor(flags, distributed), gather_tensor(counts, distributed), mn,
+                              ct, skip.astype(np.int32))
+    del tails, flags, counts
+    if np.any(fit[~skip, 4] > M):
+        raise RuntimeError("ppc loo_pit: a point's tail holds more than M = %d draws (inconsistent select)" % M)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        D = sums[:, 0] + fit[:, 1]
+        pit = np.minimum(1.0, (sums[:, 1] + fit[:, 2]) / D)
+        pit_equal = np.minimum(1.0, (sums[:, 2] + fit[:, 3]) / D)
+    k = fit[:, 0].copy()
+    for v in (pit, pit_equal, k):
+        v[skip] = np.nan
+    return pit, pit_equal, k

@@ -303,7 +303,7 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  * The reference returns raw draws only (mcmc.js:1029; README.md:44-52 leaves the summary to the caller). With millions of
  * chains the summary is formed where the draws are. Both calls read a DEVICE-resident sample block in amwg_sample_device's
  * layout, x[row][entry][chain]; neither needs a sampler handle (they are reductions over the block).
- * The summary pool: every amwg_summary_*, amwg_loo_* and amwg_ppc_pointwise call takes its device scratch from one pool per
+ * The summary pool: every amwg_summary_*, amwg_loo_* (amwg_loo_pit_* included) and amwg_ppc_pointwise call takes its device scratch from one pool per
  * device, grown on demand, never shrunk, and held (locked) by the call until it returns. A device index outside 0..63 is refused
  * with "<call>: device index out of range".
  *
@@ -442,6 +442,30 @@ AMWG_API int amwg_loo_reduce(int device, const double* dev_ll, int64_t rows, int
                              double* host_sums);
 AMWG_API int amwg_loo_fit(int device, const double* dev_tails, const int32_t* dev_counts, int32_t shards, int32_t points, int32_t tail_cap,
                           const double* host_llmin, const double* host_cut, const int32_t* host_skip, double* host_out);
+
+/* ---- LOO-PIT (sample_summary(..., ppc={..., "loo_pit": ...}), DESIGN.md §4.9) -------------------------------------------------
+ * The probability integral transform of each observation under its leave-one-out predictive, from the PSIS-LOO weights of
+ * amwg_loo_reduce / amwg_loo_fit and the replicated data of amwg_ppc_pointwise.
+ * amwg_loo_pit_reduce: over a chunk dev_ll[rows][points][chains] and the matching dev_yrep[rows][points][chains] (the same points),
+ *   with the host's llmin, cut and observations y per point: host_sums[point][3] = { sum exp(lw), sum exp(lw) [y_rep <= y],
+ *   sum exp(lw) [y_rep == y] } over the draws with lw = llmin - ll <= cut (a NaN y_rep counts in the first sum only), each formed
+ *   in a fixed order; the first has the bits of amwg_loo_reduce's second sum for the same chunk. Every draw with lw > cut has its
+ *   ll appended to dev_tail[point][tail_cap] at slot dev_count[point]++ (int32, zeroed by the caller; slots past tail_cap are
+ *   counted, not written) and its flags (1: y_rep <= y, 2: y_rep == y) at the same slot of dev_tail_flags[point][tail_cap].
+ *   Errors: an empty block, points > 65535, tail_cap outside 1..2^20, null pointers.
+ * amwg_loo_pit_fit: amwg_loo_fit over the same tails, with the flags dev_flags[shard][point][tail_cap] sorted along with the ll.
+ *   host_out[point][5] = { k, sum w, sum w [y_rep <= y], sum w [y_rep == y], the tail draws over all shards }, w the weight
+ *   exp(lw) of a tail draw (the smoothed weight of its rank when k is finite); k and sum w have amwg_loo_fit's bits. In the two flag
+ *   sums every draw of a run of equal ll takes the run's mean weight, so they do not depend on the order of tied draws (nor on
+ *   sharding or the sort). host_skip[point] != 0 gives NaN in the first four. Deterministic. Errors: as amwg_loo_fit.
+ * Device scratch of the two calls (the summary pool): 3 x 8 points + 24 points G bytes (reduce, G = min(ceil(chains / 256),
+ *   1184)), 3 x 8 points + 17 points tail_cap + 40 points bytes (fit), each part rounded up to 256 bytes. */
+AMWG_API int amwg_loo_pit_reduce(int device, const double* dev_ll, const double* dev_yrep, int64_t rows, int32_t points, int64_t chains,
+                                 const double* host_llmin, const double* host_cut, const double* host_y, int32_t tail_cap, double* dev_tail,
+                                 uint8_t* dev_tail_flags, int32_t* dev_count, double* host_sums);
+AMWG_API int amwg_loo_pit_fit(int device, const double* dev_tails, const uint8_t* dev_flags, const int32_t* dev_counts, int32_t shards,
+                              int32_t points, int32_t tail_cap, const double* host_llmin, const double* host_cut, const int32_t* host_skip,
+                              double* host_out);
 
 /* ---- posterior predictive checks (sample_summary(..., ppc=...), DESIGN.md §4.8) -----------------------------------------------
  * amwg_ppc_pointwise: dev_out[row][p][chain] = a replicated observation y_rep of point p0 + p (p < n_points, of `points` points in

@@ -571,6 +571,36 @@ BINDING(loo_fit)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// loo_pit_reduce(device, ll ptr, yrep ptr, rows, points, chains, llmin [points], cut [points], y [points], tail_cap, tail ptr,
+//                flags ptr, count ptr) -> Float64Array [points][3]                                            amwg_loo_pit_reduce
+BINDING(loo_pit_reduce)
+  const int32_t points = (int32_t)to_double(env, a.at(4));
+  const std::vector<double> mn = doubles(env, a.at(6)), ct = doubles(env, a.at(7)), y = doubles(env, a.at(8));
+  if (points < 0 || mn.size() != (size_t)points || ct.size() != (size_t)points || y.size() != (size_t)points)
+    throw Throw{"loo_pit_reduce: llmin, cut and y must hold one number per point"};
+  std::vector<double> out((size_t)points * 3);
+  if (amwg_loo_pit_reduce((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (const double*)(uintptr_t)to_u64(env, a.at(2)),
+                          (int64_t)to_double(env, a.at(3)), points, (int64_t)to_double(env, a.at(5)), mn.data(), ct.data(), y.data(),
+                          (int32_t)to_double(env, a.at(9)), (double*)(uintptr_t)to_u64(env, a.at(10)), (uint8_t*)(uintptr_t)to_u64(env, a.at(11)),
+                          (int32_t*)(uintptr_t)to_u64(env, a.at(12)), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
+// loo_pit_fit(device, tails ptr, flags ptr, counts ptr, shards, points, tail_cap, llmin [points], cut [points], skip [points])
+//   -> Float64Array [points][5]                                                                                amwg_loo_pit_fit
+BINDING(loo_pit_fit)
+  const int32_t points = (int32_t)to_double(env, a.at(5));
+  const std::vector<double> mn = doubles(env, a.at(7)), ct = doubles(env, a.at(8));
+  const std::vector<int32_t> skip = ints(env, a.at(9));
+  if (points < 0 || mn.size() != (size_t)points || ct.size() != (size_t)points || skip.size() != (size_t)points)
+    throw Throw{"loo_pit_fit: llmin, cut and skip must hold one value per point"};
+  std::vector<double> out((size_t)points * 5);
+  if (amwg_loo_pit_fit((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (const uint8_t*)(uintptr_t)to_u64(env, a.at(2)),
+                       (const int32_t*)(uintptr_t)to_u64(env, a.at(3)), (int32_t)to_double(env, a.at(4)), points, (int32_t)to_double(env, a.at(6)),
+                       mn.data(), ct.data(), skip.data(), out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
 // ppc_pointwise(handle, code [n], consts [k], family, arg_progs [K], fold_prog [f], fold_dst [f], samples ptr, rows, entries, points,
 //               p0, n_points, out ptr, stats ptr)                                                           amwg_ppc_pointwise
 BINDING(ppc_pointwise)
@@ -632,6 +662,7 @@ NAPI_MODULE_INIT() {
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
       {"summary_comoments", summary_comoments}, {"summary_nested", summary_nested},
       {"loo_pointwise", loo_pointwise}, {"loo_reduce", loo_reduce}, {"loo_fit", loo_fit},
+      {"loo_pit_reduce", loo_pit_reduce}, {"loo_pit_fit", loo_pit_fit},
       {"ppc_pointwise", ppc_pointwise}, {"summary_threshold_counts", summary_threshold_counts},
       {"peak_fp64", peak_fp64}, {"jit_status", jit_status}, {"plate_sources", plate_sources}, {"term_cache", term_cache},
       {"jit_compile_check", jit_compile_check}};
