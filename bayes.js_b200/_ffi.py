@@ -71,7 +71,7 @@ EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_samp
            "amwg_plate_sources", "amwg_get_term_cache", "amwg_summary_finite_range", "amwg_summary_histogram", "amwg_summary_histogram2d",
            "amwg_summary_comoments", "amwg_disperse_state_superchains", "amwg_summary_nested",
            "amwg_loo_pointwise", "amwg_loo_reduce", "amwg_loo_fit", "amwg_ppc_pointwise", "amwg_summary_threshold_counts",
-           "amwg_loo_pit_reduce", "amwg_loo_pit_fit"]
+           "amwg_loo_pit_reduce", "amwg_loo_pit_fit", "amwg_summary_autocov_sq", "amwg_summary_indicator_autocov"]
 
 _lib = None
 
@@ -118,6 +118,9 @@ def lib():
     L.amwg_summary_moments.argtypes = [C.c_int, vp, i64, i32, i64, vp]; L.amwg_summary_moments.restype = C.c_int
     L.amwg_summary_digit_hist.argtypes = [C.c_int, vp, i64, i32, i64, i32, vp, i32, vp]; L.amwg_summary_digit_hist.restype = C.c_int
     L.amwg_summary_autocov.argtypes = [C.c_int, vp, i64, i32, i64, vp, i64, i32, vp]; L.amwg_summary_autocov.restype = C.c_int
+    L.amwg_summary_autocov_sq.argtypes = [C.c_int, vp, i64, i32, i64, vp, vp, i64, i32, vp]; L.amwg_summary_autocov_sq.restype = C.c_int
+    L.amwg_summary_indicator_autocov.argtypes = [C.c_int, vp, i64, i32, i64, vp, i32, i64, i32, vp]
+    L.amwg_summary_indicator_autocov.restype = C.c_int
     L.amwg_summary_rank_sort.argtypes = [C.c_int, vp, i64, i32, i64, i32, C.c_double, vp, vp, vp]; L.amwg_summary_rank_sort.restype = C.c_int
     L.amwg_summary_rank_count.argtypes = [C.c_int, vp, i64, vp, i64, vp]; L.amwg_summary_rank_count.restype = C.c_int
     L.amwg_summary_rank_z.argtypes = [C.c_int, vp, vp, i64, i64, vp]; L.amwg_summary_rank_z.restype = C.c_int

@@ -28,15 +28,30 @@ __host__ __device__ __forceinline__ double autocov_scale(double q05, double q95)
   return ldexp(1.0, k);
 }
 
+struct SeriesIdentity {
+  __host__ __device__ __forceinline__ double operator()(double v) const { return v; }
+};
+
+// y = ((x - centre) * scale)^2: the squared deviations whose ESS gives mcse_sd. scale is a power of two (the host takes it from the
+// pooled sd), so y is exactly scale^2 times the unscaled square while that stays normal.
+struct SquaredDeviation {
+  double centre, scale;
+  __host__ __device__ __forceinline__ double operator()(double v) const {
+    const double d = (v - centre) * scale;
+    return d * d;
+  }
+};
+
 // One half-chain p[n * stride], n < h, of a thread's chain: adds its lag sums for the lags lag0 + k, k < kLagSlots, to acc and
 // merges its record into mom. Pass 1 reads the half for its means; pass 2 reads it again and keeps the kLagSlots centred values at
 // positions n+lag0 .. n+lag0+15 in a register ring, so every loaded value serves all lags of the window. NS = 1: the draws only;
 // NS = 3: also 1[x <= q0] and 1[x <= q1], formed from the same loads (the ring holds their bits), and the draws scaled by sc.
-// Positions at or past h count as 0, so a product exists exactly when both ends lie in the half.
-template <int NS>
+// Positions at or past h count as 0, so a product exists exactly when both ends lie in the half. tf maps every value read to the
+// series walked (SeriesIdentity: the draws; SquaredDeviation: y = ((x - centre) * scale)^2 of amwg_summary_autocov_sq).
+template <int NS, class Tf = SeriesIdentity>
 __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__ p, long long h, size_t stride, double q0, double q1, double sc,
-                                                      long long lag0, double (&acc)[NS][kLagSlots], Moments (&mom)[NS]) {
-  const double x0 = p[0];
+                                                      long long lag0, double (&acc)[NS][kLagSlots], Moments (&mom)[NS], Tf tf = Tf()) {
+  const double x0 = tf(p[0]);
   const unsigned long long x0_bits = run_bits(x0);
   unsigned long long diff = 0;
   double s0 = 0.0;
@@ -45,7 +60,7 @@ __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__
   for (; r + 8 <= h; r += 8) {                           // eight loads in flight per thread, the sum stays sequential
     double v[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) v[u] = p[(r + u) * stride];
+    for (int u = 0; u < 8; ++u) v[u] = tf(p[(r + u) * stride]);
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       s0 += v[u];
@@ -54,7 +69,7 @@ __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__
     }
   }
   for (; r < h; ++r) {
-    const double v = p[r * stride];
+    const double v = tf(p[r * stride]);
     s0 += v;
     diff |= run_bits(v) ^ x0_bits;
     if constexpr (NS == 3) { n0 += v <= q0; n1 += v <= q1; }
@@ -72,7 +87,7 @@ __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__
     const long long pp = lag0 + k;
     ring[k] = 0.0;
     if (pp < h) {
-      const double v = p[pp * stride];
+      const double v = tf(p[pp * stride]);
       ring[k] = centred(v);
       valid |= 1u << k;
       if constexpr (NS == 3) { b0 |= (unsigned)(v <= q0) << k; b1 |= (unsigned)(v <= q1) << k; }
@@ -86,7 +101,7 @@ __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__
     for (int u = 0; u < kLagSlots; ++u) {                 // unrolled: the ring's slot indices are compile-time constants
       const long long n = j + u;
       if (n < h) {
-        const double v = p[n * stride];
+        const double v = tf(p[n * stride]);
         double cur[NS];
         cur[0] = centred(v);
         if constexpr (NS == 3) { cur[1] = v <= q0 ? 1.0 - m[1] : -m[1]; cur[2] = v <= q1 ? 1.0 - m[2] : -m[2]; }
@@ -109,7 +124,7 @@ __host__ __device__ __forceinline__ void autocov_half(const double* __restrict__
         ring[u] = 0.0;
         valid &= ~bit; b0 &= ~bit; b1 &= ~bit;
         if (pp < h) {
-          const double w = p[pp * stride];
+          const double w = tf(p[pp * stride]);
           ring[u] = centred(w);
           valid |= bit;
           if constexpr (NS == 3) { if (w <= q0) b0 |= bit; if (w <= q1) b1 |= bit; }

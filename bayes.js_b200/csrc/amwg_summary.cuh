@@ -13,6 +13,9 @@
 //   K_a1  amwg_autocov_kernel       : one thread per chain: split-chain (two halves) moment records and lag sums of the draws and
 //                                     of two tail indicators, for 16 lags per pass (effective sample size, split R-hat)
 //   K_a2  amwg_merge_sums_kernel    : one CTA per (entry, series, lag) sums the per-CTA lag sums in a FIXED order
+//   K_a3  amwg_autocov_sq_kernel    : K_a1's draws series of the squared deviations ((x - centre) * scale)^2 (mcse_sd)
+//   K_i1  amwg_indicator_kernel     : one thread per chain: exact integer pair counts, edge terms and counts of the indicators
+//                                     1[x <= q_k] of both halves, 4 thresholds and 64 lags per read (ess_quantile, mcse_quantile)
 //   K_r0..K_r3  amwg_rank_hist / sort_count / sort_scan / sort_scatter : LSD radix sort of one entry's half-chain keys (8-bit
 //                                     digits, stable; digit positions equal in all keys skipped) for the rank-normalised diagnostics
 //   K_r4  amwg_rank_count_kernel    : merge-path rank counts of a sorted key array against another (integer, exact)
@@ -36,6 +39,7 @@
 #include "amwg_autocov.cuh"      // the half-chain walk of K_a1
 #include "amwg_comoments.cuh"
 #include "amwg_hist.cuh"
+#include "amwg_indicator.cuh"    // the half-chain walk of K_i1
 #include "amwg_nested.cuh"      // Moments and merge
 
 namespace summary {
@@ -386,6 +390,38 @@ __global__ void __launch_bounds__(256) amwg_autocov_kernel(const double* __restr
       }
 }
 
+// K_a3: K_a1<1>'s walk and reductions for the draws series y = ((x - cs[e][0]) * cs[e][1])^2, the squared deviations behind
+// mcse_sd: autocov_half with the SquaredDeviation transform. K_a1's text is left as it is, so its instructions do not change.
+__global__ void __launch_bounds__(256) amwg_autocov_sq_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                              const double* __restrict__ cs, long long lag0, int n_lags, int k_base, int n_total,
+                                                              Moments* __restrict__ pmom, double* __restrict__ psum) {
+  __shared__ Moments sh[256];
+  const int e = blockIdx.y;
+  const long long h = rows / 2;
+  const size_t stride = (size_t)entries * C;
+  const SquaredDeviation tf{cs[2 * e], cs[2 * e + 1]};
+  double acc[1][kLagSlots];
+#pragma unroll
+  for (int k = 0; k < kLagSlots; ++k) acc[0][k] = 0.0;
+  Moments mom[1] = {Moments{0.0, 0.0, 0.0, 0.0}};
+  for (long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.x * blockDim.x) {
+    for (int half = 0; half < 2; ++half)
+      autocov_half<1>(x + (size_t)e * C + c + (size_t)(half ? rows - h : 0) * stride, h, stride, 0.0, 0.0, 1.0, lag0, acc, mom, tf);
+  }
+  if (pmom) {
+    const Moments tot = cta_merge<256>(sh, mom[0]);
+    if (threadIdx.x == 0) pmom[(size_t)e * gridDim.x + blockIdx.x] = tot;
+    __syncthreads();
+  }
+  double* shd = reinterpret_cast<double*>(sh);
+#pragma unroll
+  for (int k = 0; k < kLagSlots; ++k)
+    if (k < n_lags) {
+      const double tot = cta_sum<256>(shd, acc[0][k]);
+      if (threadIdx.x == 0) psum[((size_t)e * n_total + k_base + k) * gridDim.x + blockIdx.x] = tot;
+    }
+}
+
 // K_a2: one CTA per (entry, series, lag) sums the per-CTA lag sums in a fixed order.
 __global__ void __launch_bounds__(256) amwg_merge_sums_kernel(const double* __restrict__ psum, int n_partial, double* __restrict__ out) {
   __shared__ double sh[256];
@@ -394,6 +430,99 @@ __global__ void __launch_bounds__(256) amwg_merge_sums_kernel(const double* __re
   for (int i = threadIdx.x; i < n_partial; i += 256) acc += psum[row * n_partial + i];
   const double tot = cta_sum<256>(sh, acc);
   if (threadIdx.x == 0) out[row] = tot;
+}
+
+// ---- exact indicator autocovariances (ess_quantile and mcse_quantile of sample_summary(..., mcse=True)) ---------------------
+// K_i1: one thread per chain (grid-stride in warp-uniform steps), both halves, each by indicator_half (amwg_indicator.cuh) for the
+// kIndGroup thresholds of blockIdx.z. The sink sums each word's pair counts across the warp (redux.sync), gathers the sums of 32
+// consecutive lags into the 32 lanes (lane l holds lag 32m + l) and adds them to per-CTA shared counters with one 64-bit shared
+// atomic per lane; the edge terms go the same way (one 32-bit warp sum while h < 2048, else three 21-bit limbs), and the counts c
+// and c^2 stay in registers until the end.
+// The CTA then adds each counter to out with one 64-bit global atomic. Integers throughout: the result does not depend on the
+// order of the atomics, the chain order or the launch shape.
+struct WarpIndicatorSink {
+  unsigned long long (*cnt)[2 + 2 * kIndLags];          // shared [kIndGroup][2 + 2 kIndLags]: C1, C2, P_t (i < 64), G_t (i < 64)
+  unsigned lane;
+  int n_lags;
+  bool small;                                           // h < 2048: an edge term and its warp sum fit in 32 bits
+  unsigned long long mine;                              // this lane's lag of the current block of 32
+  unsigned long long c1[kIndGroup], c2[kIndGroup];
+
+  __device__ __forceinline__ void flush(int k, int i, int base) {                // after lag i: lanes 0 .. i & 31 hold their lags
+    if ((i & 31) == 31 || i == n_lags - 1)
+      if (lane <= (unsigned)(i & 31)) atomicAdd(&cnt[k][base + (i & ~31) + (int)lane], mine);
+  }
+  __device__ __forceinline__ void pair(int k, int i, unsigned v) {
+    const unsigned s = __reduce_add_sync(0xffffffffu, v);                 // <= 32 * 64
+    if (lane == (unsigned)(i & 31)) mine = s;
+    flush(k, i, 2);
+  }
+  // v = c (F_t + L_t) <= 2 h^2. h < 2048 (warp-uniform): v < 2^23, one 32-bit warp sum (< 2^28); else v < 2^63 in three limbs of
+  // 21 bits, each warp sum < 2^26
+  __device__ __forceinline__ void edge(int k, int i, unsigned long long v) {
+    unsigned long long s;
+    if (small) {
+      s = __reduce_add_sync(0xffffffffu, (unsigned)v);
+    } else {
+      const unsigned long long s0 = __reduce_add_sync(0xffffffffu, (unsigned)(v & 0x1FFFFFull));
+      const unsigned long long s1 = __reduce_add_sync(0xffffffffu, (unsigned)((v >> 21) & 0x1FFFFFull));
+      const unsigned long long s2 = __reduce_add_sync(0xffffffffu, (unsigned)(v >> 42));
+      s = s0 + (s1 << 21) + (s2 << 42);
+    }
+    if (lane == (unsigned)(i & 31)) mine = s;
+    flush(k, i, 2 + kIndLags);
+  }
+  __device__ __forceinline__ void count(int k, long long c) {
+    c1[k] += (unsigned long long)c;
+    c2[k] += (unsigned long long)(c * c);
+  }
+};
+
+// out[(e*K + k)][2 + 2*n_lags] += {C1, C2, P_t..., G_t...} (zeroed by the caller), thr[e][K]
+__global__ void __launch_bounds__(256, 2) amwg_indicator_kernel(const double* __restrict__ x, long long rows, int entries, long long C,
+                                                             const double* __restrict__ thr, int K, long long lag0, int n_lags,
+                                                             unsigned long long* __restrict__ out) {
+  __shared__ unsigned long long sh[kIndGroup][2 + 2 * kIndLags];
+  __shared__ unsigned long long keep[4 * kIndGroup][256];            // indicator_half's four kept words per threshold and thread
+  const int e = blockIdx.y, k0 = blockIdx.z * kIndGroup;
+  const long long h = rows / 2;
+  const size_t stride = (size_t)entries * C;
+  double q[kIndGroup];
+#pragma unroll
+  for (int k = 0; k < kIndGroup; ++k) q[k] = k0 + k < K ? thr[(size_t)e * K + k0 + k] : __longlong_as_double(0x7ff8000000000000ll);   // NaN: no bits
+  for (int i = threadIdx.x; i < kIndGroup * (2 + 2 * kIndLags); i += blockDim.x) (&sh[0][0])[i] = 0ull;
+  __syncthreads();
+  WarpIndicatorSink sink;
+  sink.cnt = sh;
+  sink.lane = threadIdx.x & 31u;
+  sink.n_lags = n_lags;
+  sink.small = h < 2048;
+  sink.mine = 0ull;
+#pragma unroll
+  for (int k = 0; k < kIndGroup; ++k) sink.c1[k] = sink.c2[k] = 0ull;
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long c0 = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); c0 < C; c0 += step) {   // warp-uniform bound
+    const long long c = c0 + sink.lane;
+    const bool live = c < C;
+    const double* col = x + (size_t)e * C + (live ? c : 0);
+    for (int half = 0; half < 2; ++half)
+      indicator_half<kIndGroup>(col + (size_t)(half ? rows - h : 0) * stride, h, stride, live, q, lag0, n_lags, &keep[0][threadIdx.x], 256, sink);
+  }
+#pragma unroll
+  for (int k = 0; k < kIndGroup; ++k) {
+    unsigned long long a = sink.c1[k], b = sink.c2[k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
+    if (sink.lane == 0) { atomicAdd(&sh[k][0], a); atomicAdd(&sh[k][1], b); }
+  }
+  __syncthreads();
+  const int w = 2 + 2 * n_lags;
+  for (int i = threadIdx.x; i < kIndGroup * w; i += blockDim.x) {
+    const int k = i / w, f = i % w;
+    const int src = f < 2 + n_lags ? f : f - n_lags + kIndLags;       // G_t sits at 2 + kIndLags + i in shared memory
+    const unsigned long long v = sh[k][src];
+    if (k0 + k < K && v != 0ull) atomicAdd(&out[((size_t)e * K + k0 + k) * w + f], v);
+  }
 }
 
 // ---- ranks over the pooled half-chain draws (rank-normalised R-hat, bulk effective sample size) -------------------------------
@@ -834,48 +963,100 @@ extern "C" int amwg_summary_digit_hist(int device, const double* dev_samples, in
   return 0;
 }
 
-extern "C" int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
-                                    const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out) {
-  if (rows < 2) return fail("amwg_summary_autocov: rows must be at least 2 (two half-chains of one draw)");
-  if (entries <= 0 || chains <= 0) return fail("amwg_summary_autocov: empty sample block");
-  if (n_lags < 1 || n_lags > 2 * summary::kLagSlots) return fail("amwg_summary_autocov: n_lags must be 1.." + std::to_string(2 * summary::kLagSlots));
+namespace summary {
+// amwg_summary_autocov and amwg_summary_autocov_sq: the checks, the K_a1 / K_a3 passes (one per kLagSlots lags), the merges and
+// the host record. sq: params[entry][2] = {centre, scale} of the squared deviations (K_a3); else thresholds[entry][2] or null (K_a1).
+static int autocov_entry(const char* name, bool sq, int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                         const double* host_params, int64_t lag0, int32_t n_lags, double* host_out) {
+  const std::string who(name);
+  if (rows < 2) return fail(who + ": rows must be at least 2 (two half-chains of one draw)");
+  if (entries <= 0 || chains <= 0) return fail(who + ": empty sample block");
+  if (n_lags < 1 || n_lags > 2 * kLagSlots) return fail(who + ": n_lags must be 1.." + std::to_string(2 * kLagSlots));
   if (lag0 < 0 || lag0 + n_lags > rows / 2)
-    return fail("amwg_summary_autocov: the lag window [lag0, lag0 + n_lags) must lie in [0, rows/2) (rows/2 = " + std::to_string(rows / 2) + ")");
-  if (!dev_samples || !host_out) return fail("amwg_summary_autocov: null pointer");
-  if (summary::select_device(device, "amwg_summary_autocov")) return -1;
-  const int ns = host_thresholds ? 3 : 1;
-  const unsigned bx = (unsigned)summary::chain_ctas(chains);
+    return fail(who + ": the lag window [lag0, lag0 + n_lags) must lie in [0, rows/2) (rows/2 = " + std::to_string(rows / 2) + ")");
+  if (!dev_samples || !host_out || (sq && !host_params)) return fail(who + ": null pointer");
+  if (select_device(device, name)) return -1;
+  const int ns = (host_params && !sq) ? 3 : 1;
+  const unsigned bx = (unsigned)chain_ctas(chains);
   const size_t rec = (size_t)entries * ns, sums = rec * n_lags;
-  summary::Scratch sc;
-  if (sc.acquire(device, "amwg_summary_autocov", {rec * bx * sizeof(summary::Moments), sums * bx * sizeof(double), rec * 4 * sizeof(double),
-                                                  sums * sizeof(double), (size_t)entries * 2 * sizeof(double)}))
+  Scratch sc;
+  if (sc.acquire(device, name, {rec * bx * sizeof(Moments), sums * bx * sizeof(double), rec * 4 * sizeof(double),
+                                sums * sizeof(double), (size_t)entries * 2 * sizeof(double)}))
     return -1;
-  auto* pmom = sc.part<summary::Moments>(0);
+  auto* pmom = sc.part<Moments>(0);
   auto* psum = sc.part<double>(1);
   auto* d_mom = sc.part<double>(2);
   auto* d_sum = sc.part<double>(3);
   auto* d_thr = sc.part<double>(4);
-  if (host_thresholds) CUDA_TRY(cudaMemcpy(d_thr, host_thresholds, (size_t)entries * 2 * sizeof(double), cudaMemcpyHostToDevice));
-  for (int k0 = 0; k0 < n_lags; k0 += summary::kLagSlots) {                 // one pass over the block per kLagSlots lags
-    const int nk = std::min(summary::kLagSlots, n_lags - k0);
-    summary::Moments* pm = k0 == 0 ? pmom : nullptr;                         // the records do not depend on the lags
-    if (ns == 3)
-      summary::amwg_autocov_kernel<3><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, d_thr, lag0 + k0, nk, k0, n_lags, pm, psum);
+  if (host_params) CUDA_TRY(cudaMemcpy(d_thr, host_params, (size_t)entries * 2 * sizeof(double), cudaMemcpyHostToDevice));
+  for (int k0 = 0; k0 < n_lags; k0 += kLagSlots) {                          // one pass over the block per kLagSlots lags
+    const int nk = std::min(kLagSlots, n_lags - k0);
+    Moments* pm = k0 == 0 ? pmom : nullptr;                                  // the records do not depend on the lags
+    if (sq)
+      amwg_autocov_sq_kernel<<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, d_thr, lag0 + k0, nk, k0, n_lags, pm, psum);
+    else if (ns == 3)
+      amwg_autocov_kernel<3><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, d_thr, lag0 + k0, nk, k0, n_lags, pm, psum);
     else
-      summary::amwg_autocov_kernel<1><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, nullptr, lag0 + k0, nk, k0, n_lags, pm, psum);
+      amwg_autocov_kernel<1><<<dim3(bx, (unsigned)entries), 256>>>(dev_samples, rows, entries, chains, nullptr, lag0 + k0, nk, k0, n_lags, pm, psum);
   }
-  summary::amwg_merge_moments_kernel<<<(unsigned)rec, 1024>>>(pmom, (int)bx, d_mom);
-  summary::amwg_merge_sums_kernel<<<(unsigned)sums, 256>>>(psum, (int)bx, d_sum);
+  amwg_merge_moments_kernel<<<(unsigned)rec, 1024>>>(pmom, (int)bx, d_mom);
+  amwg_merge_sums_kernel<<<(unsigned)sums, 256>>>(psum, (int)bx, d_sum);
   std::vector<double> mom(rec * 4), sm(sums);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaMemcpy(mom.data(), d_mom, mom.size() * sizeof(double), cudaMemcpyDeviceToHost);
   if (e == cudaSuccess) e = cudaMemcpy(sm.data(), d_sum, sm.size() * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e != cudaSuccess) return fail(std::string("amwg_summary_autocov: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(who + ": " + cudaGetErrorString(e));
   const size_t w = 4 + (size_t)n_lags;                                        // host_out[entry][series][4 + n_lags]
   for (size_t r = 0; r < rec; ++r) {
     for (int i = 0; i < 4; ++i) host_out[r * w + i] = mom[r * 4 + i];
     for (int k = 0; k < n_lags; ++k) host_out[r * w + 4 + k] = sm[r * n_lags + k];
   }
+  return 0;
+}
+}  // namespace summary
+
+extern "C" int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                    const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out) {
+  return summary::autocov_entry("amwg_summary_autocov", false, device, dev_samples, rows, entries, chains, host_thresholds, lag0, n_lags, host_out);
+}
+
+extern "C" int amwg_summary_autocov_sq(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                       const double* host_centre, const double* host_scale, int64_t lag0, int32_t n_lags, double* host_out) {
+  std::vector<double> cs;
+  if (host_centre && host_scale && entries > 0) {
+    cs.resize((size_t)entries * 2);
+    for (int32_t e = 0; e < entries; ++e) { cs[2 * (size_t)e] = host_centre[e]; cs[2 * (size_t)e + 1] = host_scale[e]; }
+  }
+  return summary::autocov_entry("amwg_summary_autocov_sq", true, device, dev_samples, rows, entries, chains, cs.empty() ? nullptr : cs.data(),
+                                lag0, n_lags, host_out);
+}
+
+extern "C" int amwg_summary_indicator_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                              const double* host_thresholds, int32_t n_thresholds, int64_t lag0, int32_t n_lags, int64_t* host_out) {
+  if (rows < 2) return fail("amwg_summary_indicator_autocov: rows must be at least 2 (two half-chains of one draw)");
+  if (rows >= (int64_t)1 << 32) return fail("amwg_summary_indicator_autocov: more than 2^32 rows");
+  if (entries <= 0 || chains <= 0) return fail("amwg_summary_indicator_autocov: empty sample block");
+  if (n_thresholds < 1 || n_thresholds > summary::kIndMaxThresholds)
+    return fail("amwg_summary_indicator_autocov: n_thresholds must be 1.." + std::to_string(summary::kIndMaxThresholds));
+  if (n_lags < 1 || n_lags > summary::kIndLags) return fail("amwg_summary_indicator_autocov: n_lags must be 1.." + std::to_string(summary::kIndLags));
+  if (lag0 < 0 || lag0 + n_lags > rows / 2)
+    return fail("amwg_summary_indicator_autocov: the lag window [lag0, lag0 + n_lags) must lie in [0, rows/2) (rows/2 = " + std::to_string(rows / 2) + ")");
+  if (!dev_samples || !host_thresholds || !host_out) return fail("amwg_summary_indicator_autocov: null pointer");
+  if (summary::select_device(device, "amwg_summary_indicator_autocov")) return -1;
+  const unsigned bx = (unsigned)summary::chain_ctas(chains);
+  const unsigned groups = (unsigned)((n_thresholds + summary::kIndGroup - 1) / summary::kIndGroup);
+  const size_t n_thr = (size_t)entries * n_thresholds, n_out = n_thr * (2 + 2 * (size_t)n_lags);
+  summary::Scratch sc;
+  if (sc.acquire(device, "amwg_summary_indicator_autocov", {n_thr * sizeof(double), n_out * sizeof(int64_t)})) return -1;
+  auto* d_thr = sc.part<double>(0);
+  auto* d_out = sc.part<unsigned long long>(1);
+  CUDA_TRY(cudaMemcpy(d_thr, host_thresholds, n_thr * sizeof(double), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemset(d_out, 0, n_out * sizeof(int64_t)));
+  summary::amwg_indicator_kernel<<<dim3(bx, (unsigned)entries, groups), 256>>>(dev_samples, rows, entries, chains, d_thr, n_thresholds, lag0,
+                                                                              n_lags, d_out);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(host_out, d_out, n_out * sizeof(int64_t), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) return fail(std::string("amwg_summary_indicator_autocov: ") + cudaGetErrorString(e));
   return 0;
 }
 

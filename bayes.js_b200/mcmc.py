@@ -697,7 +697,7 @@ class AmwgSampler(Sampler):
         return buf
 
     def sample_summary(self, n_iterations, probs=(0.025, 0.25, 0.5, 0.75, 0.975), diagnostics=False, histogram=None, covariance=None,
-                       nested=None, loo=None, ppc=None):
+                       nested=None, loo=None, ppc=None, mcse=False):
         """Not in the reference (SURVEY 8(f).3): the same sweeps and the same kept rows as `sample(n)` (thin / monitor apply), but the
         draws stay in HBM and only their summary comes back: {name: {"mean", "sd", "rhat", "quantiles", "n_draws"}}, pooled over
         all chains and kept rows; multi-dim parameters give arrays of their `dim` ("quantiles": [len(probs), *dim], exact order
@@ -807,13 +807,25 @@ class AmwgSampler(Sampler):
         independent of the order of tied draws (a rejected step repeats its ll), and so of sharding, chunking and the sort. See
         summary.loo_pit_chunk. Every other key, and the chains' state, keep their bits. A refused loo_pit (anything but True or
         {"r_eff": ...}, an r_eff not finite and > 0, fewer than 2 draws, a tail of more than 2^20 draws) raises ValueError before
-        the chains move."""
+        the chains move.
+        mcse=True adds Monte Carlo standard errors of the quantiles and of the sd (Vehtari et al. 2021, §4.3; posterior's
+        mcse_quantile / mcse_sd, ArviZ's mcse), with any diagnostics= and every other option. Per monitored name, "ess_quantile"
+        and "mcse_quantile" are shaped like "quantiles": the split-chain ESS of the indicator 1[x <= q_p] for each p in probs,
+        formed on the device from exact integer autocovariance sums (so it does not depend on the number of GPUs or the chain
+        order), and the standard error of each returned quantile, half the distance between the two exact order statistics at
+        the ranks of ArviZ's beta rule. "mcse_sd", shaped like "mean", is the delta-method standard error of "sd" from the ESS of
+        the squared deviations (x - mean)^2. Fewer than 10 kept rows or a NaN draw give NaN; +-inf draws give mcse_sd NaN; a
+        constant entry gives M h, 0 and 0. See summary.mcse_block for the definitions and edge cases. It needs scipy
+        (scipy.special.betaincinv). Every other key, and the chains' state, keep their bits. Anything but a bool, mcse=True
+        without scipy, or 2 M h^2 >= 2^63 (M = 2 x chains, h = kept rows // 2) raises ValueError before the chains move."""
         import torch
         from .summary import (CudaBlockReducer, CudaPointwise, CudaPpc, check_diagnostics, check_loo_size, check_ppc_call, comoments_scratch_bytes,
                               covariance_block, entry_spans, histogram_block, loo_block, loo_pit_point_bytes, loo_point_bytes, loo_tail_cap,
                               nested_block, nested_scratch_bytes, ppc_block, ppc_fixed_bytes, ppc_point_bytes, resolve_covariance,
                               resolve_histogram, resolve_loo, resolve_nested, resolve_ppc, summarise_block)
+        from .summary import check_mcse, check_mcse_size, mcse_block, mcse_scratch_bytes
         check_diagnostics(diagnostics)
+        check_mcse(mcse)
         monitored = self._state_keys() if self.monitored_params is None else list(self.monitored_params)
         entries = [i for name in monitored for i in self._entries(name)]
         spans = entry_spans(monitored, {name: [len(self._entries(name))] for name in monitored})
@@ -830,6 +842,8 @@ class AmwgSampler(Sampler):
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
         if rows == 0 or not entries:
             raise JsThrow("sample_summary needs at least one kept iteration and one monitored entry")
+        if mcse:
+            check_mcse_size(rows, self.n_chains)
         sampled = list(entries)                                 # the block's entries: the monitored ones, then what log_lik reads besides
         start = {}
 
@@ -876,6 +890,8 @@ class AmwgSampler(Sampler):
             need += comoments_scratch_bytes(len(cov_plan.entries), self.local_chains)
         if superchain is not None:
             need += nested_scratch_bytes(len(entries), self.local_chains, self.first_chain, superchain)
+        if mcse:
+            need += mcse_scratch_bytes(len(entries), len(probs))
         free, _total = torch.cuda.mem_get_info(dev)
         base = need + 2 * len(entries) * self.local_chains * 8      # and the base summary's scratch: two doubles per entry and chain
         if base > 0.9 * free:
@@ -934,6 +950,7 @@ class AmwgSampler(Sampler):
         hist = None if plan is None else histogram_block(reducer, block, rows, plan, self.distributed)
         cov = None if cov_plan is None else covariance_block(reducer, block, rows, cov_plan, self.distributed)
         rn = None if superchain is None else nested_block(reducer, block, rows, self.first_chain, superchain, self.distributed)
+        mc = mcse_block(reducer, block, rows, self.n_chains, probs, mean, sd, q, self.distributed) if mcse else None
         del block
         out = {}
         for name in monitored:
@@ -954,6 +971,10 @@ class AmwgSampler(Sampler):
                     out[name][key] = val[0] if dim == [1] else val.reshape(*dim, val.shape[-1])
             if rn is not None:
                 out[name]["rhat_nested"] = shape(rn[s0:s0 + ln])
+            if mc is not None:
+                for key in ("ess_quantile", "mcse_quantile"):
+                    out[name][key] = mc[key][:, s0] if dim == [1] else mc[key][:, s0:s0 + ln].reshape(len(q), *dim)
+                out[name]["mcse_sd"] = shape(mc["mcse_sd"][s0:s0 + ln])
         if hist is not None:
             out.update(hist["pairs"])
         if cov is not None:

@@ -19,6 +19,7 @@ until it returns; the memory checks add up the calls' requests, which bounds tha
 from __future__ import annotations
 
 import ctypes as C
+import math
 import numbers
 from typing import List, NamedTuple, Optional, Sequence, Tuple
 
@@ -100,13 +101,15 @@ def _lerp(a, b, t):
 
 class RadixSelect:
     """Host side of the 8-pass select: which prefixes the device should histogram next, and how the summed counts narrow
-    each wanted order statistic down by one byte. ranks: sorted 0-based ranks, shared by all entries."""
+    each wanted order statistic down by one byte. ranks: sorted 0-based ranks [T], shared by all entries, or [entries, T], each
+    entry's own (mcse_quantile's ranks depend on each entry's ESS); at most MAX_PREFIXES distinct ranks per entry."""
 
     def __init__(self, entries: int, ranks: np.ndarray):
+        r = np.asarray(ranks, dtype=np.int64)
         self.E = entries
-        self.T = len(ranks)
+        self.T = r.shape[-1]
         self.prefix = np.zeros((entries, self.T), dtype=np.uint64)
-        self.rem = np.tile(np.asarray(ranks, dtype=np.int64), (entries, 1))
+        self.rem = np.tile(r, (entries, 1)) if r.ndim == 1 else np.array(r.reshape(entries, self.T), copy=True)
         self.npass = 0
 
     def prefixes(self) -> Tuple[np.ndarray, np.ndarray]:
@@ -236,6 +239,27 @@ class CudaBlockReducer:
         out = np.empty((entries, ns, 4 + n_lags), dtype=np.float64)
         thr = None if thresholds is None else np.ascontiguousarray(thresholds, dtype=np.float64).reshape(entries, 2)
         self._call(block, self.L.amwg_summary_autocov, block.data_ptr(), rows, entries, chains, None if thr is None else thr.ctypes.data,
+                   lag0, n_lags, out.ctypes.data)
+        return out
+
+    def autocov_sq(self, block, centre, scale, lag0: int, n_lags: int) -> np.ndarray:
+        """-> [entries, 1, 4 + n_lags]: autocov's draws record of y = ((x - centre[e]) * scale[e])^2 for this shard; see
+        amwg_summary_autocov_sq in include/amwg.h."""
+        rows, entries, chains = block.shape
+        out = np.empty((entries, 1, 4 + n_lags), dtype=np.float64)
+        c = np.ascontiguousarray(centre, dtype=np.float64)
+        s = np.ascontiguousarray(scale, dtype=np.float64)
+        self._call(block, self.L.amwg_summary_autocov_sq, block.data_ptr(), rows, entries, chains, c.ctypes.data, s.ctypes.data, lag0,
+                   n_lags, out.ctypes.data)
+        return out
+
+    def indicator_autocov(self, block, thresholds, lag0: int, n_lags: int) -> np.ndarray:
+        """-> int64 [entries, K, 2 + 2 n_lags] = {C1, C2, P_t..., G_t...} of the indicators 1[x <= thresholds[e][k]] (thresholds
+        [entries, K], K <= 16, n_lags <= 64) for this shard; see amwg_summary_indicator_autocov in include/amwg.h."""
+        rows, entries, chains = block.shape
+        thr = np.ascontiguousarray(thresholds, dtype=np.float64).reshape(entries, -1)
+        out = np.empty((entries, thr.shape[1], 2 + 2 * n_lags), dtype=np.int64)
+        self._call(block, self.L.amwg_summary_indicator_autocov, block.data_ptr(), rows, entries, chains, thr.ctypes.data, thr.shape[1],
                    lag0, n_lags, out.ctypes.data)
         return out
 
@@ -391,7 +415,8 @@ class GeyerESS:
     lag it has not got yet (None once done); `add(sums)` appends the lag sums of the next window."""
 
     def __init__(self, record: np.ndarray, h: int):
-        M, _mean, m2, sum_w = np.asarray(record[:4], dtype=np.float64)        # numpy scalars: 0/0 is NaN, not an exception
+        self.record = np.asarray(record[:4], dtype=np.float64)
+        M, _mean, m2, sum_w = self.record                              # numpy scalars: 0/0 is NaN, not an exception
         self.h, self.M = h, M
         with np.errstate(invalid="ignore", divide="ignore"):
             self.W = sum_w / (M * (h - 1))                        # h/(h-1) * mean_m acov_m(0)
@@ -501,13 +526,20 @@ def autocov_record(reducer, block, thresholds, lag0: int, n_lags: int, distribut
 
 def geyer_windows(reducer, block, thresholds, h: int, distributed: bool, max_lags: int = MAX_LAGS):
     """-> (the GeyerESS of every entry and series of reducer.autocov(block, thresholds, ...) [entries][series], the number of
-    lag windows used). The first window holds lags [0, min(max_lags, h)); the next window of at most `max_lags` consecutive
-    lags is asked for only while some estimator still needs a lag it has not got, the way RadixSelect asks for its next pass."""
+    lag windows used), by geyer_loop over autocov_record."""
+    return geyer_loop(lambda lag0, n_lags: autocov_record(reducer, block, thresholds, lag0, n_lags, distributed), h, max_lags)
+
+
+def geyer_loop(fetch, h: int, max_lags: int):
+    """-> (the GeyerESS of every entry and series of the merged records fetch(lag0, n_lags) -> [entries, series, 4 + n_lags],
+    the number of lag windows used). The first window holds lags [0, min(max_lags, h)); the next window of at most `max_lags`
+    consecutive lags is asked for only while some estimator still needs a lag it has not got, the way RadixSelect asks for its
+    next pass."""
     est: Optional[List[List[GeyerESS]]] = None
     windows = lag0 = 0
     while est is None or (lag0 < h and any(g.need() is not None for row in est for g in row)):
         n_lags = min(max_lags, h - lag0)
-        rec = autocov_record(reducer, block, thresholds, lag0, n_lags, distributed)
+        rec = fetch(lag0, n_lags)
         if est is None:
             est = [[GeyerESS(r, h) for r in series] for series in rec]
         for row, series in zip(est, rec):
@@ -696,6 +728,201 @@ def nonfinite_as_numpy(reducer, block, mean: np.ndarray, q_user: np.ndarray, M: 
     mean[nan] = np.nan
     q_user[:, nan] = np.nan
     return mean, q_user
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Monte Carlo standard errors of the quantiles and of the sd (Vehtari et al. 2021, §4.3; ArviZ's mcse(method="quantile") / "sd")
+MAX_IND_THRESHOLDS = 16                # include/amwg.h: amwg_summary_indicator_autocov, n_thresholds <= 16 per call
+MAX_IND_LAGS = 64                      # and n_lags <= 64 per window
+MCSE_BETA_PROBS = (0.1586553, 0.8413447)    # Phi(-1), Phi(1): the +-1 sd points of the beta posterior of the rank
+
+
+def check_mcse(mcse) -> None:
+    if not isinstance(mcse, bool):
+        raise ValueError("mcse must be True or False, not %r" % (mcse,))
+
+
+def check_mcse_size(rows: int, total_chains: int) -> None:
+    """mcse=True before the chains move: the indicator counters (each below 2 M h^2, M = 2 * chains, h = rows // 2) must fit in
+    int64, and scipy's beta inverse must be importable."""
+    h = rows // 2
+    if 2 * (2 * total_chains) * h * h >= 1 << 63:
+        raise ValueError("mcse=True: %d chains x %d kept rows is too many for the exact indicator counts (2 M h^2 >= 2^63, M = 2 x "
+                         "chains, h = rows // 2); raise thin() or lower n" % (total_chains, rows))
+    try:
+        from scipy.special import betaincinv  # noqa: F401
+    except ImportError:
+        raise ValueError("mcse=True needs scipy (scipy.special.betaincinv, the beta quantile of the quantiles' standard errors); "
+                         "install scipy or call with mcse=False") from None
+
+
+def mcse_scratch_bytes(entries: int, n_probs: int) -> int:
+    """device scratch of mcse_block's calls at most: the indicator thresholds and counters of one call, and the records of
+    amwg_summary_autocov_sq (per-CTA moments and lag sums of 1184 CTAs)"""
+    k = min(max(n_probs, 1), MAX_IND_THRESHOLDS)
+    return entries * (k * (8 + 8 * (2 + 2 * MAX_IND_LAGS)) + 1184 * (32 + 8 * MAX_LAGS) + 8 * (6 + MAX_LAGS))
+
+
+def indicator_record(sums: np.ndarray, M: int, h: int, lag0: int) -> np.ndarray:
+    """Exact integer sums [entries, K, 2 + 2 n] = {C1, C2, P_t..., G_t...} (t = lag0 + i) -> GeyerESS records [entries, K, 4 + n]
+    {M, C1 / (M h), (M C2 - C1^2) / (M h^2), (h C1 - C2) / h, (h^2 P_t - h (2 C2 - G_t) + (h - t) C2) / h^2 ...}: each rational
+    correctly rounded once (Python's int / int), so the record is a function of the integers only."""
+    E, K, W = sums.shape
+    n = (W - 2) // 2
+    v = sums.astype(object)                                   # Python ints: no intermediate overflows or roundings
+    C1, C2 = v[:, :, 0], v[:, :, 1]
+    P, G = v[:, :, 2:2 + n], v[:, :, 2 + n:]
+    t = np.arange(lag0, lag0 + n, dtype=object)
+    out = np.empty((E, K, 4 + n), dtype=object)
+    out[:, :, 0] = M
+    out[:, :, 1] = C1 / (M * h)
+    out[:, :, 2] = (M * C2 - C1 * C1) / (M * h * h)
+    out[:, :, 3] = (h * C1 - C2) / h
+    out[:, :, 4:] = (h * h * P - h * (2 * C2[:, :, None] - G) + (h - t) * C2[:, :, None]) / (h * h)
+    return out.astype(np.float64)
+
+
+def _indicator_sums(reducer, block, thr, lag0: int, n_lags: int, distributed: bool) -> np.ndarray:
+    """reducer.indicator_autocov of every shard, summed (sum_counts)"""
+    got = reducer.indicator_autocov(block, thr, lag0, n_lags)
+    if not distributed:
+        return np.asarray(got, dtype=np.int64)
+    import torch
+    return sum_counts(torch.from_numpy(np.ascontiguousarray(got, dtype=np.int64)).to(block.device), True).cpu().numpy()
+
+
+def quantile_ess(reducer, block, rows: int, total_chains: int, thr: np.ndarray, distributed: bool, max_lags: int = MAX_IND_LAGS):
+    """-> (ESS [entries, K] of the indicators 1[x <= thr[e][k]] on the split halves, lag windows used). K thresholds go in calls
+    of at most MAX_IND_THRESHOLDS; each call's windows are those of geyer_loop over indicator_record. An indicator that is
+    constant (C1 = 0 or C1 = M h) has ESS = M h."""
+    entries, K = thr.shape
+    h, M = rows // 2, 2 * total_chains
+    ess = np.empty((entries, K))
+    windows = 0
+    for k0 in range(0, K, MAX_IND_THRESHOLDS):
+        t = np.ascontiguousarray(thr[:, k0:k0 + MAX_IND_THRESHOLDS])
+        first = []
+
+        def fetch(lag0, n_lags):
+            sums = _indicator_sums(reducer, block, t, lag0, n_lags, distributed)
+            if not first:
+                first.append(sums[:, :, 0])
+            return indicator_record(sums, M, h, lag0)
+
+        est, w = geyer_loop(fetch, h, max_lags)
+        windows += w
+        C1 = first[0]
+        for e in range(entries):
+            for k, g in enumerate(est[e]):
+                ess[e, k0 + k] = M * h if C1[e, k] == 0 or C1[e, k] == M * h else g.ess
+    return ess, windows
+
+
+def quantile_mcse_ranks(ess: np.ndarray, probs: Sequence[float], S: int):
+    """ArviZ's _mcse_quantile ranks: (a1, a2) = the MCSE_BETA_PROBS quantiles of Beta(ess p + 1, ess (1 - p) + 1), i1 =
+    rint(max(a1 S - 1, 0)), i2 = rint(min(a2 S - 1, S - 1)) (rint: half to even). ess [P, entries] -> (i1, i2) int64 [P, entries],
+    and where ess is NaN (ranks 0 there)."""
+    from scipy.special import betaincinv
+    p = np.asarray(probs, dtype=np.float64)[:, None]
+    bad = ~np.isfinite(ess)
+    e = np.where(bad, 1.0, ess)
+    a1 = betaincinv(e * p + 1, e * (1 - p) + 1, MCSE_BETA_PROBS[0])
+    a2 = betaincinv(e * p + 1, e * (1 - p) + 1, MCSE_BETA_PROBS[1])
+    i1 = np.rint(np.maximum(a1 * S - 1, 0))
+    i2 = np.rint(np.minimum(a2 * S - 1, S - 1))
+    bad |= ~(np.isfinite(i1) & np.isfinite(i2))
+    return np.where(bad, 0, i1).astype(np.int64), np.where(bad, 0, i2).astype(np.int64), bad
+
+
+def pow2_scale(sd: np.ndarray) -> np.ndarray:
+    """2^-ilogb(sd) clamped to [2^-1022, 2^1023]; 1 where sd is 0 or not finite"""
+    out = np.ones(len(sd))
+    for e, v in enumerate(np.asarray(sd, dtype=np.float64)):
+        if np.isfinite(v) and v > 0:
+            out[e] = math.ldexp(1.0, min(max(1 - math.frexp(float(v))[1], -1022), 1023))
+    return out
+
+
+def mcse_block(reducer, block, rows: int, total_chains: int, probs: Sequence[float], mean: np.ndarray, sd: np.ndarray, q_user: np.ndarray,
+               distributed: bool, max_lags: int = MAX_IND_LAGS) -> dict:
+    """-> {"ess_quantile" [len(probs), entries], "mcse_quantile" [len(probs), entries], "mcse_sd" [entries]} over all shards;
+    mean, sd and q_user are summarise_block's. Only reads the block.
+
+    h = rows // 2 and the halves are those of `split_chain_diagnostics`; M = 2 * chains over all GPUs; S = rows * chains, every
+    kept draw; q_p the returned quantile (numpy's linear rule).
+      ess_quantile   the split-chain ESS of b = 1[x <= q_p]. Per half-chain m with positions 0..h-1: c_m = sum_n b_mn, F_mt and
+                     L_mt the count among its first and last t positions. The integers C1 = sum c_m, C2 = sum c_m^2, P_t = sum_m
+                     sum_{n<h-t} b_mn b_m,n+t and G_t = sum_m c_m (F_mt + L_mt) (amwg_summary_indicator_autocov, summed over shards
+                     by sum_counts) give GeyerESS its exact inputs: mean of the half-chain means C1 / (M h), m2 = (M C2 - C1^2) /
+                     (M h^2), sum_w = (h C1 - C2) / h and lag sum_t = (h^2 P_t - h (2 C2 - G_t) + (h - t) C2) / h^2 (sum_w at t =
+                     0), each rounded once to the nearest double (indicator_record). So the ESS is a function of integers only:
+                     the same for any sharding, number of GPUs, chain order or launch shape. A constant indicator (C1 = 0 or
+                     C1 = M h) gives M h, as in split_chain_diagnostics; W = 0 otherwise gives NaN (GeyerESS).
+      mcse_quantile  ArviZ's rule: (a1, a2) the 0.1586553 and 0.8413447 quantiles of Beta(ess p + 1, ess (1 - p) + 1)
+                     (scipy.special.betaincinv), i1 = rint(max(a1 S - 1, 0)), i2 = rint(min(a2 S - 1, S - 1)) (half to even, as
+                     numpy.rint), and mcse = (x_(i2) - x_(i1)) / 2 with x_(i) the exact 0-based order statistics over all S
+                     draws (one more radix select at per-entry ranks, at most 16 probabilities per select). Unlike ArviZ, an ess of
+                     NaN gives NaN (ArviZ's nanmax / nanmin would take the extreme draws).
+      mcse_sd        the delta-method estimator of posterior / ArviZ: with x_bar the returned mean and s = 2^-ilogb(sd) (clamped
+                     to normal powers of two; 1 when sd is 0 or not finite), y = ((x - x_bar) s)^2 on the split halves
+                     (amwg_summary_autocov_sq, records merged by merge_autocov_records); y_bar = the mean of the half-chain means,
+                     v = (sum of within M2 + h * M2 of the half means) / (M h), the ddof-0 variance of y, ess_y = GeyerESS of y;
+                     mcse_sd = sqrt(v / (4 y_bar ess_y)) / s. For even rows y_bar and v are over all draws, as in ArviZ; for odd
+                     rows the middle row is left out of them, as it is out of every split-chain quantity.
+    Edge cases: fewer than 10 rows (MIN_ROWS): all NaN. A NaN draw in an entry: all three NaN. +-inf draws without NaN:
+    ess_quantile as defined (the indicators are finite), mcse_quantile by IEEE arithmetic on the two order statistics, mcse_sd
+    NaN. A constant entry (sd 0): ess_quantile M h, mcse_quantile 0, mcse_sd 0. Multiplying the draws by 2^j (no overflow or
+    underflow) leaves ess_quantile's bits and multiplies mcse_quantile and mcse_sd by exactly 2^j."""
+    entries = block.shape[1]
+    P = len(probs)
+    out = {"ess_quantile": np.full((P, entries), np.nan), "mcse_quantile": np.full((P, entries), np.nan),
+           "mcse_sd": np.full(entries, np.nan)}
+    if rows < MIN_ROWS:
+        return out
+    h, M, S = rows // 2, 2 * total_chains, rows * total_chains
+    nan_e = np.zeros(entries, dtype=bool)
+    inf_e = np.zeros(entries, dtype=bool)
+    if not np.all(np.isfinite(mean)):                         # which entries hold a NaN, which +-inf only (nonfinite_as_numpy)
+        keys = _select(reducer, block, np.unique([0, S - 1]), distributed).prefix
+        kmin, kmax = keys[:, 0], keys[:, -1]
+        nan_e = (kmin < _KEY_NEG_INF) | (kmax > _KEY_POS_INF)
+        inf_e = ~nan_e & ((kmin == _KEY_NEG_INF) | (kmax == _KEY_POS_INF))
+    if P:
+        ess, _ = quantile_ess(reducer, block, rows, total_chains, np.ascontiguousarray(np.asarray(q_user, dtype=np.float64).T), distributed,
+                              max_lags)
+        ess = ess.T                                           # [P, entries]
+        ess[:, nan_e] = np.nan
+        i1, i2, bad = quantile_mcse_ranks(ess, probs, S)
+        mq = np.empty((P, entries))
+        per_select = MAX_PREFIXES // 2
+        for first in range(0, P, per_select):
+            n = min(per_select, P - first)
+            ranks = np.empty((entries, 2 * n), dtype=np.int64)
+            ranks[:, 0::2] = i1[first:first + n].T
+            ranks[:, 1::2] = i2[first:first + n].T
+            vals = _select(reducer, block, ranks, distributed).values()
+            with np.errstate(invalid="ignore", over="ignore"):
+                mq[first:first + n] = ((vals[:, 1::2] - vals[:, 0::2]) / 2).T
+        mq[bad] = np.nan
+        out["ess_quantile"], out["mcse_quantile"] = ess, mq
+
+    ok = ~nan_e & ~inf_e & np.isfinite(mean)
+    scale = pow2_scale(sd)
+    centre = np.where(ok, mean, 0.0)
+    est, _ = geyer_loop(lambda lag0, n_lags: merge_autocov_records(gather(reducer.autocov_sq(block, centre, scale, lag0, n_lags), block,
+                                                                              distributed)), h, MAX_LAGS)
+    for e in range(entries):
+        if not ok[e]:
+            continue
+        if sd[e] == 0:
+            out["mcse_sd"][e] = 0.0
+            continue
+        g = est[e][0]
+        _, ybar, m2, sum_w = g.record
+        v = (sum_w + h * m2) / (M * h)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            out["mcse_sd"][e] = np.sqrt(v / (4.0 * ybar * g.ess)) / scale[e]
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------------------------

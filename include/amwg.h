@@ -332,6 +332,21 @@ AMWG_API int amwg_primitive_eval(int32_t kind, const double* x, int64_t n, uint6
  *   spread and the largest |x - mean|: outliers further out (spread 1e-10, outliers near 1e150) overflow once scaled. Errors: rows < 2, n_lags outside 1..32, lag0 + n_lags > h, null
  *   dev_samples / host_out.
  *
+ * amwg_summary_autocov_sq: amwg_summary_autocov's draws series without thresholds (one series, the same record layout and lag
+ *   windows) of y = ((x - host_centre[entry]) * host_scale[entry])^2, the squared deviations whose ESS gives mcse_sd
+ *   (sample_summary(..., mcse=True)). host_centre and host_scale are host arrays [entries]; the caller passes a power of two as
+ *   the scale. The half-chain walk is amwg_summary_autocov's (autocov_half with a series transform). Errors: those of
+ *   amwg_summary_autocov, and null host_centre / host_scale.
+ * amwg_summary_indicator_autocov: exact integer autocovariance sums of the indicators b = 1[x <= host_thresholds[entry][k]],
+ *   k < n_thresholds, on the split halves of amwg_summary_autocov (h = rows/2, M = 2*chains half-chains). Per half-chain m with
+ *   c_m = sum_n b_mn and F_mt / L_mt the count among its first / last t positions, host_out[entry][k][2 + 2*n_lags] (int64) =
+ *   { C1 = sum_m c_m, C2 = sum_m c_m^2, P_t = sum_m sum_{n<h-t} b_mn b_m,n+t for t = lag0 .. lag0+n_lags-1, then G_t = sum_m c_m
+ *   (F_mt + L_mt) for the same t }, overwritten. Integers: shards add up exactly, and the result does not depend on the chain
+ *   order, the launch shape or the number of GPUs. Every counter stays below 2*M*h^2 (the caller keeps that below 2^63). One read
+ *   of the block serves 4 thresholds and the whole window when lag0 < 64 (two reads otherwise). host_thresholds is host memory
+ *   [entries][n_thresholds]. Errors: rows < 2 or >= 2^32, an empty block, n_thresholds outside 1..16, n_lags outside 1..64, a
+ *   window [lag0, lag0 + n_lags) outside [0, rows/2), null pointers, a bad device index.
+ *
  * Ranks over the pooled half-chain draws (rank-normalised R-hat and bulk ESS, Vehtari et al. 2021, §4). One entry per call; the
  * caller owns every device buffer (keys, indices, rank sums, z-block), so the three calls keep no state between them.
  * amwg_summary_rank_sort: sorts the n = 2*(rows/2)*chains half-chain draws of `entry` (numbered i = r*chains + c, r < 2h: rows
@@ -395,6 +410,11 @@ AMWG_API int amwg_summary_digit_hist(int device, const double* dev_samples, int6
                                      const uint64_t* dev_prefix, int32_t n_prefix, uint64_t* dev_counts);
 AMWG_API int amwg_summary_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
                                   const double* host_thresholds, int64_t lag0, int32_t n_lags, double* host_out);
+AMWG_API int amwg_summary_autocov_sq(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                     const double* host_centre, const double* host_scale, int64_t lag0, int32_t n_lags, double* host_out);
+AMWG_API int amwg_summary_indicator_autocov(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains,
+                                            const double* host_thresholds, int32_t n_thresholds, int64_t lag0, int32_t n_lags,
+                                            int64_t* host_out);
 AMWG_API int amwg_summary_rank_sort(int device, const double* dev_samples, int64_t rows, int32_t entries, int64_t chains, int32_t entry,
                                     double centre, uint64_t* dev_keys, uint32_t* dev_index, int32_t* host_passes);
 AMWG_API int amwg_summary_rank_count(int device, const uint64_t* dev_q, int64_t nq, const uint64_t* dev_r, int64_t nr, int64_t* dev_acc);

@@ -434,6 +434,40 @@ BINDING(summary_autocov)
     fail_from_library();
   return f64_array(env, out.data(), out.size());
 END_BINDING
+// summary_autocov_sq(device, samples ptr, rows, entries, chains, centre [entries], scale [entries], lag0, n_lags)
+//   -> Float64Array [entries][1][4 + n_lags]                                                           amwg_summary_autocov_sq
+BINDING(summary_autocov_sq)
+  const int32_t entries = (int32_t)to_double(env, a.at(3));
+  const int32_t n_lags = (int32_t)to_double(env, a.at(8));
+  const std::vector<double> centre = doubles(env, a.at(5)), scale = doubles(env, a.at(6));
+  if (entries < 0 || centre.size() != (size_t)entries || scale.size() != (size_t)entries)
+    throw Throw{"summary_autocov_sq: centre and scale must hold one number per entry"};
+  std::vector<double> out((size_t)std::max(entries, 0) * (4 + (size_t)std::max(n_lags, 0)));
+  if (amwg_summary_autocov_sq((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)), entries,
+                              (int64_t)to_double(env, a.at(4)), centre.data(), scale.data(), (int64_t)to_double(env, a.at(7)), n_lags, out.data()) != 0)
+    fail_from_library();
+  return f64_array(env, out.data(), out.size());
+END_BINDING
+// summary_indicator_autocov(device, samples ptr, rows, entries, chains, thresholds [entries][K], K, lag0, n_lags)
+//   -> BigInt64Array [entries][K][2 + 2 n_lags] (exact integers)                                   amwg_summary_indicator_autocov
+BINDING(summary_indicator_autocov)
+  const int32_t entries = (int32_t)to_double(env, a.at(3));
+  const int32_t K = (int32_t)to_double(env, a.at(6));
+  const int32_t n_lags = (int32_t)to_double(env, a.at(8));
+  const std::vector<double> thr = doubles(env, a.at(5));
+  if (entries < 0 || K < 0 || thr.size() != (size_t)entries * (size_t)K)
+    throw Throw{"summary_indicator_autocov: thresholds must hold [entries][K] numbers"};
+  const size_t n = (size_t)entries * (size_t)K * (2 + 2 * (size_t)std::max(n_lags, 0));
+  void* data = nullptr;
+  napi_value buf, ta;
+  check(env, napi_create_arraybuffer(env, n * sizeof(int64_t), &data, &buf), "arraybuffer");
+  if (amwg_summary_indicator_autocov((int)to_double(env, a.at(0)), (const double*)(uintptr_t)to_u64(env, a.at(1)), (int64_t)to_double(env, a.at(2)),
+                                     entries, (int64_t)to_double(env, a.at(4)), thr.data(), K, (int64_t)to_double(env, a.at(7)), n_lags,
+                                     (int64_t*)data) != 0)
+    fail_from_library();
+  check(env, napi_create_typedarray(env, napi_bigint64_array, n, buf, 0, &ta), "BigInt64Array");
+  return ta;
+END_BINDING
 // summary_rank_sort(device, samples ptr, rows, entries, chains, entry, centre (NaN: bulk), keys ptr [2n], index ptr [2n])
 //   -> number of radix passes run                                                                          amwg_summary_rank_sort
 BINDING(summary_rank_sort)
@@ -658,6 +692,7 @@ NAPI_MODULE_INIT() {
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},
+      {"summary_autocov_sq", summary_autocov_sq}, {"summary_indicator_autocov", summary_indicator_autocov},
       {"summary_rank_sort", summary_rank_sort}, {"summary_rank_count", summary_rank_count}, {"summary_rank_z", summary_rank_z},
       {"summary_finite_range", summary_finite_range}, {"summary_histogram", summary_histogram}, {"summary_histogram2d", summary_histogram2d},
       {"summary_comoments", summary_comoments}, {"summary_nested", summary_nested},
