@@ -71,7 +71,8 @@ EXPORTS = ["amwg_create", "amwg_destroy", "amwg_burn", "amwg_sample", "amwg_samp
            "amwg_plate_sources", "amwg_get_term_cache", "amwg_summary_finite_range", "amwg_summary_histogram", "amwg_summary_histogram2d",
            "amwg_summary_comoments", "amwg_disperse_state_superchains", "amwg_summary_nested",
            "amwg_loo_pointwise", "amwg_loo_reduce", "amwg_loo_fit", "amwg_ppc_pointwise", "amwg_summary_threshold_counts",
-           "amwg_loo_pit_reduce", "amwg_loo_pit_fit", "amwg_summary_autocov_sq", "amwg_summary_indicator_autocov"]
+           "amwg_loo_pit_reduce", "amwg_loo_pit_fit", "amwg_summary_autocov_sq", "amwg_summary_indicator_autocov",
+           "amwg_set_ladder", "amwg_ladder_info"]
 
 _lib = None
 
@@ -108,6 +109,8 @@ def lib():
     L.amwg_checkpoint_load.argtypes = [vp, C.POINTER(vp), C.POINTER(i64), i32, i32]; L.amwg_checkpoint_load.restype = C.c_int
     L.amwg_set_adapting.argtypes = [vp, i32]; L.amwg_set_adapting.restype = C.c_int
     L.amwg_info.argtypes = [vp, vp, vp, vp]; L.amwg_info.restype = C.c_int
+    L.amwg_set_ladder.argtypes = [vp, pd, i32]; L.amwg_set_ladder.restype = C.c_int
+    L.amwg_ladder_info.argtypes = [vp, C.POINTER(u64), C.POINTER(i64)]; L.amwg_ladder_info.restype = C.c_int
     L.amwg_kernel_launches.argtypes = [vp]; L.amwg_kernel_launches.restype = i64
     L.amwg_last_sweep_kernel_ms.argtypes = [vp]; L.amwg_last_sweep_kernel_ms.restype = dbl
     L.amwg_n_chains.argtypes = [vp]; L.amwg_n_chains.restype = u64

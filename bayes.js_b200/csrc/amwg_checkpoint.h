@@ -11,7 +11,7 @@
 //   8           4       u32 format version (1)
 //   12          4       u32 P
 //   16          4       u32 D
-//   20          4       u32 reserved (0)
+//   20          4       u32 K: 0, or the rungs per ladder of a tempered handle (amwg_set_ladder, 2..256)
 //   24          8       u64 model fingerprint
 //   32          8       u64 seed
 //   40          8       u64 first_chain (global id of the image's first chain)
@@ -23,8 +23,12 @@
 //               8*C     rng_n            u64 [C]      (stream position: Math.random() calls consumed)
 //               4*D*C   acceptance count i32 [D][C]
 //               P*C     perm_ext         u8  [P][C]   (P > 16 only: the substepper order, one byte per named parameter)
+//               8*K     beta             f64 [K]      (K > 0 only: the ladder; first_chain and C are multiples of K)
+//               8       rounds           u64          (K > 0 only: swap rounds performed)
+//               8*(C/K)*(K-1)  accepts   u64 [C/K][K-1] (K > 0 only: accepted swaps per ladder and rung pair)
 //   end         8       u64 checksum (checksum() below) of bytes [0, end)
-// Per chain: 20*D + 16 bytes when P <= 16, 20*D + 8 + P when P > 16.
+// Per chain: 20*D + 16 bytes when P <= 16, 20*D + 8 + P when P > 16. An untempered image (K = 0) is the same bytes as before the
+// ladder section existed.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -127,10 +131,11 @@ inline bool binary_values_ok(const amwg_param* params, int n_params, const doubl
 // ---- layout ---------------------------------------------------------------------------------------------------------------------
 constexpr uint64_t kFixedHeader = 56;
 struct Layout {
-  uint64_t state, pls, perm, rng_n, acc, perm_ext, sum, total;    // byte offsets of the sections; perm / perm_ext: ~0 when absent
+  uint64_t state, pls, perm, rng_n, acc, perm_ext, ladder, accepts, sum, total;   // byte offsets; perm / perm_ext / ladder: ~0 when absent
 };
 constexpr uint64_t kAbsent = ~0ull;
-inline Layout layout(uint64_t D, uint64_t P, uint64_t C) {
+constexpr uint32_t kMaxRungs = 256;
+inline Layout layout(uint64_t D, uint64_t P, uint64_t C, uint64_t K = 0) {
   Layout L{};
   uint64_t o = kFixedHeader + 24 * D;
   L.state = o; o += 8 * D * C;
@@ -139,6 +144,7 @@ inline Layout layout(uint64_t D, uint64_t P, uint64_t C) {
   L.rng_n = o; o += 8 * C;
   L.acc = o; o += 4 * D * C;
   if (P > 16) { L.perm_ext = o; o += P * C; } else L.perm_ext = kAbsent;
+  if (K) { L.ladder = o; L.accepts = o + 8 * K + 8; o = L.accepts + 8 * (C / K) * (K - 1); } else L.ladder = L.accepts = kAbsent;
   L.sum = o;
   L.total = o + 8;
   return L;
@@ -151,6 +157,9 @@ struct Header {
   uint64_t fingerprint = 0, seed = 0, first_chain = 0, n_chains = 0;
   std::vector<uint64_t> is_adapting;
   std::vector<double> iter_since, batch_count;
+  uint32_t K = 0;                      // tempered ladder: K rungs with beta[K], `rounds` swap rounds performed (0: untempered)
+  std::vector<double> beta;
+  uint64_t rounds = 0;
 };
 
 inline void put_u32(uint8_t* p, uint32_t v) { std::memcpy(p, &v, 4); }
@@ -158,16 +167,22 @@ inline void put_u64(uint8_t* p, uint64_t v) { std::memcpy(p, &v, 8); }
 inline uint32_t get_u32(const uint8_t* p) { uint32_t v; std::memcpy(&v, p, 4); return v; }
 inline double get_f64(const uint8_t* p) { double v; std::memcpy(&v, p, 8); return v; }
 
-// The header of an image of layout(h.D, h.P, h.n_chains).total bytes; the arrays go to their sections (the caller's copies), then seal().
+// The header of an image of layout(h.D, h.P, h.n_chains, h.K).total bytes, and with K > 0 the ladder's beta and rounds; the arrays
+// (and the accepts) go to their sections (the caller's copies), then seal().
 inline void write_header(uint8_t* out, const Header& h) {
   std::memcpy(out, kMagic, 8);
-  put_u32(out + 8, h.version); put_u32(out + 12, h.P); put_u32(out + 16, h.D); put_u32(out + 20, 0);
+  put_u32(out + 8, h.version); put_u32(out + 12, h.P); put_u32(out + 16, h.D); put_u32(out + 20, h.K);
   put_u64(out + 24, h.fingerprint); put_u64(out + 32, h.seed); put_u64(out + 40, h.first_chain); put_u64(out + 48, h.n_chains);
   for (uint32_t c = 0; c < h.D; ++c) {
     uint8_t* r = out + kFixedHeader + 24 * (uint64_t)c;
     put_u64(r, h.is_adapting[c]);
     std::memcpy(r + 8, &h.iter_since[c], 8);
     std::memcpy(r + 16, &h.batch_count[c], 8);
+  }
+  if (h.K) {
+    const Layout L = layout(h.D, h.P, h.n_chains, h.K);
+    for (uint32_t r = 0; r < h.K; ++r) std::memcpy(out + L.ladder + 8 * (uint64_t)r, &h.beta[r], 8);
+    put_u64(out + L.ladder + 8 * (uint64_t)h.K, h.rounds);
   }
 }
 inline void seal(uint8_t* out, const Layout& L) { put_u64(out + L.sum, checksum(out, L.sum)); }
@@ -186,18 +201,22 @@ inline std::string parse(const uint8_t* p, int64_t n, View& v) {
   if (v.h.version != kVersion) return "restore: unsupported format version " + std::to_string(v.h.version) + " (this library reads version 1)";
   v.h.P = get_u32(p + 12); v.h.D = get_u32(p + 16);
   v.h.fingerprint = load_u64(p + 24); v.h.seed = load_u64(p + 32); v.h.first_chain = load_u64(p + 40); v.h.n_chains = load_u64(p + 48);
-  const uint64_t D = v.h.D, P = v.h.P, C = v.h.n_chains;
+  v.h.K = get_u32(p + 20);
+  const uint64_t D = v.h.D, P = v.h.P, C = v.h.n_chains, K = v.h.K;
   const uint64_t per = per_chain_bytes(D, P);
-  if (get_u32(p + 20) != 0 || D == 0 || D > (1u << 24) || P == 0 || P > D || C == 0 || C > ((uint64_t)1 << 40) / per ||
-      (uint64_t)n != layout(D, P, C).total)
+  if ((K != 0 && (K < 2 || K > kMaxRungs || C % K || v.h.first_chain % K)) || D == 0 || D > (1u << 24) || P == 0 || P > D || C == 0 ||
+      C > ((uint64_t)1 << 40) / per || (uint64_t)n != layout(D, P, C, K).total)
     return "restore: the image is truncated or its size does not match its header";
-  v.L = layout(D, P, C);
+  v.L = layout(D, P, C, K);
   if (load_u64(p + v.L.sum) != checksum(p, v.L.sum)) return "restore: the image is damaged (checksum mismatch)";
   v.h.is_adapting.resize(D); v.h.iter_since.resize(D); v.h.batch_count.resize(D);
   for (uint64_t c = 0; c < D; ++c) {
     const uint8_t* r = p + kFixedHeader + 24 * c;
     v.h.is_adapting[c] = load_u64(r); v.h.iter_since[c] = get_f64(r + 8); v.h.batch_count[c] = get_f64(r + 16);
   }
+  v.h.beta.resize(K);
+  for (uint64_t r = 0; r < K; ++r) v.h.beta[r] = get_f64(p + v.L.ladder + 8 * r);
+  v.h.rounds = K ? load_u64(p + v.L.ladder + 8 * K) : 0;
   v.p = p;
   return "";
 }
@@ -208,6 +227,7 @@ struct Target {
   int D = 0, P = 0;
   std::vector<amwg_param> params;
   std::vector<double> batch_size;      // per component
+  std::vector<double> beta;            // the handle's ladder (empty: untempered)
 };
 
 // Chains [dst, dst + count) of the handle (handle-local ids) come from chains [src, src + count) of image `img` (image-local ids).
@@ -228,7 +248,14 @@ inline std::string check(const std::vector<View>& views, const Target& t, std::v
     if (v.h.fingerprint != t.fingerprint || (int)v.h.D != t.D || (int)v.h.P != t.P)
       return "restore: the image was taken with a different model, data or options";
   for (const View& v : views) {
-    bool same = v.h.seed == h0.seed;
+    if (v.h.K && t.beta.empty()) return "restore: the image is of a tempered ladder (options.temperatures) and this sampler is not tempered";
+    if (!v.h.K && !t.beta.empty()) return "restore: this sampler is a tempered ladder (options.temperatures) and the image is not";
+    bool same_ladder = v.h.K == t.beta.size();
+    for (uint32_t r = 0; same_ladder && r < v.h.K; ++r) same_ladder = dbits(v.h.beta[r]) == dbits(t.beta[r]);
+    if (!same_ladder) return "restore: the image was taken with other temperatures";
+  }
+  for (const View& v : views) {
+    bool same = v.h.seed == h0.seed && v.h.rounds == h0.rounds;
     for (int c = 0; same && c < t.D; ++c)
       same = v.h.is_adapting[c] == h0.is_adapting[c] && dbits(v.h.iter_since[c]) == dbits(h0.iter_since[c]) &&
              dbits(v.h.batch_count[c]) == dbits(h0.batch_count[c]);
@@ -269,6 +296,9 @@ inline std::string check(const std::vector<View>& views, const Target& t, std::v
     pieces.clear();
     return "restore: chains [" + std::to_string(next) + ", " + std::to_string(gap_end) + ") are not covered by the images";
   }
+  const uint64_t K = t.beta.size();                 // whole ladders only (images and handles of a tempered run always hold whole ladders)
+  for (const Piece& pc : pieces)
+    if (K && (pc.src % K || pc.dst % K || pc.count % K)) { pieces.clear(); return "restore: the images split a ladder"; }
   // per chain, over the chains the handle takes
   const int D = t.D, P = t.P;
   std::vector<double> x(D);
@@ -331,6 +361,15 @@ inline void gather(const std::vector<View>& views, const std::vector<Piece>& pie
     const Span sp = span(v.L, D, P, s);
     for (uint64_t r = 0; r < sp.rows; ++r)
       std::memcpy(dst + (r * n_chains + pc.dst) * sp.width, v.p + sp.off + (r * v.h.n_chains + pc.src) * sp.width, (size_t)(pc.count * sp.width));
+  }
+}
+
+// The accepted-swap counters of a tempered handle's ladders ([n_chains / K][K - 1] u64), assembled from the pieces into dst.
+inline void gather_accepts(const std::vector<View>& views, const std::vector<Piece>& pieces, uint64_t K, uint8_t* dst) {
+  const uint64_t w = 8 * (K - 1);
+  for (const Piece& pc : pieces) {
+    const View& v = views[pc.img];
+    std::memcpy(dst + pc.dst / K * w, v.p + v.L.accepts + pc.src / K * w, (size_t)(pc.count / K * w));
   }
 }
 

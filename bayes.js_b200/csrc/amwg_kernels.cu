@@ -32,6 +32,7 @@
 #include "amwg_ld.cuh"
 #include "amwg_tma.cuh"
 #include "amwg_init.cuh"
+#include "amwg_temper.cuh"
 #include "amwg_checkpoint.h"
 
 namespace amwg {
@@ -44,6 +45,7 @@ constexpr int kStack = 32;          // operand stack of the interpreter; validat
 constexpr int kThreads = 128;       // CTA size of the per-chain kernels (one thread per chain)
 constexpr int kMinBlocks = 7;       // resident CTAs per SM the sweep kernels are compiled for (register cap)
 constexpr int kAdaptChunk = 64;
+constexpr size_t kEventPool = 256;               // event pairs a sampler keeps for timing its sweep launches (amwg_last_sweep_kernel_ms)
 constexpr long long kHostChunkSweeps = 10;       // sample() to a host buffer: sweeps per launch, so copies overlap compute at this granularity
 constexpr unsigned kSmemBudget = 200u * 1024u;   // bytes of dynamic shared memory we are willing to fill with data
 constexpr unsigned kRingStageBytes = 16u * 1024u;   // TMA tile ring for columns that do not fit: 2 stages of 16 KB (six CTAs per SM beside it)
@@ -836,8 +838,11 @@ __global__ void __launch_bounds__(kThreads) amwg_disperse_kernel(ModelDev m, Cha
 // scheduler then execute the same few hundred instructions together (instruction-cache hits instead of every warp streaming
 // the whole sweep body past the others), while the CTAs resident on one SM drift apart and overlap their fp64 loops with each
 // other's bookkeeping. Threads past the last chain shadow chain C-1 and write nothing, so they can take part in the barriers.
-template <bool CACHE>
-__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
+// TEMPER (DESIGN.md §2 "Tempered ladders"): chain g runs at beta = ld.beta[g mod K] -- every Metropolis log-ratio and the binary
+// step's two log densities are multiplied by it, curr stays the untempered log_post -- and only rung-0 chains are recorded, at
+// column (g - first_chain) / K of a [rows][n_monitor][C / K] output. The untempered instantiations do not read `ld`.
+template <bool CACHE, bool TEMPER = false>
+__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa, LadderDev ld) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -851,6 +856,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
   const unsigned long long chain = valid ? tid : C - 1;
   double* st = a.state + chain;
   const unsigned long long gchain = a.first_chain + chain;      // global chain id: the Philox counter's upper words
+  double beta = 1.0;
+  int rung = 0;
+  if constexpr (TEMPER) { rung = (int)(gchain % (unsigned long long)ld.K); beta = ld.beta[rung]; }
 
   RandomStream g;
   g.init(a.rng_n[chain]);
@@ -879,7 +887,11 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
             if (!have_der) { EvalState es{st, C, -1, 0.0}; run_ctx(ctx, es, derived_pc(m, es), der, false); have_der = true; }
             v = der[e - m.D];
           }
-          sa.out[((unsigned long long)row * sa.n_monitor + j) * C + chain] = v;
+          if constexpr (TEMPER) {
+            if (rung == 0) sa.out[((unsigned long long)row * sa.n_monitor + j) * (C / ld.K) + chain / ld.K] = v;
+          } else {
+            sa.out[((unsigned long long)row * sa.n_monitor + j) * C + chain] = v;
+          }
         }
       }
       if (rec_now) ++row;
@@ -995,7 +1007,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
               const unsigned long long ti = (unsigned long long)t * C + chain;
               lpq = lpq + (tbc[t] == cq ? a.tcand[ti] : a.tval[ti]);
             }
-            const double accept_prob = js_exp(lpq - curr);
+            const double accept_prob = js_exp(TEMPER ? beta * (lpq - curr) : lpq - curr);
             if (accept_prob > coin) {
               curr = lpq;
               if (valid) {
@@ -1011,8 +1023,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
         } else if (pa.type == AMWG_BINARY) {
           // BinaryStepper.step (mcmc.js:753-767); log_post of the current value is the cached one
           double z0raw = (cur == 0.0) ? curr : lp_new, z1raw = (cur == 0.0) ? lp_new : curr;
-          double mx = js_max(z0raw, z1raw);
-          double z0 = z0raw - mx, z1 = z1raw - mx;
+          const double t0 = TEMPER ? beta * z0raw : z0raw, t1 = TEMPER ? beta * z1raw : z1raw;   // tempered densities (curr stays untempered)
+          double mx = js_max(t0, t1);
+          double z0 = t0 - mx, z1 = t1 - mx;
           double zero_prob = js_exp(z0 - js_log(js_exp(z0) + js_exp(z1)));
           bool zero = g.next(a.seed, gchain) < zero_prob;
           const bool changed = zero != (cur == 0.0);
@@ -1025,7 +1038,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
             }
         } else if (need) {
           // Metropolis accept (mcmc.js:527-534): strict >, NaN rejects
-          double accept_prob = js_exp(lp_new - curr);
+          double accept_prob = js_exp(TEMPER ? beta * (lp_new - curr) : lp_new - curr);
           if (accept_prob > g.next(a.seed, gchain)) {
             curr = lp_new;
             if (valid) {
@@ -1061,8 +1074,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_sweep_kernel(ModelD
 // fits beside the model and the data (scratch_smem_off >= 0: small models, e.g. the headline one) it lives in SHARED memory for
 // the whole launch, one column per thread (row stride = CTA size, conflict-free): state and term cache are read from HBM once
 // per launch and written back once, the per-sweep temporaries never leave the SM. Otherwise the rows are the global arrays
-// (row stride = C), which amwg_create lays out back to back in the same order.
-__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa) {
+// (row stride = C), which amwg_create lays out back to back in the same order. TEMPER: as amwg_sweep_kernel's.
+template <bool TEMPER = false>
+__global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(ModelDev m, ChainArrays a, SweepArgs sa, LadderDev ld) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ Ctx ctx;
   __shared__ __align__(8) unsigned long long bar;
@@ -1074,6 +1088,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(M
   const unsigned long long chain = valid ? tid : C - 1;         // they take part in the CTA-wide data pass and the barriers
   const unsigned long long gchain = a.first_chain + chain;
   const int P = m.n_params, D = m.D, NT = m.n_terms;
+  double beta = 1.0;
+  int rung = 0;
+  if constexpr (TEMPER) { rung = (int)(gchain % (unsigned long long)ld.K); beta = ld.beta[rung]; }
   const bool in_smem = m.scratch_smem_off >= 0;
   // rows of the working set: wk[row * ws]; state rows: sp[c * ss]
   double* wk = in_smem ? reinterpret_cast<double*>(smem + m.scratch_smem_off) + threadIdx.x : a.tval + chain;
@@ -1112,7 +1129,11 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(M
             if (!have_der) { EvalState es{sp, ws, -1, 0.0}; run_ctx(ctx, es, derived_pc(m, es), der, false); have_der = true; }
             v = der[e - D];
           }
-          sa.out[((unsigned long long)row * sa.n_monitor + j) * C + chain] = v;
+          if constexpr (TEMPER) {
+            if (rung == 0) sa.out[((unsigned long long)row * sa.n_monitor + j) * (C / ld.K) + chain / ld.K] = v;
+          } else {
+            sa.out[((unsigned long long)row * sa.n_monitor + j) * C + chain] = v;
+          }
         }
       }
       if (rec_now) ++row;
@@ -1176,7 +1197,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) amwg_stat_sweep_kernel(M
       EvalState es{sp, ws, c, prop};
       es.tval = wk; es.tcand = wk + (unsigned long long)rTC * ws; es.tstride = ws;
       const double lp_new = eval_logpost<true>(ctx, es, ctx.comp_prog[c]);
-      const double accept_prob = js_exp(lp_new - curr);         // Metropolis accept (mcmc.js:527-534): strict >, NaN rejects
+      const double accept_prob = js_exp(TEMPER ? beta * (lp_new - curr) : lp_new - curr);   // Metropolis accept (mcmc.js:527-534): strict >, NaN rejects
       if (accept_prob > coin) {
         curr = lp_new;
         sp[(unsigned long long)c * ws] = prop;
@@ -1327,6 +1348,15 @@ struct amwg_sampler {
   std::string jit_note = "not attempted";
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pool;
   std::vector<int64_t> col_n;      // values per data column (amwg_loo_pointwise checks its program's reads against them)
+  // tempered ladder (amwg_set_ladder, DESIGN.md §2 "Tempered ladders"): K > 0 when set
+  int K = 0;
+  std::vector<double> beta;        // [K] 1 / T_r
+  double* d_beta = nullptr;
+  unsigned long long* d_swap_acc = nullptr;   // [C / K][K - 1] accepted swaps per ladder and rung pair
+  uint64_t rounds = 0;             // swap rounds performed
+  bool moved = false;              // a sweep, dispersal, set_state or restore has run: the ladder can no longer be set
+  LadderDev ladder() const { return LadderDev{d_beta, K}; }
+  unsigned long long recorded_chains() const { return K ? a.C / (unsigned long long)K : a.C; }   // columns of a sample row
 };
 
 template <typename T>
@@ -1699,7 +1729,10 @@ extern "C" int amwg_create(const amwg_model* md, uint64_t n_chains, uint64_t fir
   s->smem_bytes = smem_used;
   if (cudaFuncSetAttribute(amwg_sweep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_sweep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
-      cudaFuncSetAttribute(amwg_stat_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
+      cudaFuncSetAttribute(amwg_stat_sweep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
+      cudaFuncSetAttribute(amwg_sweep_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
+      cudaFuncSetAttribute(amwg_sweep_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
+      cudaFuncSetAttribute(amwg_stat_sweep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_relp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
       cudaFuncSetAttribute(amwg_disperse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget) != cudaSuccess ||
@@ -1764,6 +1797,7 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
   const unsigned long long C = s->a.C;
   long long i0 = 0;
   size_t n_events = 0;
+  double ms = 0.0;                                 // sweep-kernel time of the launches already folded in
   long long rows_copied = 0;
   while (i0 < n) {
     long long L = n - i0;
@@ -1776,7 +1810,17 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
     if (record && host_out && L > kHostChunkSweeps) L = kHostChunkSweeps;   // finer launches: the D2H of finished rows trails the sweeps closely
     // ... and the last launches taper off (.., 10, 5, 3, 2), because the copy of the final launch's rows is the one that nothing hides
     if (record && host_out && n - i0 <= kHostChunkSweeps && L > 2) L = std::min(L, std::max<long long>(2, (n - i0 + 1) / 2));
+    if (s->K) L = 1;                                                          // a tempered ladder swaps after every sweep
     SweepArgs sa{L, i0, thin, record, n_monitor, d_monitor, d_out};
+    if (n_events == kEventPool) {                  // fold the finished launches' times in, so the pool stays bounded (one launch per
+      CUDA_TRY(cudaEventSynchronize(s->ev_pool[n_events - 1].second));     // sweep on a tempered handle)
+      for (size_t k = 0; k < n_events; ++k) {
+        float t = 0.f;
+        CUDA_TRY(cudaEventElapsedTime(&t, s->ev_pool[k].first, s->ev_pool[k].second));
+        ms += t;
+      }
+      n_events = 0;
+    }
     if (n_events >= s->ev_pool.size()) {
       cudaEvent_t e0, e1;
       CUDA_TRY(cudaEventCreate(&e0)); CUDA_TRY(cudaEventCreate(&e1));
@@ -1789,15 +1833,31 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
       for (int k = 0; k < kMaxColumns; ++k) ja.col[k] = k < s->m.n_columns ? s->m.col_global[k] : nullptr;
       void* kargs[] = {&ja};
       CUDA_TRY(cudaLaunchKernel((const void*)s->jit_kernel, dim3(grid_for(C, s->jit_threads)), dim3((unsigned)s->jit_threads), kargs, s->jit_smem, s->stream));
+    } else if (s->K) {
+      const dim3 grid(grid_for(C, kThreads));
+      if (s->m.stat_prog >= 0) amwg_stat_sweep_kernel<true><<<grid, kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
+      else if (s->m.n_terms > 0) amwg_sweep_kernel<true, true><<<grid, kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
+      else amwg_sweep_kernel<false, true><<<grid, kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
     } else {
-      if (s->m.stat_prog >= 0) amwg_stat_sweep_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
-      else if (s->m.n_terms > 0) amwg_sweep_kernel<true><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
-      else amwg_sweep_kernel<false><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa);
+      if (s->m.stat_prog >= 0) amwg_stat_sweep_kernel<<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
+      else if (s->m.n_terms > 0) amwg_sweep_kernel<true><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
+      else amwg_sweep_kernel<false><<<grid_for(C, kThreads), kThreads, s->smem_bytes, s->stream>>>(s->m, s->a, sa, s->ladder());
     }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(s->ev_pool[n_events].second, s->stream));
     n_events++;
     s->launches++;
+    s->moved = true;
+    if (s->K) {                     // the swap round of this sweep; the adaptation below touches none of its arrays
+      const unsigned long long pairs = (C / (unsigned long long)s->K) * (unsigned long long)swap_pairs(s->K, s->rounds);
+      if (pairs) {
+        amwg_swap_kernel<<<grid_for(pairs, 256), 256, 0, s->stream>>>(s->a.state, s->a.curr_lp, s->a.tval, s->D, s->m.n_terms, C, s->a.first_chain, s->a.seed,
+                                                                    s->ladder(), (unsigned long long)s->rounds, s->d_swap_acc);
+        CUDA_TRY(cudaGetLastError());
+        s->launches++;
+      }
+      s->rounds++;
+    }
 
     // chain-invariant bookkeeping of OnedimMetropolisStepper (mcmc.js:536-551)
     bool any = false;
@@ -1838,7 +1898,7 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
       if (rows_done > rows_copied) {
         cudaEvent_t done = s->ev_pool[n_events - 1].second;
         CUDA_TRY(cudaStreamWaitEvent(s->copy_stream, done, 0));
-        size_t row_elems = (size_t)n_monitor * (size_t)C;
+        size_t row_elems = (size_t)n_monitor * (size_t)s->recorded_chains();
         CUDA_TRY(cudaMemcpyAsync(host_out + (size_t)rows_copied * row_elems, d_out + (size_t)rows_copied * row_elems,
                                  (size_t)(rows_done - rows_copied) * row_elems * sizeof(double), cudaMemcpyDeviceToHost, s->copy_stream));
         rows_copied = rows_done;
@@ -1847,7 +1907,6 @@ static int run_sweeps(amwg_sampler* s, long long n, int record, long long thin, 
   }
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   if (record && host_out) CUDA_TRY(cudaStreamSynchronize(s->copy_stream));
-  double ms = 0.0;
   for (size_t k = 0; k < n_events; ++k) {
     float t = 0.f;
     CUDA_TRY(cudaEventElapsedTime(&t, s->ev_pool[k].first, s->ev_pool[k].second));
@@ -1897,7 +1956,7 @@ extern "C" int amwg_sample(amwg_sampler* s, int64_t n, int64_t thin, const int32
   if (n == 0) { s->last_sweep_ms = 0.0; return 0; }
   if (n_monitor > 0 && !host_out) return fail("amwg_sample: host_out is NULL");
   size_t rows = (size_t)((n + thin - 1) / thin);
-  size_t bytes = rows * (size_t)n_monitor * (size_t)s->a.C * sizeof(double);
+  size_t bytes = rows * (size_t)n_monitor * (size_t)s->recorded_chains() * sizeof(double);
   if (bytes > s->d_out_bytes) {
     if (s->d_out) cudaFree(s->d_out);
     s->d_out = nullptr; s->d_out_bytes = 0;
@@ -1956,6 +2015,7 @@ extern "C" int amwg_set_state(amwg_sampler* s, const double* host_in) {
   if (!s || !host_in) return fail("amwg_set_state: NULL argument");
   if (check_binary_values(s->params.data(), s->P, host_in, (size_t)s->a.C, "amwg_set_state")) return -1;
   CUDA_TRY(cudaSetDevice(s->device));
+  s->moved = true;
   return commit_state(s, host_in, cudaMemcpyHostToDevice);
 }
 
@@ -1969,6 +2029,7 @@ extern "C" int amwg_disperse_state_superchains(amwg_sampler* s, double radius, i
   if (!(radius > 0.0) || radius == INFINITY) return fail("amwg_disperse_state: radius must be finite and > 0");
   if (superchain_size < 1) return fail("amwg_disperse_state: superchain_size must be >= 1");
   CUDA_TRY(cudaSetDevice(s->device));
+  s->moved = true;
   const unsigned long long C = s->a.C;
   double* d_x = nullptr;
   unsigned char* d_done = nullptr;
@@ -2013,20 +2074,24 @@ extern "C" int amwg_model_fingerprint(const amwg_model* md, uint64_t* out) {
 
 extern "C" int amwg_checkpoint_size(amwg_sampler* s, int64_t* out) {
   if (!s || !out) return fail("amwg_checkpoint_size: NULL argument");
-  *out = (int64_t)ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C).total;
+  *out = (int64_t)ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C, (uint64_t)s->K).total;
   return 0;
 }
 
 extern "C" int amwg_checkpoint_save(amwg_sampler* s, uint8_t* host_out, int64_t cap) {
   if (!s || !host_out) return fail("amwg_checkpoint_save: NULL argument");
-  const ckpt::Layout L = ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C);
+  const ckpt::Layout L = ckpt::layout((uint64_t)s->D, (uint64_t)s->P, s->a.C, (uint64_t)s->K);
   if (cap < (int64_t)L.total) return fail("amwg_checkpoint_save: the buffer holds " + std::to_string(cap) + " bytes, the image needs " + std::to_string(L.total));
   CUDA_TRY(cudaSetDevice(s->device));
   ckpt::Header h;
   h.P = (uint32_t)s->P; h.D = (uint32_t)s->D; h.fingerprint = s->fingerprint; h.seed = s->a.seed; h.first_chain = s->a.first_chain; h.n_chains = s->a.C;
   h.is_adapting.assign(s->is_adapting.begin(), s->is_adapting.end());
   h.iter_since = s->iter_since; h.batch_count = s->batch_count;
+  h.K = (uint32_t)s->K; h.beta = s->beta; h.rounds = s->rounds;
   ckpt::write_header(host_out, h);
+  if (s->K)
+    CUDA_TRY(cudaMemcpyAsync(host_out + L.accepts, s->d_swap_acc, sizeof(unsigned long long) * (size_t)(s->a.C / (uint64_t)s->K) * (size_t)(s->K - 1),
+                             cudaMemcpyDeviceToHost, s->stream));
   const void* src[ckpt::kSections] = {s->a.state, s->a.pls, s->a.perm, s->a.rng_n, s->a.acc, s->a.perm_ext};
   for (int k = 0; k < ckpt::kSections; ++k) {
     const ckpt::Span sp = ckpt::span(L, s->D, s->P, (ckpt::Section)k);
@@ -2050,6 +2115,7 @@ extern "C" int amwg_checkpoint_load(amwg_sampler* s, const uint8_t* const* image
   ckpt::Target t;
   t.fingerprint = s->fingerprint; t.first_chain = s->a.first_chain; t.n_chains = s->a.C; t.D = s->D; t.P = s->P;
   t.params = s->params;
+  t.beta = s->beta;
   t.batch_size.resize(s->D);
   for (int c = 0; c < s->D; ++c) t.batch_size[c] = s->opts[c].batch_size;
   std::vector<ckpt::Piece> pieces;
@@ -2058,6 +2124,7 @@ extern "C" int amwg_checkpoint_load(amwg_sampler* s, const uint8_t* const* image
   if (dry_run) return 0;
 
   CUDA_TRY(cudaSetDevice(s->device));
+  s->moved = true;
   const unsigned long long C = s->a.C;
   void* dst[ckpt::kSections] = {s->a.state, s->a.pls, s->a.perm, s->a.rng_n, s->a.acc, s->a.perm_ext};
   for (int k = 0; k < ckpt::kSections; ++k)
@@ -2069,6 +2136,13 @@ extern "C" int amwg_checkpoint_load(amwg_sampler* s, const uint8_t* const* image
                                  pc.count * sp.width, sp.rows, cudaMemcpyHostToDevice, s->stream));
     }
   const ckpt::Header& h = views[0].h;
+  if (s->K) {                       // the ladders' accepted-swap counters, and the round counter
+    const uint64_t K = (uint64_t)s->K, w = K - 1;
+    for (const ckpt::Piece& pc : pieces)
+      CUDA_TRY(cudaMemcpyAsync(s->d_swap_acc + pc.dst / K * w, views[pc.img].p + views[pc.img].L.accepts + pc.src / K * w * 8,
+                               (size_t)(pc.count / K * w * 8), cudaMemcpyHostToDevice, s->stream));
+    s->rounds = h.rounds;
+  }
   s->a.seed = h.seed;
   for (int c = 0; c < s->D; ++c) { s->is_adapting[c] = (unsigned char)h.is_adapting[c]; s->iter_since[c] = h.iter_since[c]; s->batch_count[c] = h.batch_count[c]; }
   CUDA_TRY(cudaMemcpyAsync(s->d_adapting, s->is_adapting.data(), (size_t)s->D, cudaMemcpyHostToDevice, s->stream));
@@ -2104,6 +2178,48 @@ extern "C" int amwg_info(amwg_sampler* s, double* scalars, double* prop_log_scal
   if (acceptance_count) CUDA_TRY(cudaMemcpyAsync(acceptance_count, s->a.acc, sizeof(int) * DC, cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   return 0;
+}
+
+// ---- tempered ladders (DESIGN.md §2 "Tempered ladders") -------------------------------------------------------------------------
+extern "C" int amwg_set_ladder(amwg_sampler* s, const double* beta, int32_t K) {
+  if (!s || !beta) return fail("amwg_set_ladder: NULL argument");
+  if (s->K) return fail("amwg_set_ladder: the handle already has a ladder");
+  if (s->moved) return fail("amwg_set_ladder: the chains have moved; set the ladder right after amwg_create");
+  if (K < 2 || K > kMaxRungs) return fail("amwg_set_ladder: a ladder has between 2 and 256 rungs");
+  if (beta[0] != 1.0) return fail("amwg_set_ladder: beta[0] must be 1");
+  for (int r = 1; r < K; ++r)
+    if (!(beta[r] > 0.0 && beta[r] < beta[r - 1])) return fail("amwg_set_ladder: beta must be positive and strictly decreasing");
+  if (s->a.C % (uint64_t)K || s->a.first_chain % (uint64_t)K)
+    return fail("amwg_set_ladder: the handle's first chain and chain count must be multiples of K (no ladder may straddle two handles)");
+  CUDA_TRY(cudaSetDevice(s->device));
+  const size_t n_acc = (size_t)(s->a.C / (uint64_t)K) * (size_t)(K - 1);
+  double* d_beta = nullptr;
+  unsigned long long* d_acc = nullptr;
+  if (dev_upload(s, beta, (size_t)K, &d_beta) || dev_alloc(s, n_acc, &d_acc)) return -1;
+  CUDA_TRY(cudaMemsetAsync(d_acc, 0, sizeof(unsigned long long) * n_acc, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  s->K = K; s->beta.assign(beta, beta + K); s->d_beta = d_beta; s->d_swap_acc = d_acc; s->rounds = 0;
+  s->jit_kernel = nullptr;        // tempered sweeps run on the interpreter kernels
+  s->jit_note = "tempered ladder (options.temperatures): interpreter kernels";
+  return 0;
+}
+
+// rounds performed, and accepted swaps summed over the handle's ladders per rung pair (accepts: [K - 1]); returns K, 0 untempered
+extern "C" int amwg_ladder_info(amwg_sampler* s, uint64_t* rounds, int64_t* accepts) {
+  if (!s) return fail("amwg_ladder_info: NULL handle");
+  if (rounds) *rounds = s->rounds;
+  if (!s->K) return 0;
+  if (accepts) {
+    CUDA_TRY(cudaSetDevice(s->device));
+    const size_t ladders = (size_t)(s->a.C / (uint64_t)s->K), w = (size_t)(s->K - 1);
+    std::vector<unsigned long long> per(ladders * w);
+    CUDA_TRY(cudaMemcpyAsync(per.data(), s->d_swap_acc, sizeof(unsigned long long) * per.size(), cudaMemcpyDeviceToHost, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+    for (size_t r = 0; r < w; ++r) accepts[r] = 0;
+    for (size_t l = 0; l < ladders; ++l)
+      for (size_t r = 0; r < w; ++r) accepts[r] += (int64_t)per[l * w + r];
+  }
+  return s->K;
 }
 
 // 1 when the handle runs the run-time specialised sweep, 0 when it runs the interpreter kernels; `note` says what was built or why not

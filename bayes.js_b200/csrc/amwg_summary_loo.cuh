@@ -390,7 +390,7 @@ extern "C" int amwg_loo_pointwise(amwg_sampler* s, const int32_t* host_code, int
   if (stage_pointwise_program(s, sc, who, (const void*)summary::amwg_loo_pointwise_kernel, smem, host_code, n_code, host_consts, n_consts,
                               host_fold_prog, host_fold_dst, n_fold, &d_code, &d_consts, &d_cols))
     return -1;
-  const long long C = (long long)s->a.C;
+  const long long C = (long long)s->recorded_chains();      // the block's chain axis: the cold chains of a tempered ladder
   const dim3 grid((unsigned)((C + kThreads - 1) / kThreads), (unsigned)std::min<int64_t>(rows, 65535), (unsigned)((rows + 65534) / 65535));
   summary::amwg_loo_pointwise_kernel<<<grid, kThreads, smem>>>(d_code, n_code, d_consts, n_consts, body_prog, d_cols, dev_samples, entries, rows,
                                                                C, (int)p0, n_points, dev_out);

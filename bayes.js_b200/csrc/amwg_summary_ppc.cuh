@@ -100,6 +100,7 @@ extern "C" int amwg_ppc_pointwise(amwg_sampler* s, const int32_t* host_code, int
                                   int64_t points, int64_t p0, int32_t n_points, double* dev_out, double* dev_stats) {
   const char* who = "amwg_ppc_pointwise";
   if (!s) return fail("amwg_ppc_pointwise: NULL handle");
+  if (s->K) return fail("amwg_ppc_pointwise: predictive checks of tempered ladders (options.temperatures) are not supported yet");
   if (!host_code || !host_consts || !host_arg_progs || !dev_samples || !dev_out || !dev_stats || (n_fold > 0 && (!host_fold_prog || !host_fold_dst)))
     return fail("amwg_ppc_pointwise: null pointer");
   if (family < 0 || family >= ppc::kFamilies) return fail("amwg_ppc_pointwise: unknown family");

@@ -13,8 +13,10 @@ shaped exactly like the reference's), ``seed``, ``device``, ``distributed``, ``f
 the first chain, default 0), ``faithful`` (no factorised likelihood plates: bit-faithful, slower),
 ``init_radius`` (over-dispersed starting points drawn on the device, DESIGN.md §2; default: every chain
 starts at the params' init), ``superchain_size`` (chains per superchain: with ``init_radius`` the chains of a
-superchain start at one point, and ``sample_summary(n, nested=True)`` uses it; DESIGN.md §4.6). ``sampler.set_state(values)`` places the chains anywhere; ``sampler.checkpoint()`` and
-``sampler.restore(images)`` stop and resume a run bit for bit.
+superchain start at one point, and ``sample_summary(n, nested=True)`` uses it; DESIGN.md §4.6), ``temperatures`` (parallel
+tempering: ladders of K neighbouring chains at temperatures T_0 = 1 < ... < T_{K-1} that swap states after every sweep, so that
+multimodal posteriors are sampled; sample() and sample_summary() return the T = 1 chains; DESIGN.md §2). ``sampler.set_state(values)``
+places the chains anywhere; ``sampler.checkpoint()`` and ``sampler.restore(images)`` stop and resume a run bit for bit.
 """
 from __future__ import annotations
 
@@ -249,6 +251,30 @@ def rnorm(mean, sd):
 
 
 DISPERSE_ATTEMPTS = 100         # csrc/amwg_init.cuh kDisperseAttempts
+MAX_RUNGS = 256                 # csrc/amwg_temper.cuh kMaxRungs
+
+
+def ladder_betas(temperatures, n_chains: int) -> List[float]:
+    """options.temperatures -> [beta_r = 1.0 / T_r], one IEEE division each: the doubles the device and the reference use. Raises
+    unless there are 2..256 finite temperatures, T_0 = 1, strictly increasing, whose count K divides options.chains (global chain
+    g is rung g mod K of ladder g // K, DESIGN.md §2 "Tempered ladders")."""
+    if isinstance(temperatures, (str, bytes, dict)) or not hasattr(temperatures, "__len__"):
+        raise JsThrow("options.temperatures must be a list of numbers")
+    temps = list(np.asarray(temperatures, dtype=object).reshape(-1)) if isinstance(temperatures, np.ndarray) else list(temperatures)
+    if not all(is_number(t) for t in temps):
+        raise JsThrow("options.temperatures must be a list of numbers")
+    temps = [float(t) for t in temps]
+    if not 2 <= len(temps) <= MAX_RUNGS:
+        raise JsThrow("options.temperatures must have between 2 and %d entries" % MAX_RUNGS)
+    if not all(math.isfinite(t) for t in temps):
+        raise JsThrow("options.temperatures must be finite")
+    if temps[0] != 1.0:
+        raise JsThrow("options.temperatures must start at 1")
+    if not all(a < b for a, b in zip(temps, temps[1:])):
+        raise JsThrow("options.temperatures must be strictly increasing")
+    if n_chains % len(temps):
+        raise JsThrow("options.temperatures: their number must divide options.chains")
+    return [1.0 / t for t in temps]
 
 
 def dispersal_failure_message(n_failed: int, n_chains: int, distributed: bool = False, device: int = 0) -> Optional[str]:
@@ -398,6 +424,12 @@ class AmwgSampler(Sampler):
             if self.n_chains % int(size):
                 raise JsThrow("options.superchain_size must divide options.chains")
         self.superchain_size = None if size is None else int(size)
+        temps = get_option("temperatures", options, None)                 # parallel tempering (DESIGN.md §2 "Tempered ladders")
+        self.betas = None if temps is None else ladder_betas(temps, self.n_chains)
+        self.temperatures = None if temps is None else [float(t) for t in temps]
+        if self.betas is not None and self.superchain_size is not None:
+            raise JsThrow("options.superchain_size cannot be combined with options.temperatures: superchains of tempered chains are not defined")
+        K = 1 if self.betas is None else len(self.betas)
 
         # flat component layout: Object.keys(params) order, row-major inside a parameter
         self._offsets: Dict[str, int] = {}
@@ -413,8 +445,14 @@ class AmwgSampler(Sampler):
         # shard the chains when running one process per GPU (torch.distributed, see parallel.py)
         self.first_chain, self.local_chains = int(get_option("first_chain", options, 0)), self.n_chains
         if self.distributed:
-            from .parallel import shard_chains
+            from .parallel import check_ladder_shards, shard_chains
             self.first_chain, self.local_chains = shard_chains(self.n_chains)
+            if self.betas is not None:
+                check_ladder_shards(self.n_chains, K)
+        elif self.betas is not None and self.first_chain % K:
+            raise JsThrow("options.first_chain must be a multiple of the number of temperatures")
+        # the chains sample() and sample_summary() return: all of them, or the T = 1 rung of every ladder
+        self.cold_chains, self.local_cold = self.n_chains // K, self.local_chains // K
 
         self._build_model(resolved)
         return ["AmwgStepper"]
@@ -504,6 +542,12 @@ class AmwgSampler(Sampler):
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
         self._handle = h
+        if self.betas is not None:
+            b = np.asarray(self.betas, dtype=np.float64)
+            if L.amwg_set_ladder(h, b.ctypes.data_as(C.POINTER(C.c_double)), b.size) != 0:
+                err = L.amwg_last_error().decode()
+                self.close()
+                raise JsThrow(err)
         if self.init_radius is not None:
             self._disperse(self.init_radius)
 
@@ -544,13 +588,14 @@ class AmwgSampler(Sampler):
             return [self.n_comp + self._derived_names.index(name)]
         return []          # JS: state[name] is undefined -> the column is filled with undefined
 
-    def _shape_out(self, name: str, arr: np.ndarray) -> np.ndarray:
-        """arr: [rows, entries, chains] -> reference-shaped array ([rows, *dim] for one chain, else [rows, chains, *dim])."""
+    def _shape_out(self, name: str, arr: np.ndarray, chains_total: Optional[int] = None) -> np.ndarray:
+        """arr: [rows, entries, chains] -> reference-shaped array ([rows, *dim] for one chain, else [rows, chains, *dim]); one chain
+        means `chains_total` chains in all (default options.chains; sample() passes the cold chains of a tempered sampler)."""
         rows, _, chains = arr.shape
         dim = self.params[name]["dim"] if name in self.params else [1]
         a = np.moveaxis(arr, 1, 2)                        # [rows, chains, entries]
         a = a.reshape(rows, chains) if list(dim) == [1] else a.reshape(rows, chains, *dim)
-        return a[:, 0] if self.n_chains == 1 else a
+        return a[:, 0] if (self.n_chains if chains_total is None else chains_total) == 1 else a
 
     # -- the reference's methods -----------------------------------------------------------------
     def step(self):
@@ -681,7 +726,7 @@ class AmwgSampler(Sampler):
             if ln == 0:
                 out[name] = np.full((rows,), np.nan)
             else:
-                out[name] = self._shape_out(name, raw[:, s:s + ln, :])
+                out[name] = self._shape_out(name, raw[:, s:s + ln, :], self.cold_chains)
         return out
 
     def _sample_raw(self, n: int, thin: int, entries: List[int], rows: int) -> np.ndarray:
@@ -690,7 +735,7 @@ class AmwgSampler(Sampler):
         if self.distributed:
             from .parallel import sample_and_gather
             return sample_and_gather(self, n, thin, mon, rows)
-        buf = _pinned_empty((rows, len(entries), self.local_chains))
+        buf = _pinned_empty((rows, len(entries), self.local_cold))
         rc = L.amwg_sample(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(entries), buf.ctypes.data)
         if rc != 0:
             raise JsThrow(L.amwg_last_error().decode())
@@ -837,13 +882,18 @@ class AmwgSampler(Sampler):
         superchain = resolve_nested(nested, self.superchain_size, first, held)
         loo_plan = resolve_loo(loo, named)
         ppc_plan = resolve_ppc(ppc, named)
+        if self.betas is not None and superchain is not None:
+            raise ValueError("nested= is not available with options.temperatures: superchains of tempered chains are not defined")
+        if self.betas is not None and ppc_plan is not None:
+            raise ValueError("ppc= is not available with options.temperatures: its stream positions are defined per chain id")
+        n_chains, local_chains = self.cold_chains, self.local_cold      # the block's chain axis: the T = 1 chains
         n = int(n_iterations)
         thin = abs(int(self.thinning_interval))
         rows = 0 if (n <= 0 or thin == 0) else (n + thin - 1) // thin
         if rows == 0 or not entries:
             raise JsThrow("sample_summary needs at least one kept iteration and one monitored entry")
         if mcse:
-            check_mcse_size(rows, self.n_chains)
+            check_mcse_size(rows, n_chains)
         sampled = list(entries)                                 # the block's entries: the monitored ones, then what log_lik reads besides
         start = {}
 
@@ -858,12 +908,12 @@ class AmwgSampler(Sampler):
                     sampled.extend(self._entries(name))
         if loo_plan is not None:
             from .tracer import trace_log_lik
-            loo_m = check_loo_size(rows * self.n_chains, loo_plan.r_eff)
+            loo_m = check_loo_size(rows * n_chains, loo_plan.r_eff)
             lik = trace_log_lik(loo_plan.log_lik, self.params, self._offsets, self.data, loo_plan.points)
         if ppc_plan is not None:
             from .tracer import trace_log_lik
             if ppc_plan.loo_pit is not None:
-                pit_m = check_loo_size(rows * self.n_chains, ppc_plan.loo_pit, "ppc loo_pit")
+                pit_m = check_loo_size(rows * n_chains, ppc_plan.loo_pit, "ppc loo_pit")
             ppc_lik = trace_log_lik(ppc_plan.log_lik, self.params, self._offsets, self.data, ppc_plan.points, what="ppc")
             ppc_family, ppc_y, ppc_args = ppc_lik.observed_call(ppc_plan.points)
             ppc_code = check_ppc_call(ppc_family, rows, ppc_plan.points)
@@ -877,30 +927,30 @@ class AmwgSampler(Sampler):
                 pit_prog = ppc_lik.lower(start)                   # the log-likelihood of the same ld.* call, as loo= lowers its body
         L = _ffi.lib()
         dev = torch.device("cuda", self.device)
-        need = rows * len(sampled) * self.local_chains * 8
+        need = rows * len(sampled) * local_chains * 8
         if len(sampled) > len(entries):
-            need += rows * len(entries) * self.local_chains * 8         # the monitored entries' block, copied out after the loo / ppc pass
+            need += rows * len(entries) * local_chains * 8         # the monitored entries' block, copied out after the loo / ppc pass
         if ppc_plan is not None:
-            need += ppc_fixed_bytes(rows, self.local_chains)
+            need += ppc_fixed_bytes(rows, local_chains)
         if plan is not None:
             # edges and counts of the histograms, and the extremes (8 B each)
             nb, pb = plan.bins or 0, plan.pair_bins
             need += 8 * (len(entries) * (2 * nb + 4 + pb + 1 + 5) + len(plan.pairs) * pb * pb)
         if cov_plan is not None:
-            need += comoments_scratch_bytes(len(cov_plan.entries), self.local_chains)
+            need += comoments_scratch_bytes(len(cov_plan.entries), local_chains)
         if superchain is not None:
-            need += nested_scratch_bytes(len(entries), self.local_chains, self.first_chain, superchain)
+            need += nested_scratch_bytes(len(entries), local_chains, self.first_chain, superchain)
         if mcse:
             need += mcse_scratch_bytes(len(entries), len(probs))
         free, _total = torch.cuda.mem_get_info(dev)
-        base = need + 2 * len(entries) * self.local_chains * 8      # and the base summary's scratch: two doubles per entry and chain
+        base = need + 2 * len(entries) * local_chains * 8      # and the base summary's scratch: two doubles per entry and chain
         if base > 0.9 * free:
             raise JsThrow("sample_summary: the sample block (%.1f GB) does not fit in device memory; raise thin() or lower n" % (need / 1e9))
         if diagnostics == "rank" and rows >= 10:
             # rank_diagnostics, per entry: keys 2 x 8 B, indices 2 x 4 B, rank sums 8 B, a ring buffer 8 B and two z-blocks 2 x 8 B per
             # ranked draw (the ring buffers hold the largest shard, at most one chain more than this one), and the sort's tile
             # tables (2 x 256 x 4 B per 2048 keys)
-            ranked = 2 * (rows // 2) * (self.local_chains + (1 if self.distributed else 0))
+            ranked = 2 * (rows // 2) * (local_chains + (1 if self.distributed else 0))
             scratch = 56 * ranked + 2 * 256 * 4 * (-(-ranked // 2048))
             if base + scratch > 0.9 * free:
                 raise JsThrow("sample_summary: the sample block (%.1f GB) and the scratch of diagnostics=\"rank\" (%.1f GB) do not fit in "
@@ -918,14 +968,14 @@ class AmwgSampler(Sampler):
             return chunk_points
         world = torch.distributed.get_world_size() if self.distributed else 1
         if loo_plan is not None:
-            chunk_points = chunk_size(loo_point_bytes(rows, self.local_chains, loo_tail_cap(loo_m), world), loo_plan.points,
+            chunk_points = chunk_size(loo_point_bytes(rows, local_chains, loo_tail_cap(loo_m), world), loo_plan.points,
                                       "pointwise log-likelihood")
         if ppc_plan is not None:
-            per_point = ppc_point_bytes(rows, self.local_chains)
+            per_point = ppc_point_bytes(rows, local_chains)
             if ppc_plan.loo_pit is not None:                      # LOO-PIT holds a chunk of ll beside the chunk of y_rep
-                per_point += loo_pit_point_bytes(rows, self.local_chains, loo_tail_cap(pit_m), world)
+                per_point += loo_pit_point_bytes(rows, local_chains, loo_tail_cap(pit_m), world)
             ppc_chunk = chunk_size(per_point, ppc_plan.points, "replicated data")
-        block = torch.empty((rows, len(sampled), self.local_chains), dtype=torch.float64, device=dev)
+        block = torch.empty((rows, len(sampled), local_chains), dtype=torch.float64, device=dev)
         mon = np.asarray(sampled, dtype=np.int32)
         torch.cuda.current_stream(dev).synchronize()   # the library writes `block` on its own stream: torch's queued work goes first
         rc = L.amwg_sample_device(self._handle, n, thin, mon.ctypes.data_as(C.POINTER(C.c_int32)), len(sampled), block.data_ptr())
@@ -934,23 +984,23 @@ class AmwgSampler(Sampler):
         reducer = CudaBlockReducer(self.device)
         loo_out = None
         if loo_plan is not None:
-            loo_out = loo_block(reducer, CudaPointwise(self._handle, loo_prog, block, self.device), rows, self.n_chains, loo_plan.points,
+            loo_out = loo_block(reducer, CudaPointwise(self._handle, loo_prog, block, self.device), rows, n_chains, loo_plan.points,
                                 loo_plan.r_eff, chunk_points, self.distributed)
         ppc_out = None
         if ppc_plan is not None:
             pit = None
             if ppc_plan.loo_pit is not None:
                 pit = (CudaPointwise(self._handle, pit_prog, block, self.device), ppc_plan.loo_pit)
-            ppc_out = ppc_block(reducer, CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points), rows, self.n_chains,
+            ppc_out = ppc_block(reducer, CudaPpc(self._handle, ppc_prog, ppc_offs, ppc_code, block, ppc_plan.points), rows, n_chains,
                                 ppc_plan.points, ppc_family, ppc_y, probs, ppc_chunk, self.distributed, loo_pit=pit)
         if len(sampled) > len(entries):
             block = block[:, :len(entries)].contiguous()
-        res = summarise_block(reducer, block, rows, self.n_chains, probs, self.distributed, diagnostics)
+        res = summarise_block(reducer, block, rows, n_chains, probs, self.distributed, diagnostics)
         mean, sd, rhat, q = res[:4]
         hist = None if plan is None else histogram_block(reducer, block, rows, plan, self.distributed)
         cov = None if cov_plan is None else covariance_block(reducer, block, rows, cov_plan, self.distributed)
         rn = None if superchain is None else nested_block(reducer, block, rows, self.first_chain, superchain, self.distributed)
-        mc = mcse_block(reducer, block, rows, self.n_chains, probs, mean, sd, q, self.distributed) if mcse else None
+        mc = mcse_block(reducer, block, rows, n_chains, probs, mean, sd, q, self.distributed) if mcse else None
         del block
         out = {}
         for name in monitored:
@@ -961,7 +1011,7 @@ class AmwgSampler(Sampler):
             shape = (lambda a: float(a[0])) if dim == [1] else (lambda a, dim=dim: np.asarray(a).reshape(*dim))
             out[name] = {"mean": shape(mean[s0:s0 + ln]), "sd": shape(sd[s0:s0 + ln]), "rhat": shape(rhat[s0:s0 + ln]),
                          "quantiles": q[:, s0] if dim == [1] else q[:, s0:s0 + ln].reshape(len(q), *dim),
-                         "n_draws": rows * self.n_chains}
+                         "n_draws": rows * n_chains}
             if diagnostics:
                 for key, val in res[4][0].items():
                     out[name][key] = shape(val[s0:s0 + ln])
@@ -1024,8 +1074,27 @@ class AmwgSampler(Sampler):
                 "iterations_since_adaption": invariant([scal[c * 3 + 1] for c in e]),
                 "batch_count": invariant([scal[c * 3 + 2] for c in e]),
             }
-        return {"state": self.state, "thin": self.thinning_interval, "monitor": self.monitored_params,
-                "steppers": [per_param]}
+        out = {"state": self.state, "thin": self.thinning_interval, "monitor": self.monitored_params,
+               "steppers": [per_param]}
+        if self.betas is not None:
+            out["tempering"] = self._tempering_info()
+        return out
+
+    def _tempering_info(self) -> Dict[str, Any]:
+        """options.temperatures: the swap rounds so far and, per rung pair (r, r + 1), the swaps accepted and attempted over this
+        handle's ladders (round k attempts the pairs r = k mod 2)."""
+        K = len(self.betas)
+        rounds = C.c_uint64(0)
+        acc = np.zeros(K - 1, dtype=np.int64)
+        L = _ffi.lib()
+        if L.amwg_ladder_info(self._handle, C.byref(rounds), acc.ctypes.data_as(C.POINTER(C.c_int64))) < 0:
+            raise JsThrow(L.amwg_last_error().decode())
+        k = int(rounds.value)
+        ladders = self.local_chains // K
+        att = np.asarray([ladders * ((k + 1 - (r & 1)) // 2) for r in range(K - 1)], dtype=np.int64)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            rate = np.where(att > 0, acc / np.maximum(att, 1), np.nan)
+        return {"temperatures": list(self.temperatures), "rounds": k, "swap_accepts": acc, "swap_attempts": att, "swap_rate": rate}
 
     # -- instrumentation (not in the reference) -------------------------------------------------------
     def kernel_launches(self) -> int:

@@ -32,6 +32,24 @@ def shard_bounds(n_chains: int, rank: int, world_size: int) -> Tuple[int, int]:
     return first, base + (1 if rank < rem else 0)
 
 
+def ladder_shard_error(n_chains: int, world_size: int, K: int):
+    """None when every rank's shard (shard_bounds) starts at a multiple of K and holds a multiple of K chains, so that no ladder of K
+    tempered chains straddles two GPUs (DESIGN.md §2 "Tempered ladders"); otherwise the message options.temperatures raises."""
+    for r in range(int(world_size)):
+        first, count = shard_bounds(n_chains, r, world_size)
+        if first % K or count % K:
+            return ("options.temperatures: with options.distributed every GPU must hold whole ladders; %d chains over %d GPUs give "
+                    "rank %d the chains [%d, %d), which is not a multiple of %d" % (n_chains, world_size, r, first, first + count, K))
+    return None
+
+
+def check_ladder_shards(n_chains: int, K: int) -> None:
+    from .tracer import JsThrow
+    err = ladder_shard_error(n_chains, world()[1], K)
+    if err:
+        raise JsThrow(err)
+
+
 def shard_chains(n_chains: int) -> Tuple[int, int]:
     rank, ws = world()
     return shard_bounds(n_chains, rank, ws)
@@ -164,10 +182,11 @@ def sample_and_gather(sampler, n: int, thin: int, mon: np.ndarray, rows: int) ->
     L = _ffi.lib()
     dev = torch.device("cuda", sampler.device)
     ws, rank = dist.get_world_size(), dist.get_rank()
-    counts = [shard_bounds(sampler.n_chains, r, ws)[1] for r in range(ws)]
+    K = sampler.n_chains // sampler.cold_chains                 # a tempered sampler records the T = 1 chain of every ladder
+    counts = [shard_bounds(sampler.n_chains, r, ws)[1] // K for r in range(ws)]
     mode = getattr(sampler, "gather", "all")
     collect = mode == "all" or mode == "root"
-    out_chains = sampler.n_chains if (mode == "all" or (mode == "root" and rank == 0)) else sampler.local_chains
+    out_chains = sampler.cold_chains if (mode == "all" or (mode == "root" and rank == 0)) else sampler.local_cold
     host = _pinned_empty((rows, len(mon), out_chains))
     host_t = torch.from_numpy(host)
     monp = mon.ctypes.data_as(C.POINTER(C.c_int32))
@@ -178,7 +197,7 @@ def sample_and_gather(sampler, n: int, thin: int, mon: np.ndarray, rows: int) ->
     while row0 < rows:
         r = min(chunk_rows, rows - row0)
         n_chunk = min(n - row0 * thin, r * thin)               # sample(a) then sample(b) == sample(a+b) when a is a multiple of thin
-        local = torch.empty((r, len(mon), sampler.local_chains), dtype=torch.float64, device=dev)
+        local = torch.empty((r, len(mon), sampler.local_cold), dtype=torch.float64, device=dev)
         torch.cuda.current_stream(dev).synchronize()
         rc = L.amwg_sample_device(sampler._handle, n_chunk, thin, monp, len(mon), local.data_ptr())      # blocks until the chunk is in HBM
         if rc != 0:

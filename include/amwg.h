@@ -282,6 +282,21 @@ AMWG_API int amwg_set_adapting(amwg_sampler* s, int32_t flag);
  * prop_log_scale[c][chain], acceptance_count[c][chain] (host; either may be NULL) */
 AMWG_API int amwg_info(amwg_sampler* s, double* scalars, double* prop_log_scale, int32_t* acceptance_count);
 
+/* Tempered ladders (not in the reference; DESIGN.md §2 "Tempered ladders"): parallel tempering over neighbouring chains.
+ * amwg_set_ladder: global chain g becomes rung g mod K of ladder floor(g / K) and targets exp(beta[g mod K] * log_post). beta[r] =
+ *   1 / T_r as the host computed it; beta[0] = 1, strictly decreasing and > 0, 2 <= K <= 256, and the handle's first chain and chain
+ *   count must be multiples of K. Allowed once, after amwg_create and before any sweep, dispersal, set_state or restore; otherwise an
+ *   error is returned and the handle is unchanged. From then on every sweep is followed by swap round k (k = rounds so far): in every
+ *   ladder each rung r = k (mod 2) with r + 1 < K exchanges state, log_post and term cache with rung r + 1 iff
+ *   js_exp((beta[r] - beta[r+1]) * (lp[r+1] - lp[r])) > uniform #(2^63 + 2^62 + k) of rung r's stream. amwg_sample /
+ *   amwg_sample_device record rung 0 only: out is [rows][n_monitor][n_chains / K]. Tempered handles run the interpreter kernels and
+ *   refuse amwg_ppc_pointwise. Their checkpoint images also carry K, beta, the round counter and every ladder's swap counts; a
+ *   restore needs the same ladder on both sides (DESIGN.md §2 "Checkpoints").
+ * amwg_ladder_info: *rounds (when not null) receives the rounds performed; accepts (when not null, K - 1 entries) the accepted swaps
+ *   of each rung pair summed over the handle's ladders. Returns K, or 0 for an untempered handle. */
+AMWG_API int amwg_set_ladder(amwg_sampler* s, const double* beta, int32_t K);
+AMWG_API int amwg_ladder_info(amwg_sampler* s, uint64_t* rounds, int64_t* accepts);
+
 /* instrumentation */
 AMWG_API int64_t amwg_kernel_launches(const amwg_sampler* s);   /* kernels this handle has launched so far       */
 AMWG_API double amwg_last_sweep_kernel_ms(const amwg_sampler* s); /* CUDA-event time of the sweep kernels of the last burn/sample call */

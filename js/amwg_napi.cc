@@ -115,6 +115,7 @@ struct Handle {
   amwg_sampler* s = nullptr;
   int n_comp = 0, n_derived = 0;
   uint64_t n_chains = 0;
+  uint64_t recorded = 0;           // chains a sample row holds: n_chains, or n_chains / K with a tempered ladder (set_ladder)
 };
 void finalize_handle(napi_env, void* data, void*) {
   Handle* h = (Handle*)data;
@@ -250,7 +251,7 @@ BINDING(sample)
   Handle* h = handle_of(env, a.at(0));
   const int64_t n = (int64_t)to_double(env, a.at(1)), thin = (int64_t)to_double(env, a.at(2));
   std::vector<int32_t> mon = ints(env, a.at(3));
-  const size_t rows = (n <= 0 || thin < 1) ? 0 : (size_t)((n + thin - 1) / thin), total = rows * mon.size() * (size_t)h->n_chains;
+  const size_t rows = (n <= 0 || thin < 1) ? 0 : (size_t)((n + thin - 1) / thin), total = rows * mon.size() * (size_t)(h->recorded ? h->recorded : h->n_chains);
   void* data = nullptr;
   napi_value buf, ta;
   check(env, napi_create_arraybuffer(env, total * sizeof(double), &data, &buf), "arraybuffer");
@@ -339,6 +340,28 @@ BINDING(restore)
   uint64_t seed = 0;
   std::memcpy(&seed, images[0] + 32, 8);              // the checked images all carry this seed (DESIGN.md §2 layout)
   return js_number(env, (double)seed);
+END_BINDING
+// set_ladder(handle, betas[])                                                  amwg_set_ladder (options.temperatures)
+BINDING(set_ladder)
+  Handle* h = handle_of(env, a.at(0));
+  std::vector<double> beta = doubles(env, a.at(1));
+  if (amwg_set_ladder(h->s, beta.data(), (int32_t)beta.size()) != 0) fail_from_library();
+  h->recorded = h->n_chains / (uint64_t)beta.size();
+  return js_undefined(env);
+END_BINDING
+// ladder_info(handle) -> {rounds, accepts: Float64Array [K - 1] of accepted swaps}  amwg_ladder_info
+BINDING(ladder_info)
+  Handle* h = handle_of(env, a.at(0));
+  uint64_t rounds = 0;
+  std::vector<int64_t> acc(256, 0);
+  const int K = amwg_ladder_info(h->s, &rounds, acc.data());
+  if (K < 0) fail_from_library();
+  std::vector<double> accepts(acc.begin(), acc.begin() + (K > 1 ? K - 1 : 0));      // exact up to 2^53
+  napi_value o;
+  check(env, napi_create_object(env, &o), "object");
+  napi_set_named_property(env, o, "rounds", js_number(env, (double)rounds));
+  napi_set_named_property(env, o, "accepts", f64_array(env, accepts.data(), accepts.size()));
+  return o;
 END_BINDING
 // set_adapting(handle, flag)                                                    amwg_set_adapting (mcmc.js:1060-1073)
 BINDING(set_adapting)
@@ -688,7 +711,8 @@ NAPI_MODULE_INIT() {
   const struct { const char* name; napi_callback fn; } table[] = {
       {"create", create}, {"destroy", destroy}, {"burn", burn}, {"sample", sample}, {"sample_device", sample_device}, {"get_state", get_state},
       {"get_log_post", get_log_post}, {"set_state", set_state}, {"disperse_state", disperse_state},
-      {"model_fingerprint", model_fingerprint}, {"checkpoint", checkpoint}, {"restore", restore}, {"set_adapting", set_adapting}, {"info", info}, {"kernel_launches", kernel_launches},
+      {"model_fingerprint", model_fingerprint}, {"checkpoint", checkpoint}, {"restore", restore}, {"set_adapting", set_adapting}, {"info", info},
+      {"set_ladder", set_ladder}, {"ladder_info", ladder_info}, {"kernel_launches", kernel_launches},
       {"last_sweep_kernel_ms", last_sweep_kernel_ms}, {"n_chains", n_chains}, {"last_error", last_error}, {"abi_version", abi_version},
       {"ld_eval", ld_eval}, {"primitive_eval", primitive_eval}, {"stream_uniforms", stream_uniforms}, {"device_log", device_log},
       {"summary_moments", summary_moments}, {"summary_digit_hist", summary_digit_hist}, {"summary_autocov", summary_autocov},

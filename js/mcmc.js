@@ -12,7 +12,9 @@
 // New, non-reference options: `chains` (default 1: output shaped exactly like the reference's), `seed`, `device`, `first_chain`,
 // `faithful` (no factorised likelihood plates: bit-faithful sums, slower), `scope` ({name: value} for identifiers log_post uses
 // from an enclosing scope that a recording from source cannot see), `init_radius` (over-dispersed starting points drawn on the
-// device, DESIGN.md §2), `superchain_size` (chains per superchain that start at one point, DESIGN.md §4.6). New methods: `sampler.set_state(values)` places the chains anywhere; `sampler.checkpoint()` and
+// device, DESIGN.md §2), `superchain_size` (chains per superchain that start at one point, DESIGN.md §4.6), `temperatures` (parallel
+// tempering: ladders of K neighbouring chains at T_0 = 1 < ... < T_{K-1} that swap states after every sweep; sample() returns the
+// T = 1 chains, DESIGN.md §2). New methods: `sampler.set_state(values)` places the chains anywhere; `sampler.checkpoint()` and
 // `sampler.restore(images)` stop and resume a run bit for bit.
 (function (root, factory) {
   if (typeof define === "function" && define.amd) { define(["./amwg_trace", "./amwg_native"], factory); }
@@ -177,8 +179,22 @@
   }
 
   // ---------------------------------------------------------------------------------------------- the device model
+  // options.temperatures -> [1 / T_r]; throws unless 2..256 finite, T_0 = 1, strictly increasing, and their number divides n_chains
+  function ladder_betas(temps, n_chains) {
+    var i, out = [];
+    if (!is_array(temps)) { throw "options.temperatures must be a list of numbers"; }
+    for (i = 0; i < temps.length; i++) { if (!is_number(temps[i])) { throw "options.temperatures must be a list of numbers"; } }
+    if (temps.length < 2 || temps.length > 256) { throw "options.temperatures must have between 2 and 256 entries"; }
+    for (i = 0; i < temps.length; i++) { if (!isFinite(temps[i])) { throw "options.temperatures must be finite"; } }
+    if (temps[0] !== 1) { throw "options.temperatures must start at 1"; }
+    for (i = 1; i < temps.length; i++) { if (!(temps[i - 1] < temps[i])) { throw "options.temperatures must be strictly increasing"; } }
+    if (n_chains % temps.length !== 0) { throw "options.temperatures: their number must divide options.chains"; }
+    for (i = 0; i < temps.length; i++) { out.push(1.0 / temps[i]); }
+    return out;
+  }
+
   function DeviceModel(params, names, log_post, data, options, resolved) {
-    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed, radius, size, failed;
+    var i, j, c, name, p, ncomp, off, flat, r, o, n_comp = 0, prog, seed, radius, size, failed, temps;
     this.params = params; this.names = names; this.offsets = {};
     for (i = 0; i < names.length; i++) { this.offsets[names[i]] = n_comp; n_comp += product(params[names[i]].dim); }
     this.n_comp = n_comp;
@@ -196,6 +212,12 @@
       if (this.n_chains % size !== 0) { throw "options.superchain_size must divide options.chains"; }
     }
     this.superchain_size = size;
+    temps = get_option("temperatures", options, null);              // parallel tempering (DESIGN.md §2 "Tempered ladders")
+    this.temperatures = temps;
+    this.betas = temps === null ? null : ladder_betas(temps, this.n_chains);
+    if (this.betas !== null && size !== null) { throw "options.superchain_size cannot be combined with options.temperatures: superchains of tempered chains are not defined"; }
+    if (this.betas !== null && this.first_chain % this.betas.length !== 0) { throw "options.first_chain must be a multiple of the number of temperatures"; }
+    this.n_cold = this.betas === null ? this.n_chains : this.n_chains / this.betas.length;     // the chains sample() returns
     prog =tracer.trace(log_post, names, params, this.offsets, n_comp, data, {faithful: !!get_option("faithful", options, false), scope: get_option("scope", options, null),
                                                                                 base_state: get_option("base_state", options, null)});
     this.program = prog;
@@ -223,6 +245,7 @@
       }
     }
     this.handle = native.create(desc, this.n_chains, this.first_chain, this.seed, this.device);
+    if (this.betas !== null) { native.set_ladder(this.handle, this.betas); }
     if (radius !== null) {
       failed = size === null ? native.disperse_state(this.handle, radius) : native.disperse_state(this.handle, radius, size);
       if (failed > 0) {
@@ -241,8 +264,9 @@
   };
   // raw: flat [rows][n_entries][chains]; -> reference-shaped draws of `name` (entries s..s+ln): [rows] of numbers / nested arrays for one
   // chain, [rows][chains] of the same otherwise
-  DeviceModel.prototype.shape_out = function (name, raw, rows, n_entries, s, ln) {
-    var dim = this.params.hasOwnProperty(name) ? this.params[name].dim : [1], C = this.n_chains, out = [], r, c, e, one, row, scalar = array_equal(dim, [1]);
+  DeviceModel.prototype.shape_out = function (name, raw, rows, n_entries, s, ln, chains) {
+    var dim = this.params.hasOwnProperty(name) ? this.params[name].dim : [1], C = chains === undefined ? this.n_chains : chains, out = [], r, c, e, one, row,
+        scalar = array_equal(dim, [1]);
     for (r = 0; r < rows; r++) {
       row = [];
       for (c = 0; c < C; c++) {
@@ -304,7 +328,7 @@
     for (i = 0; i < monitored.length; i++) {
       e = spans[monitored[i]];
       if (e[1] === 0) { col = []; for (j = 0; j < rows; j++) { col.push(undefined); } out[monitored[i]] = col; }      // JS: state[name] is undefined
-      else { out[monitored[i]] = this.shape_out(monitored[i], raw, rows, entries.length, e[0], e[1]); }
+      else { out[monitored[i]] = this.shape_out(monitored[i], raw, rows, entries.length, e[0], e[1], this.n_cold); }
     }
     return out;
   };
@@ -365,7 +389,7 @@
     thin = Math.abs(Math.floor(this.thinning_interval));
     if (!(thin >= 1)) { throw "sample_raw needs thin >= 1"; }
     rows = n <= 0 ? 0 : Math.ceil(Math.floor(n) / thin);
-    return {data: native.sample(m.handle, Math.floor(n), thin, entries), shape: [rows, entries.length, m.n_chains], entries: labels};
+    return {data: native.sample(m.handle, Math.floor(n), thin, entries), shape: [rows, entries.length, m.n_cold], entries: labels};
   };
   AmwgSampler.prototype.step = function () { this.burn(1); return this.model.state(); };
   AmwgSampler.prototype.state = function () { return this.model.state(); };
@@ -387,7 +411,13 @@
   AmwgSampler.prototype.stop_adaptation = function () { native.set_adapting(this.model.handle, 0); };
   AmwgSampler.prototype.info = function () {
     // the reference returns the thin / monitor METHODS under those keys (mcmc.js:977-980, a bug); the values are returned here
-    return {state: this.model.state(), thin: this.thinning_interval, monitor: this.monitored_params, steppers: [this.model.info()]};
+    var out = {state: this.model.state(), thin: this.thinning_interval, monitor: this.monitored_params, steppers: [this.model.info()]}, m = this.model, K, li, r, k, att = [], rate = [];
+    if (m.betas !== null) {               // options.temperatures: swap rounds, and per rung pair the swaps accepted / attempted over this sampler's ladders
+      K = m.betas.length; li = native.ladder_info(m.handle); k = li.rounds;
+      for (r = 0; r < K - 1; r++) { att.push((m.n_chains / K) * Math.floor((k + 1 - (r % 2)) / 2)); rate.push(att[r] > 0 ? li.accepts[r] / att[r] : NaN); }
+      out.tempering = {temperatures: m.temperatures.slice(), rounds: k, swap_accepts: li.accepts, swap_attempts: att, swap_rate: rate};
+    }
+    return out;
   };
   AmwgSampler.prototype.close = function () { if (this.model && this.model.handle !== null) { native.destroy(this.model.handle); this.model.handle = null; } };
   AmwgSampler.prototype.sweep_kernel = function () { return native.jit_status(this.model.handle); };
